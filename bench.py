@@ -1,19 +1,22 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the DASR SRN hot path on B200 (contract in the task statement).
+"""bench.py — headline benchmark of the DASR SRN hot path on H100.
 
 Workload (BASELINE.json configs[1]): RRDBNet-23 x4 generator forward, batch 16 x 3 x 256 x 256 synthetic LR
-images per GPU (weak scaling), tcgen05 bf16 kernels (fp32 accumulate), random-init weights of the
+images per GPU (weak scaling), wgmma bf16 kernels (fp32 accumulate), random-init weights of the
 reference architecture.  metric = output megapixels / second over all GPUs.
 
   value : device-timed steps, inputs resident in HBM (CUDA events, max over ranks)
   e2e   : the same metric through the public API (SRModel.feed_data -> test -> get result) with PINNED HOST
           input and output buffers, H2D + D2H inside the timed region
-  roofline      : the tcgen05 conv kernel (all conv_tc launches of a step bracketed by CUDA events)
+  roofline      : the wgmma conv kernel (all conv_tc launches of a step bracketed by CUDA events)
   cpu_baseline  : the oracle port of the reference forward on the host cores (bounded sample)
   train         : DASR_Model train step (BASELINE configs[2]: B=32, HR crop 128) iterations / second, fp32 kernels
 
-`--impl reference` times the reference algorithm's CPU path (oracle port: the reference is pure Python and
-/root/reference does not exist on the GPU box) on the host cores with all threads.
+`--impl reference` times the reference algorithm's CPU path (oracle port of the pure-Python reference) on the host
+cores with all threads.
+
+`--dump-outputs DIR` writes what the timed forward returned in its last step (a fixed 2x2-strided sample of the x4 SR
+output, float32, 50 MB) to DIR/sr_output.npy; inputs and weights are deterministic, so two builds can be compared.
 """
 import argparse
 import json
@@ -41,8 +44,8 @@ def peaks():
     p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get('bf16_tflops_sustained', d.get('bf16_tflops', 1400.0)), 'measured (MEASURED_PEAKS.json bf16_tflops_sustained)'
-    return 1400.0, 'fallback (B200_PROFILING.md sustained ~1.4 PFLOP/s)'
+        return d.get('bf16_tflops_sustained', d.get('bf16_tflops', 989.0)), 'measured (MEASURED_PEAKS.json bf16_tflops_sustained)'
+    return 989.0, 'data sheet (H100 SXM dense BF16 at 700 W; not reached on a power-limited card)'
 
 
 class ClockSampler:
@@ -207,9 +210,15 @@ def main():
     ap.add_argument('--steps', type=int, default=10)
     ap.add_argument('--warmup', type=int, default=3)
     ap.add_argument('--impl', default='dasr_b200')
-    ap.add_argument('--train-steps', type=int, default=20)
+    ap.add_argument('--train-steps', type=int, default=None,
+                    help='timed steps of the train-step and DSN legs (default: --steps; 0 skips them); '
+                         'their fp32 parity mode times at most 3 of them')
     ap.add_argument('--no-cpu-baseline', action='store_true')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the last timed step\'s SR output (2x2-strided sample, float32) to DIR/sr_output.npy')
     args = ap.parse_args()
+    if args.train_steps is None:
+        args.train_steps = args.steps
     rank = int(os.environ.get('RANK', 0))
     local_rank = int(os.environ.get('LOCAL_RANK', 0))
     world = int(os.environ.get('WORLD_SIZE', 1))
@@ -279,6 +288,10 @@ def main():
         launches = _lib.LAUNCHES - l0
         ms = max_over_ranks(e0.elapsed_time(e1) / K)
         clocks = sampler.stop() if sampler else None
+        if args.dump_outputs and rank == 0:
+            import numpy as np
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            np.save(os.path.join(args.dump_outputs, 'sr_output.npy'), out[:, :, ::2, ::2].float().cpu().numpy())
         del out
         # roofline: time of the conv_tc launch sequence = step time minus the (few) non-conv kernels of a forward,
         # which are timed here on the same shapes: layout change of the input, zero fill, per-chunk feature copy,
@@ -346,7 +359,7 @@ def main():
         barrier()
         e2e_ms = max_over_ranks(e0.elapsed_time(e1) / K)
         # ---------------------------------------------------------------- same launches with IEEE half operands
-        # (precision 'fp16': tcgen05 kind::f16 with F16 instead of BF16 operands — the mode that meets the 3-decimal
+        # (precision 'fp16': wgmma with F16 instead of BF16 operands — the mode that meets the 3-decimal
         # PSNR / SSIM gate, tests/test_gpu_parity_scale.py); reported beside the bf16 headline, not instead of it
         fp16_ms = None
         if os.environ.get('DASR_BENCH_FP16', '1') != '0' and netG.precision == 'bf16':
@@ -355,11 +368,11 @@ def main():
                 netG(x_dev)
             barrier()
             e0.record()
-            for _ in range(min(K, 10)):
+            for _ in range(K):
                 out = netG(x_dev)
             e1.record()
             barrier()
-            fp16_ms = max_over_ranks(e0.elapsed_time(e1) / min(K, 10))
+            fp16_ms = max_over_ranks(e0.elapsed_time(e1) / K)
             del out
             netG.precision = 'bf16'
     model.fake_H = None
@@ -397,13 +410,6 @@ def main():
     peak, peak_src = peaks()
     flops_step = FLOP_PER_LR_PIXEL * BATCH * LR * LR
     ach = flops_step / (tc_ms * 1e-3) / 1e12
-    traffic, traffic_src = None, None
-    for name in ('r2_traffic.json', 'r1_traffic.json'):
-        tp = os.path.join(ROOT, 'profiles', name)
-        if os.path.exists(tp):
-            traffic = json.load(open(tp)).get('dram_bytes_per_launch_avg')
-            traffic_src = 'static: ncu launch list of this command, profiles/%s (not re-measured in this run)' % name
-            break
     line = {
         'metric': METRIC, 'value': world * out_mp(BATCH, LR) / (ms * 1e-3), 'unit': 'MP/s', 'n_gpus': world, 'steps': K,
         'warmup': W, 'ms_per_step': ms, 'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None, 'dtype': 'bf16',
@@ -411,15 +417,15 @@ def main():
         'config': {'workload': 'RRDBNet-23 x4 inference, batch 16 x 3x256x256 per GPU, forward_chop off (BASELINE configs[1])',
                    'weights': 'random init (deterministic synthetic), reference architecture nb=23 nf=64 gc=32',
                    'parallelism': 'dp%d (independent replicas, no collective on the inference path)' % world,
-                   'l2': 'working set (3 x 537 MB dense-block buffers + 2.1 GB HR activations) >> 126 MB L2: no flush needed'},
+                   'l2': 'working set (3 x 537 MB dense-block buffers + 2.1 GB HR activations) >> 50 MB L2: no flush needed'},
         'e2e': {'value': world * out_mp(BATCH, LR) / (e2e_ms * 1e-3), 'unit': 'MP/s', 'ms_per_step': e2e_ms,
                 'h2d_bytes_per_step': x_host.numel() * 4, 'd2h_bytes_per_step': y_host.numel() * 4,
                 'api': 'SRModel.feed_data(pinned host LR) -> SRModel.test() -> pinned host copy of fake_H (copy stream, double buffered)'},
         'gpu_launches': launches,
         'clocks': clocks,
-        'roofline': {'bound': 'tensor', 'kernel': 'dasr::conv_tc2_kernel / conv_tc_kernel (tcgen05 implicit-GEMM 3x3 conv)',
+        'roofline': {'bound': 'tensor', 'kernel': 'dasr::conv_tc_kernel (wgmma implicit-GEMM 3x3 conv)',
                      'achieved': ach, 'peak': peak, 'unit': 'TFLOP/s', 'frac': ach / peak, 'peak_source': peak_src,
-                     'traffic': traffic, 'traffic_source': traffic_src, 'launches_per_step': n_tc, 'avg_launch_ms': tc_ms / n_tc,
+                     'launches_per_step': n_tc, 'avg_launch_ms': tc_ms / n_tc,
                      'algorithmic_flops_per_step': flops_step, 'non_conv_ms_per_step': non_tc_ms},
     }
     if fp16_ms:
@@ -504,7 +510,7 @@ def bench_train(args, dev, local_rank, world, barrier, max_over_ranks, precision
     ms = max_over_ranks(e0.elapsed_time(e1) / args.train_steps)
     res = {'metric': 'DASR SRN train iterations/sec (G + patch-D + VGG19 perceptual + weighted L1, Adam x2)',
            'value': 1e3 / ms, 'unit': 'it/s', 'ms_per_step': ms, 'steps': args.train_steps,
-           'dtype': 'f32' if precision == 'fp32' else 'bf16 (G and VGG19: tcgen05 fprop+dgrad, G wgrad tcgen05 with fp32 accumulation; D, losses, Adam fp32)',
+           'dtype': 'f32' if precision == 'fp32' else 'bf16 (G and VGG19: wgmma fprop+dgrad, G wgrad wgmma with fp32 accumulation; D, losses, Adam fp32)',
            'config': {'workload': 'BASELINE configs[2]: batch 32 (2B=64 LR 32x32 through G), HR crop 128, fs wavelet, per GPU',
                       'global_batch': 32 * world, 'parallelism': 'dp%d, one flat-bucket NCCL all-reduce of G+D grads per step' % world},
            'gpu_launches_per_step': (_lib.LAUNCHES - l0) // args.train_steps,
@@ -564,7 +570,7 @@ def bench_dsn(args, dev, rank, world, barrier, max_over_ranks, precision='fp32')
     ms = max_over_ranks(e0.elapsed_time(e1) / args.train_steps)
     res = {'metric': 'DSN train iterations/sec (De_resnet + FS discriminator + VGG16 perceptual + LL colour loss, Adam x2)',
            'value': 1e3 / ms, 'unit': 'it/s', 'ms_per_step': ms, 'steps': args.train_steps,
-           'dtype': 'f32' if precision == 'fp32' else 'bf16 (De_resnet trunk and VGG16 on tcgen05, fp32 accumulation; stride-2 tail, discriminator, losses, Adam fp32)',
+           'dtype': 'f32' if precision == 'fp32' else 'bf16 (De_resnet trunk and VGG16 on wgmma, fp32 accumulation; stride-2 tail, discriminator, losses, Adam fp32)',
            'config': {'workload': 'BASELINE configs[4]: batch 8, crop 256 -> 64, wavelet cat, per GPU', 'global_batch': B * world},
            'gpu_launches_per_step': (_lib.LAUNCHES - l0) // args.train_steps}
     del mg, md, gl

@@ -1,4 +1,4 @@
-"""dasr_b200 — B200-native (sm_100a) implementation of the DASR SRN training / inference hot path.
+"""dasr_b200 — H100-native (sm_90a) implementation of the DASR SRN training / inference hot path.
 
 Layout:
   csrc/     hand-written CUDA kernels + the C ABI (include/dasr_b200.h)  -> lib/libdasr_b200.so

@@ -1,4 +1,4 @@
-// BatchNorm2d + LeakyReLU for the BatchNorm variant of the DSN frequency-separation discriminator — sm_100a, fp32 NHWC,
+// BatchNorm2d + LeakyReLU for the BatchNorm variant of the DSN frequency-separation discriminator — sm_90a, fp32 NHWC,
 // HBM-bound (two passes over a tensor of a few MB).
 //
 // Replaces (reference, codes/DSN/model.py:173-190): nn.BatchNorm2d(C) (affine, eps 1e-5, momentum 0.1, running statistics)
@@ -103,7 +103,7 @@ __global__ void bn_lrelu_bwd_kernel(const float* __restrict__ x, const float* __
 
 
 // ---- split form for large tensors (the 64..512-channel layers of the 128x128 / 192x192 BatchNorm discriminators): one block
-// per 32 channels leaves 140 SMs idle (measured 1.1 ms for 16 MB).  Three launches instead: per-(split, channel) partial sums
+// per 32 channels leaves most SMs idle.  Three launches instead: per-(split, channel) partial sums
 // in double, a per-channel finalize in fixed order (deterministic), an elementwise apply.  The partial sums live in the
 // OUTPUT buffer (y / dx), which the apply pass overwrites afterwards: no workspace argument, nothing allocated.
 __global__ void bn_partial_fwd_kernel(const float* __restrict__ x, double* __restrict__ part, long M, int C, long rows_per_split) {
@@ -224,7 +224,7 @@ __global__ void bn_stats_eval_kernel(const float* __restrict__ running_mean, con
 // number of pixel splits of the large-tensor form (0 = use the one-block-per-32-channels kernel)
 static int bn_splits(long M, int C) {
   if (M < 4096) return 0;
-  long s = (2L * 148 + cdiv(C, 32) - 1) / cdiv(C, 32);
+  long s = (2L * num_sms() + cdiv(C, 32) - 1) / cdiv(C, 32);
   if (s > M / 256) s = M / 256;
   if (s > 256) s = 256;
   return s < 2 ? 0 : (int)s;
@@ -246,7 +246,7 @@ int dasr_bn_lrelu_fwd(const float* x, float* y, const float* gamma, const float*
   if (S > 0 && !training) {      // eval: statistics are given, only the elementwise pass is large
     bn_stats_eval_kernel<<<cdiv(C, 128), 128, 0, st>>>(running_mean, running_var, stats, C, eps);
     const long total = M * C;
-    bn_apply_fwd_kernel<<<(unsigned)min((long)148 * 8, (total + 255) / 256), 256, 0, st>>>(x, y, gamma, beta, stats, total, C, slope);
+    bn_apply_fwd_kernel<<<(unsigned)min((long)num_sms() * 8, (total + 255) / 256), 256, 0, st>>>(x, y, gamma, beta, stats, total, C, slope);
     return check_launch("bn_lrelu_fwd");
   }
   if (S > 0 && (reinterpret_cast<uintptr_t>(y) & 7) == 0 && x != y) {
@@ -255,7 +255,7 @@ int dasr_bn_lrelu_fwd(const float* x, float* y, const float* gamma, const float*
     bn_partial_fwd_kernel<<<dim3(cdiv(C, 32), S), block, 0, st>>>(x, part, M, C, rps);
     bn_finalize_fwd_kernel<<<cdiv(C, 128), 128, 0, st>>>(part, S, running_mean, running_var, stats, M, C, eps, momentum);
     const long total = M * C;
-    bn_apply_fwd_kernel<<<(unsigned)min((long)148 * 8, (total + 255) / 256), 256, 0, st>>>(x, y, gamma, beta, stats, total, C, slope);
+    bn_apply_fwd_kernel<<<(unsigned)min((long)num_sms() * 8, (total + 255) / 256), 256, 0, st>>>(x, y, gamma, beta, stats, total, C, slope);
     return check_launch("bn_lrelu_fwd");
   }
   bn_lrelu_fwd_kernel<<<grid, block, 0, st>>>(x, y, gamma, beta, running_mean, running_var, stats, M, C, eps,
@@ -275,7 +275,7 @@ int dasr_bn_lrelu_bwd(const float* x, const float* y, const float* dy, const flo
     bn_partial_bwd_kernel<<<dim3(cdiv(C, 32), S), block, 0, st>>>(x, y, dy, stats, part, M, C, rps, slope);
     bn_finalize_bwd_kernel<<<cdiv(C, 128), 128, 0, st>>>(part, S, dgamma, dbeta, C);
     const long total = M * C;
-    bn_apply_bwd_kernel<<<(unsigned)min((long)148 * 8, (total + 255) / 256), 256, 0, st>>>(x, y, dy, gamma, stats, dgamma, dbeta, dx,
+    bn_apply_bwd_kernel<<<(unsigned)min((long)num_sms() * 8, (total + 255) / 256), 256, 0, st>>>(x, y, dy, gamma, stats, dgamma, dbeta, dx,
                                                                                            total, M, C, training, slope);
     return check_launch("bn_lrelu_bwd");
   }

@@ -1,7 +1,7 @@
 // Generic fp32 implicit-GEMM convolution on CUDA cores: forward / transposed-gather (dgrad) and
 // filter gradient.  This is the exact-arithmetic mode of the path (fp32 FMA, fp32 storage) used for
 // the 1e-3 rel-Linf parity gate and for the odd-shaped layers (Cin=3/9, 4x4 stride-2 discriminator
-// convs, Cout=1/3) that do not map onto tcgen05 tiles.
+// convs, Cout=1/3) that do not map onto the tensor-core tiles.
 //
 // Reference call sites replaced: nn.Conv2d in block.py:142-143 (conv_block), architecture.py:998-1018
 // (NLayerDiscriminator), architecture.py:1076 (VGG19 features); autograd's conv backward for them.
@@ -25,7 +25,7 @@ int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;   // H100 SXM
   }
   return n;
 }
@@ -71,9 +71,9 @@ constexpr int KSUB = BK / 16;
 // Arithmetic of the 64x64x16 tile product (DasrConvF32Params.math, DASR_F32_MATH_*):
 //   FMA    : fp32 FMA on CUDA cores, 4x4 outputs per thread                      (exact mode, default)
 //   TF32   : mma.sync m16n8k8 tf32, fp32 accumulate (10-bit significand operands) (mixed-precision training: the fp32 side
-//            nets — discriminators, stride-2 / 5x5 layers — whose shapes do not fit the tcgen05 tiles)
+//            nets — discriminators, stride-2 / 5x5 layers — whose shapes do not fit the tensor-core tiles)
 //   TF32X3 : a = hi + lo, b = hi + lo in tf32; lo*hi + hi*lo + hi*hi              (fp32-level error on tensor cores)
-// The odd shapes of these layers (Cin 3/9, 4x4 stride 2, 5x5, Cout 1) rule out the tcgen05 halo-tile kernel; warp-level
+// The odd shapes of these layers (Cin 3/9, 4x4 stride 2, 5x5, Cout 1) rule out the wgmma halo-tile kernel; warp-level
 // MMA on the gathered tile keeps the generic gather and still leaves the FMA pipe.
 constexpr int MATH_FMA = 1, MATH_TF32 = 2, MATH_TF32X3 = 3;
 template <int MATH> struct Pad {       // row strides of the two shared-memory tiles: conflict-free for each access pattern
@@ -274,7 +274,7 @@ __global__ void __launch_bounds__(256) conv2d_f32_kernel(const float* __restrict
 // ---------------------------------------------------------------------------------------------
 // Thin-N form (cout <= 16, long K): the logit layers of the discriminators (512 -> 1 with 4x4 taps, 256 -> 1) and the input
 // gradient of their first layers (N = 3 / 9).  The 64-wide output tile of the implicit-GEMM kernel would be 84-98 % empty and
-// the grid tiny (18 CTAs walking K = 8192: 0.64 ms for 9 MFLOP under ncu).  Here ONE WARP owns an output pixel: the lanes stride
+// the grid tiny (18 CTAs walking K = 8192).  Here ONE WARP owns an output pixel: the lanes stride
 // over the input channels of every tap (coalesced float4 loads), keep `cout` running sums each, and reduce them with shuffles in a
 // fixed order (deterministic).  Same operands, same epilogue contract as conv2d_f32_kernel; exact fp32 FMA arithmetic.
 // ---------------------------------------------------------------------------------------------
@@ -696,7 +696,7 @@ static int wgrad_splits(const DasrConvF32Params* p) {
   long P = (long)p->N * p->OH * p->OW;
   int K = p->kh * p->kw * p->cin;
   int tiles = cdiv(K, BM) * cdiv(p->cout, BN);
-  int want = cdiv(2 * 148, tiles);
+  int want = cdiv(2 * num_sms(), tiles);
   long maxs = (P + 255) / 256;
   int s = (int)(want < maxs ? want : maxs);
   if (s < 1) s = 1;

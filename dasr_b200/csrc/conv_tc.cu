@@ -1,4 +1,4 @@
-// tcgen05 implicit-GEMM 3x3 convolution for sm_100a — the RRDB hot kernel.
+// wgmma implicit-GEMM 3x3 convolution for sm_90a — the RRDB hot kernel.
 //
 // Replaces (reference, codes/SRN): ResidualDenseBlock_5C.conv1..5 + torch.cat + x5*0.2+x
 // (models/modules/block.py:262-286), RRDB / ShortcutBlock residuals (block.py:305-309, 103-105),
@@ -9,33 +9,34 @@
 // (tap, 32-channel chunk).  One tile = 16 rows x 8 cols of output pixels.
 //   * A: ONE TMA load per 32-channel chunk brings the (16+2)x(8+2) halo tile (zero fill outside the
 //     image) into shared memory as 180 rows x 64 B, 64B-swizzled.  Each of the 9 taps is then just a
-//     different UMMA shared-memory descriptor on that same tile: start address shifted by
+//     different wgmma shared-memory descriptor on that same tile: start address shifted by
 //     (dy*10+dx) rows, 8-row groups (= one image row of the tile) 10 rows apart (SBO = 640 B).
 //     Activations cross L2->SMEM once per chunk instead of once per tap (9x less than im2col/TMA-im2col).
 //   * B: the whole filter set of this CTA's Cout tile stays resident in shared memory for the
 //     lifetime of the persistent CTA ([tap][chunk][nt rows x 64 B], 64B-swizzled).
-//   * D: fp32 accumulators in TMEM, double buffered so the epilogue of tile i overlaps the MMAs of
-//     tile i+1.
-// Warp roles (320 threads): warp 0 = TMA producer, warp 1 = TMEM allocator + elected-lane MMA issuer,
-// warps 2..9 = epilogue (TMEM -> registers -> bias/pre/act/scale/residuals -> bf16 tile in swizzled shared
-// memory -> TMA store; pre-activation addend and residual tiles arrive by TMA as well).
+//   * D: fp32 accumulators in registers: two consumer warpgroups, each owning 64 pixels (8 image rows) of the tile,
+//     issue m64nNk16 wgmmas and then run the epilogue on their own accumulators.
+// Warp roles (320 threads): warps 0..7 = the two consumer warpgroups (wgmma + epilogue: registers ->
+// bias/pre/act/scale/residuals -> bf16 tile in swizzled shared memory), warp 8 = TMA producer (A halo tiles, resident
+// filters), warp 9 = epilogue TMA (pre-activation addend and residual tiles in, finished tiles out).
+//
+// Cluster pair (dasr_conv_tc2): two CTAs of a (1, 2, 1) cluster take the two Cout halves of the SAME pixel tiles; each
+// keeps only its half of the filters resident, and the leader's TMA multicasts every A halo tile into both CTAs, so an
+// activation tile crosses L2 -> SMEM once for the pair.  That is what lets a 192-wide filter set (221 KB) run as one tile.
 #include <stdlib.h>
 #include "tc_common.cuh"
 
 namespace dasr {
 
-// conv_tc_kernel runs EPI_WGS epilogue warpgroups (4 warps each, one per TMEM lane quarter) and MMA_WARPS issuer warps.
-// Measured on B200 (selftest fused, K=32 N=64 tile: 1.22-1.31 us against 0.72 us of MMA time): 4 warpgroups instead of 2,
-// 2 issuer warps instead of 1, 4 TMEM accumulators instead of 2, alternate-tile epilogues and 4 staging buffers all
-// leave the tile time unchanged, so the defaults stay at the smallest configuration.
-constexpr int EPI_WGS = 2;
-constexpr int EPI_WARPS = 4 * EPI_WGS;
-constexpr int MMA_WARPS = 1;                         // 2: two issuer warps take alternate tiles
-constexpr int TCK_WARPS = 2 + EPI_WARPS + 1 + (MMA_WARPS - 1);   // producer, MMA issuer 0, epilogue warps, epilogue-TMA warp, MMA issuer 1
-constexpr int TCK_THREADS = 32 * TCK_WARPS;
+constexpr int CONS_WARPS = 8;                        // two consumer warpgroups
+constexpr int PROD_WARP = CONS_WARPS;                // A / filter TMA producer
+constexpr int EPI_TMA_WARP = CONS_WARPS + 1;         // staged-epilogue TMA
+constexpr int TCK_THREADS = 32 * (CONS_WARPS + 2);
+constexpr int ACC_REGS = 128;                        // nt <= 256: a warpgroup's 64 x nt fp32 accumulators per thread
+constexpr int A_STAGE_ROWS = 192;                    // halo tile rows reserved per stage: the taps-in-N path reads 3 x 64
 
-struct EpiMaps {          // TMA descriptors of the staged epilogue: [out, pre, res1, res2] x [64-channel box, 32-channel box]
-  CUtensorMap m[8];
+struct EpiMaps {          // TMA descriptors of the staged epilogue: [out, pre, res1, res2] x [64-, 32-, 16-channel box]
+  CUtensorMap m[12];
 };
 
 struct TcKernelArgs {
@@ -54,23 +55,82 @@ struct TcKernelArgs {
   int stages;
   int w_bytes;       // resident filter bytes of one CTA
   int a_stage_bytes; // bytes of one A stage
-  int tmem_cols;     // allocated TMEM columns (nacc accumulators of acc_stride columns)
-  int nacc;          // TMEM accumulator buffers (2 or 4): MMAs of tile i+nacc wait for the epilogue reads of tile i
-  int acc_stride;
   int epi_bytes;     // bytes of ONE staged epilogue tile: 128 pixels x nt channels bf16
   int has_pre, has_res1, has_res2;
   int nbuf;          // staged-epilogue tile buffers (2..4): pre / residual tiles are requested nbuf tiles ahead
+  int pair;          // 1: launched as (1, 2, 1) clusters, A tiles multicast by the leader (rank 0)
 };
 
+__device__ __forceinline__ float2 h16x2_to_f2(uint32_t u, int f16) {
+  if (f16) return __half22float2(*reinterpret_cast<const __half2*>(&u));
+  return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u));
+}
+__device__ __forceinline__ uint32_t f2_to_h16x2(float a, float b, int f16) {
+  uint32_t u;
+  if (f16) *reinterpret_cast<__half2*>(&u) = __floats2half2_rn(a, b);
+  else *reinterpret_cast<__nv_bfloat162*>(&u) = __floats2bfloat162_rn(a, b);
+  return u;
+}
+__device__ __forceinline__ uint32_t lds32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr));
+  return v;
+}
+__device__ __forceinline__ void sts32(uint32_t addr, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
 
-// EPI_MODE / HAS_PRE / NRES are compile-time so that each instantiation carries only its own epilogue code
-// (the all-in-one kernel spread the per-group loop over ~32 KB of SASS and stalled on instruction fetch).
+// Staged tile layout: nb64 blocks of 64 channels (128 B rows, SWIZZLE_128B), then a 32-channel block (64 B rows,
+// SWIZZLE_64B) if nt & 32, then a 16-channel block (32 B rows, SWIZZLE_32B) if nt & 16.  Byte offset of (pixel m, channel c).
+__device__ __forceinline__ uint32_t staged_off(int m, int c, int nb64, bool tail32) {
+  int base, ch, sw;
+  if (c < (nb64 << 6)) {
+    base = (c >> 6) * EPI_BLK64_BYTES + m * 128; ch = (c & 63) >> 3; sw = m & 7;
+  } else if (tail32 && c < (nb64 << 6) + 32) {
+    base = nb64 * EPI_BLK64_BYTES + m * 64; ch = (c & 31) >> 3; sw = (m >> 1) & 3;
+  } else {
+    base = nb64 * EPI_BLK64_BYTES + (tail32 ? EPI_BLK32_BYTES : 0) + m * 32; ch = (c & 15) >> 3; sw = (m >> 2) & 1;
+  }
+  return (uint32_t)(base + ((ch ^ sw) << 4) + (c & 7) * 2);
+}
+
+// block i of a staged tile: channel offset, byte offset, map column (0: 64, 1: 32, 2: 16 channels)
+__device__ __forceinline__ void staged_block(int i, int nb64, bool tail32, int& col, int& off, int& kind) {
+  if (i < nb64) { col = i * 64; off = i * EPI_BLK64_BYTES; kind = 0; }
+  else if (tail32 && i == nb64) { col = nb64 * 64; off = nb64 * EPI_BLK64_BYTES; kind = 1; }
+  else { col = nb64 * 64 + (tail32 ? 32 : 0); off = nb64 * EPI_BLK64_BYTES + (tail32 ? EPI_BLK32_BYTES : 0); kind = 2; }
+}
+
+// one tap of one A load: ksteps K = 16 wgmmas of N = nt
+template <int N, int F16>
+__device__ __forceinline__ void issue_tap(float* acc, uint32_t a_addr, uint64_t a_hi, uint32_t b_addr, uint32_t b_slot,
+                                          uint64_t b_hi, int ksteps, int first) {
+#pragma unroll
+  for (int ks = 0; ks < 4; ks++) {
+    if (ks < ksteps)
+      wgmma<N, F16, 0>(acc, make_desc(a_addr + 32u * ks, a_hi), make_desc(b_addr + (uint32_t)(ks >> 1) * b_slot + 32u * (ks & 1), b_hi),
+                       (first && ks == 0) ? 0 : 1);
+  }
+}
+
+template <int F16>
+__device__ __forceinline__ void issue_tap_rt(int nt, float* acc, uint32_t a_addr, uint64_t a_hi, uint32_t b_addr, uint32_t b_slot,
+                                             uint64_t b_hi, int ksteps, int first) {
+  switch (nt) {
+#define DASR_TAP_CASE(n) case n: issue_tap<n, F16>(acc, a_addr, a_hi, b_addr, b_slot, b_hi, ksteps, first); break;
+    DASR_TAP_CASE(16) DASR_TAP_CASE(32) DASR_TAP_CASE(48) DASR_TAP_CASE(64) DASR_TAP_CASE(80) DASR_TAP_CASE(96)
+    DASR_TAP_CASE(112) DASR_TAP_CASE(128) DASR_TAP_CASE(144) DASR_TAP_CASE(160) DASR_TAP_CASE(176) DASR_TAP_CASE(192)
+    DASR_TAP_CASE(208) DASR_TAP_CASE(224) DASR_TAP_CASE(240) DASR_TAP_CASE(256)
+#undef DASR_TAP_CASE
+    default: break;
+  }
+}
+
+// EPI_MODE / HAS_PRE / NRES are compile-time so that each instantiation carries only its own epilogue code.
 template <int EPI_MODE, bool HAS_PRE, int NRES>
 __global__ void __launch_bounds__(TCK_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ CUtensorMap tmap_w,
                const __grid_constant__ EpiMaps em, const TcKernelArgs a) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // carve: [W resident][A stages][staged tiles x2: out/pre][res1 x2][res2 x2][barriers, bias]
+  // carve: [W resident][A stages][staged tiles: out/pre][res1][res2][barriers, tap offsets, bias]
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sW = smem;
   uint8_t* sA = smem + a.w_bytes;
@@ -80,15 +140,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
   uint8_t* sR2 = sR1 + (NRES >= 1 ? nbuf * a.epi_bytes : 0);     // [nbuf]
   uint64_t* bars = reinterpret_cast<uint64_t*>(sR2 + (NRES >= 2 ? nbuf * a.epi_bytes : 0));
   uint64_t* full_bar = bars;                     // [stages]  A chunk landed
-  uint64_t* empty_bar = bars + MAX_STAGES;       // [stages]  A chunk consumed
+  uint64_t* empty_bar = bars + MAX_STAGES;       // [stages]  A chunk consumed (leader of a pair: by both CTAs)
   uint64_t* w_bar = bars + 2 * MAX_STAGES;       // [1]       resident filters landed
-  uint64_t* tfull_bar = bars + 2 * MAX_STAGES + 1;    // [4]  accumulator complete
-  uint64_t* tempty_bar = bars + 2 * MAX_STAGES + 5;   // [4]  accumulator drained
-  uint64_t* pre_bar = bars + 2 * MAX_STAGES + 9;      // [4]  pre / residual tiles landed in staging buffer b
-  uint64_t* sfull_bar = bars + 2 * MAX_STAGES + 13;   // [4]  staging buffer b holds a finished tile
-  uint64_t* sfree_bar = bars + 2 * MAX_STAGES + 17;   // [4]  staging buffer b has been read by its TMA stores
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * MAX_STAGES + 21);
-  float* sBias = reinterpret_cast<float*>(bars + 2 * MAX_STAGES + 22);   // [nt] (16-byte aligned)
+  uint64_t* pre_bar = w_bar + 1;                 // [4]       pre / residual tiles landed in staging buffer b
+  uint64_t* sfull_bar = pre_bar + 4;             // [4]       staging buffer b holds a finished tile
+  uint64_t* sfree_bar = sfull_bar + 4;           // [4]       staging buffer b has been read by its TMA stores
+  uint32_t* sTap = reinterpret_cast<uint32_t*>(bars + 2 * MAX_STAGES + 16);   // [9] A byte offset of each tap
+  float* sBias = reinterpret_cast<float*>(bars + 2 * MAX_STAGES + 24);        // [nt] (16-byte aligned)
 
   const DasrConvTcParams& p = a.p;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -96,40 +154,49 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
   const int ntile = blockIdx.y - var * a.n_ntiles;
   const int nt = p.nt;
   const int ntaps = p.ntaps;
-  const int acc_stride = a.acc_stride;
-  const uint32_t nacc = (uint32_t)a.nacc;
-  const int nb64 = nt >> 6;                      // staged tile = nb64 blocks of 64 channels + (nt & 32) tail block
-  const bool tail32 = (nt & 32) != 0;
+  const int nb64 = nt >> 6;
+  const bool tail32 = (nt & 32) != 0, tail16 = (nt & 16) != 0;
+  const int nblocks = nb64 + (tail32 ? 1 : 0) + (tail16 ? 1 : 0);
   const bool has_loads = (EPI_MODE == 0) && (HAS_PRE || NRES > 0);
+  const bool pair = a.pair != 0;
+  const uint32_t rank = pair ? cluster_ctarank() : 0u;
+  const uint32_t a_row = a.chunk64 ? 2u * ROW_B : (uint32_t)ROW_B;    // bytes per pixel row of an A tile
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_in);
     tma_prefetch_desc(&tmap_w);
     for (int s = 0; s < a.stages; s++) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], CONS_WARPS * ((pair && rank == 0) ? 2 : 1));   // one arrive per consumer warp (of both CTAs)
     }
     mbar_init(w_bar, 1);
     for (int b = 0; b < 4; b++) {
-      mbar_init(&tfull_bar[b], 1);
-      mbar_init(&tempty_bar[b], EPI_WARPS);  // one arrive per epilogue warp that reads this accumulator
-    }
-    for (int b = 0; b < 4; b++) {
       mbar_init(&pre_bar[b], 1);
-      mbar_init(&sfull_bar[b], EPI_WARPS);
+      mbar_init(&sfull_bar[b], CONS_WARPS);
       mbar_init(&sfree_bar[b], 1);
     }
     fence_barrier_init();
+    for (int t = 0; t < 9; t++) {
+      const int tt = t < ntaps ? t : 0;
+      sTap[t] = (p.a_mode == 0) ? (uint32_t)(p.tap_dy[var][tt] * HALO_W + p.tap_dx[var][tt]) * a_row : (uint32_t)(tt * A_TAP_BYTES);
+    }
   }
-  if (warp == 1) tmem_alloc(tmem_ptr, (uint32_t)a.tmem_cols);
   for (int i = threadIdx.x; i < nt; i += TCK_THREADS) sBias[i] = a.bias ? a.bias[ntile * nt + i] : 0.f;
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
+  if (pair) cluster_sync();              // both CTAs' barriers initialised before any multicast or remote arrive
   pdl_launch_dependents();               // the next launch may start its prologue on SMs this grid has left
 
-  if (warp == 0) {
+  auto tile_xyz = [&](long tile, int& x0, int& y0, int& n) {
+    const uint32_t te = (uint32_t)(p.tile_rev ? a.ntiles - 1 - tile : tile);   // 32-bit tile arithmetic (checked on the host)
+    const uint32_t r = te / (uint32_t)a.tiles_x;
+    const int tx = (int)(te - r * (uint32_t)a.tiles_x);
+    n = (int)(r / (uint32_t)a.tiles_y);
+    const int ty = (int)(r - (uint32_t)n * (uint32_t)a.tiles_y);
+    x0 = tx * TILE_W;
+    y0 = ty * TILE_H;
+  };
+
+  if (warp == PROD_WARP) {
     // =========================== TMA producer (A halo tiles, resident filters) ===========================
     if (lane == 0) {
       // resident filters: rows [(var*ntaps + tap)*nchunks + c]*cout + ntile*nt .. +nt of the packed filter
@@ -140,30 +207,21 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
           int row = ((var * ntaps + tap) * a.nchunks + c) * p.cout + ntile * nt;
           tma_load_2d(sW + (size_t)slot * nt * ROW_B, &tmap_w, w_bar, 0, row);
         }
-    }
-    int stage = 0;
-    uint32_t phase = 0;
-    if (lane == 0) pdl_wait();           // activations come from the previous launch (filters / bias above do not)
-    __syncwarp();
-    for (long tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x) {
-      const uint32_t te = (uint32_t)(p.tile_rev ? a.ntiles - 1 - tile : tile);   // 32-bit tile arithmetic (checked on the host)
-      const uint32_t r = te / (uint32_t)a.tiles_x;
-      const int tx = (int)(te - r * (uint32_t)a.tiles_x);
-      const int n = (int)(r / (uint32_t)a.tiles_y);
-      const int ty = (int)(r - (uint32_t)n * (uint32_t)a.tiles_y);
-      int x0 = tx * TILE_W, y0 = ty * TILE_H;
-      if (lane == 0) {
+      pdl_wait();                        // activations come from the previous launch (filters / bias above do not)
+      int stage = 0;
+      uint32_t phase = 0;
+      for (long tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x) {
+        int x0, y0, n;
+        tile_xyz(tile, x0, y0, n);
         for (int c = 0; c < a.nloads; c++) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* dst = sA + (size_t)stage * a.a_stage_bytes;
-          if (a.chunk64) {
-            // 64 channels per load: the TMA engine is request-bound at ~4 cycles per row (measured: 15.5 B/clk/SM with 64 B
-            // rows, 31-34 with 128 B rows), and a K = 64 tile with few MMAs (sub-pixel upconv, last layer) waits for it
-            mbar_expect_tx(&full_bar[stage], 2 * A_HALO_BYTES);
-            tma_load_4d(dst, &tmap_in, &full_bar[stage], p.in_coff + c * 2 * CHUNK, x0 - 1, y0 - 1, n);
-          } else if (p.a_mode == 0) {
-            mbar_expect_tx(&full_bar[stage], A_HALO_BYTES);
-            tma_load_4d(dst, &tmap_in, &full_bar[stage], p.nchunk_list ? p.chunk_off[c] : p.in_coff + c * CHUNK, x0 - 1, y0 - 1, n);
+          if (p.a_mode == 0) {
+            // 64 channels per load when the slice allows it: half the TMA requests per byte
+            const int ch = a.chunk64 ? p.in_coff + c * 2 * CHUNK : (p.nchunk_list ? p.chunk_off[c] : p.in_coff + c * CHUNK);
+            mbar_expect_tx(&full_bar[stage], (uint32_t)((a.chunk64 ? 2 : 1) * A_HALO_BYTES));
+            if (!pair) tma_load_4d(dst, &tmap_in, &full_bar[stage], ch, x0 - 1, y0 - 1, n);
+            else if (rank == 0) tma_load_4d_mc(dst, &tmap_in, &full_bar[stage], ch, x0 - 1, y0 - 1, n, (uint16_t)3);
           } else {
             mbar_expect_tx(&full_bar[stage], (uint32_t)(ntaps * A_TAP_BYTES));
             for (int tap = 0; tap < ntaps; tap++)
@@ -173,120 +231,28 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
           if (++stage == a.stages) { stage = 0; phase ^= 1; }
         }
       }
-      __syncwarp();
     }
-  } else if (warp == 1 || (MMA_WARPS > 1 && warp == TCK_WARPS - 1)) {
-    // =========================== MMA issuers (alternate tiles) ===========================
-    const uint32_t mi = (warp == 1) ? 0u : 1u;
-    // The whole warp walks the (warp-uniform) pipeline; one elected lane issues the tcgen05.mma
-    // instructions, so descriptors live in uniform registers and no per-lane serialisation is emitted.
-    const uint32_t idesc = make_idesc_16(128, nt, p.f16);
-    // EPI_MODE 3 ("taps in N", last layer): the halo tile is read as a PLAIN 180-row K-major tile (8-row groups 512 B apart)
-    const uint32_t a_row = a.chunk64 ? 2u * ROW_B : (uint32_t)ROW_B;          // bytes per pixel row of an A tile
-    const uint32_t a_sbo = (p.a_mode == 0 && EPI_MODE != 3) ? (uint32_t)HALO_W * a_row : 8u * a_row;
-    // layout type: SWIZZLE_64B (4) for 64 B rows, SWIZZLE_128B (2) for the 64-channel chunks
-    const uint64_t a_hi = ((uint64_t)((a_sbo >> 4) & 0x3FFF) << 32) | ((uint64_t)1 << 46) | ((uint64_t)(a.chunk64 ? 2 : 4) << 61) | ((uint64_t)1 << 16);
-    const int ksteps = a.chunk64 ? 4 : 2;                                      // K = 16 steps per A load
-    const uint64_t b_hi = ((uint64_t)(((8 * ROW_B) >> 4) & 0x3FFF) << 32) | ((uint64_t)1 << 46) | ((uint64_t)4 << 61) | ((uint64_t)1 << 16);
-    const uint32_t a_lo0 = smem_u32(sA) >> 4;
-    const uint32_t a_stage_lo = (uint32_t)a.a_stage_bytes >> 4;
-    const uint32_t b_lo0 = smem_u32(sW) >> 4;
-    const uint32_t b_slot_lo = (uint32_t)(nt * ROW_B) >> 4;
-    uint32_t tap_lo[9];
-#pragma unroll
-    for (int t = 0; t < 9; t++) {
-      int tt = t < ntaps ? t : 0;
-      tap_lo[t] = (p.a_mode == 0) ? ((uint32_t)(p.tap_dy[var][tt] * HALO_W + p.tap_dx[var][tt]) * a_row) >> 4
-                                  : (uint32_t)(tt * A_TAP_BYTES) >> 4;
-    }
-    mbar_wait(w_bar, 0);
-    tc_fence_after();
-    int stage = 0;
-    uint32_t phase = 0;
-    uint32_t it = 0;
-    for (long tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x, it++) {
-      if ((it % MMA_WARPS) != mi) {          // the other issuer's tile: only walk the ring position past it
-        for (int c = 0; c < a.nloads; c++)
-          if (++stage == a.stages) { stage = 0; phase ^= 1; }
-        continue;
-      }
-      const int acc = (int)(it % nacc);
-      const uint32_t acc_phase = (it / nacc) & 1;
-      mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + (uint32_t)(acc * acc_stride);
-      for (int c = 0; c < a.nloads; c++) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t a_lo = a_lo0 + (uint32_t)stage * a_stage_lo;
-          const uint32_t b_tap_step = (uint32_t)a.nchunks * b_slot_lo;
-          // K step ks of this load reads 32 B at offset 32 * ks of every A row and the 32-channel filter chunk
-          // cb + (ks >> 1) at offset 32 * (ks & 1) of its rows
-          const uint32_t cb = a.chunk64 ? 2u * (uint32_t)c : (uint32_t)c;
-          if constexpr (EPI_MODE == 3) {
-            // D'[halo pixel][tap * out_nc + c] = A[halo pixel][K] * B'[K][tap * out_nc + c]: every halo pixel against the
-            // filters of ALL taps at once — 2 M-halves (halo rows 0..127, 128..255; rows >= 180 are never read) x K steps
-            // instead of 9 taps x K steps; the epilogue adds the nine shifted partial results.
-#pragma unroll
-            for (int mh = 0; mh < 2; mh++) {
-              const uint32_t al = a_lo + (uint32_t)mh * ((128u * a_row) >> 4);
-              for (int ks = 0; ks < ksteps; ks++) {
-                const uint32_t bl = b_lo0 + (cb + (uint32_t)(ks >> 1)) * b_slot_lo + 2u * (uint32_t)(ks & 1);
-                umma_bf16(d_tmem + (uint32_t)mh * 32u, a_hi | (uint64_t)((al + 2u * ks) & 0x3FFF), b_hi | (uint64_t)(bl & 0x3FFF), idesc,
-                          (uint32_t)((c | ks) != 0));
-              }
-            }
-          } else {
-#pragma unroll
-            for (int tap = 0; tap < 9; tap++) {
-              if (tap < ntaps) {
-                const uint32_t al = a_lo + tap_lo[tap];
-                for (int ks = 0; ks < ksteps; ks++) {
-                  const uint32_t bl = b_lo0 + (cb + (uint32_t)(ks >> 1)) * b_slot_lo + (uint32_t)tap * b_tap_step + 2u * (uint32_t)(ks & 1);
-                  umma_bf16(d_tmem, a_hi | (uint64_t)((al + 2u * ks) & 0x3FFF), b_hi | (uint64_t)(bl & 0x3FFF), idesc,
-                            (uint32_t)((c | tap | ks) != 0));
-                }
-              }
-            }
-          }
-          umma_commit(&empty_bar[stage]);  // smem slot reusable once these MMAs retire
-          if (c == a.nloads - 1) umma_commit(&tfull_bar[acc]);  // accumulator complete -> epilogue
-        }
-        __syncwarp();
-        if (++stage == a.stages) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == TCK_WARPS - MMA_WARPS) {
+    __syncwarp();
+  } else if (warp == EPI_TMA_WARP) {
     // =========================== epilogue TMA warp ===========================
     // Feeds the staged epilogue: pre-activation / residual tiles in (nbuf tiles ahead), finished tiles out.
     if constexpr (EPI_MODE == 0) {
       const int co_base = p.out_coff + ntile * nt;
-      const int omap = (p.out_mul == 2) ? 2 * var : 0;      // sub-pixel variants: one strided output map pair per parity
+      const int omap = (p.out_mul == 2) ? 3 * var : 0;      // sub-pixel variants: one strided output map triple per parity
       const uint32_t load_bytes = (uint32_t)(((HAS_PRE ? 1 : 0) + NRES) * a.epi_bytes);
       pdl_wait();                      // pre / residual tiles and the output slots belong to earlier launches until now
-      auto tile_xyz = [&](long tile, int& x0, int& y0, int& n) {
-        const uint32_t te = (uint32_t)(p.tile_rev ? a.ntiles - 1 - tile : tile);
-        const uint32_t r = te / (uint32_t)a.tiles_x;
-        const int tx = (int)(te - r * (uint32_t)a.tiles_x);
-        n = (int)(r / (uint32_t)a.tiles_y);
-        const int ty = (int)(r - (uint32_t)n * (uint32_t)a.tiles_y);
-        x0 = tx * TILE_W;
-        y0 = ty * TILE_H;
-      };
       auto issue_loads = [&](long tile, int b) {      // lane 0 issues
         int x0, y0, n;
         tile_xyz(tile, x0, y0, n);
         if (lane == 0) {
           mbar_expect_tx(&pre_bar[b], load_bytes);
           const int cb = ntile * nt;
-          for (int i = 0; i < nb64 + (tail32 ? 1 : 0); i++) {
-            const int wide = i < nb64;
-            const int off = wide ? i * EPI_BLK64_BYTES : nb64 * EPI_BLK64_BYTES;
-            const int col = cb + (wide ? i * 64 : nb64 * 64);
-            if constexpr (HAS_PRE) tma_load_4d(sS + b * a.epi_bytes + off, &em.m[wide ? 2 : 3], &pre_bar[b], p.pre_coff + col, x0, y0, n);
-            if constexpr (NRES >= 1) tma_load_4d(sR1 + b * a.epi_bytes + off, &em.m[wide ? 4 : 5], &pre_bar[b], p.res1_coff + col, x0, y0, n);
-            if constexpr (NRES >= 2) tma_load_4d(sR2 + b * a.epi_bytes + off, &em.m[wide ? 6 : 7], &pre_bar[b], p.res2_coff + col, x0, y0, n);
+          for (int i = 0; i < nblocks; i++) {
+            int col, off, k;
+            staged_block(i, nb64, tail32, col, off, k);
+            if constexpr (HAS_PRE) tma_load_4d(sS + b * a.epi_bytes + off, &em.m[3 + k], &pre_bar[b], p.pre_coff + cb + col, x0, y0, n);
+            if constexpr (NRES >= 1) tma_load_4d(sR1 + b * a.epi_bytes + off, &em.m[6 + k], &pre_bar[b], p.res1_coff + cb + col, x0, y0, n);
+            if constexpr (NRES >= 2) tma_load_4d(sR2 + b * a.epi_bytes + off, &em.m[9 + k], &pre_bar[b], p.res2_coff + cb + col, x0, y0, n);
           }
         }
         __syncwarp();
@@ -297,9 +263,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
           if ((long)blockIdx.x + k * G < a.ntiles) issue_loads(blockIdx.x + k * G, k);
       }
       // The store of tile i is retired (its staging buffer handed back: next pre/residual loads, or sfree) only after
-      // the store of tile i+1 has been issued: `wait_group.read 1` then covers tile i while tile i+1 is still being read,
-      // so the shared-memory read of one tile overlaps the wait for the next (measured on the pair kernel: the
-      // serialised issue -> wait_read -> retire loop was the bottleneck of the small launches).
+      // the store of tile i+1 has been issued: `wait_group.read 1` then covers tile i while tile i+1 is still being read.
       uint32_t it = 0;
       long prev_tile = -1;
       int prev_b = 0;
@@ -317,10 +281,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
           int x0, y0, n;
           tile_xyz(tile, x0, y0, n);
           mbar_wait(&sfull_bar[b], (it / (uint32_t)nbuf) & 1);
-          for (int i = 0; i < nb64 + (tail32 ? 1 : 0); i++) {
-            const int wide = i < nb64;
-            const int off = wide ? i * EPI_BLK64_BYTES : nb64 * EPI_BLK64_BYTES;
-            tma_store_4d(&em.m[(wide ? 0 : 1) + omap], sS + b * a.epi_bytes + off, co_base + (wide ? i * 64 : nb64 * 64), x0, y0, n);
+          for (int i = 0; i < nblocks; i++) {
+            int col, off, k;
+            staged_block(i, nb64, tail32, col, off, k);
+            tma_store_4d(&em.m[k + omap], sS + b * a.epi_bytes + off, co_base + col, x0, y0, n);
           }
           bulk_commit();
           if (prev_tile >= 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");   // the previous tile's stores have read their buffer
@@ -337,73 +301,106 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
       }
       if (lane == 0) bulk_wait0();                 // all stores complete before the CTA (and its smem) goes away
     }
-  } else {
-    // =========================== epilogue warps (2..9) ===========================
-    // Two warpgroups work on the SAME tile: warpgroup w takes the 16-column groups g with g % 2 == w.
-    // The epilogue is instruction-latency bound (one warp per scheduler), so: branch-free activation,
-    // the next TMEM load in flight while the current group is processed, finished tile staged in swizzled
-    // shared memory and written by the TMA warp.
+  } else if (warp < CONS_WARPS) {
+    // =========================== consumer warpgroups (warps 0..7): wgmma + epilogue ===========================
     if constexpr (EPI_MODE != 0) pdl_wait();   // direct epilogues read residual / mask tensors and write the output themselves
-    const int ew = warp - 2;                // 0..EPI_WARPS-1
-    const int wg = ew >> 2;                 // warpgroup 0..EPI_WGS-1
-    const int q = warp & 3;                 // TMEM lane quarter this warp may access
-    const int m = q * 32 + lane;            // accumulator row = tile pixel
-    const int py = m >> 3, px = m & 7;
+    const int wg = warp >> 2, wi = warp & 3;
+    const int f16 = p.f16;
+    // EPI_MODE 3 ("taps in N", last layer): the halo tile is read as a PLAIN K-major tile (8-row groups 8 rows apart)
+    const uint32_t a_sbo = (p.a_mode == 0 && EPI_MODE != 3) ? (uint32_t)HALO_W * a_row : 8u * a_row;
+    const uint64_t a_hi = desc_hi(16, a_sbo, a.chunk64 ? DESC_SW128 : DESC_SW64);
+    const uint64_t b_hi = desc_hi(16, 8 * ROW_B, DESC_SW64);
+    const int ksteps = a.chunk64 ? 4 : 2;                                      // K = 16 steps per A load
+    const uint32_t sA_u = smem_u32(sA), sW_u = smem_u32(sW);
+    const uint32_t b_slot = (uint32_t)(nt * ROW_B);
+    // first A row of this warpgroup's 64 pixels: 8 image rows down the halo tile, or 64 rows of a per-tap tile
+    const uint32_t wg_off = (EPI_MODE == 3) ? 64u * wg * a_row : (p.a_mode == 0 ? 8u * wg * HALO_W * a_row : 64u * wg * (uint32_t)ROW_B);
     const int co_base = ntile * nt;
     const int OW = p.W * p.out_mul, OH = p.H * p.out_mul;
-    const int ngroups = nt >> 4;
-    const int act = p.act, f16 = p.f16;
+    const int act = p.act;
     const float slope = p.slope, alpha = p.alpha;
-    const bool scale = alpha != 1.f;
-    const int sw64 = (m >> 1) & 3, sw128 = m & 7;
-    const uint32_t sS_u = smem_u32(sS), sR1_u = smem_u32(sR1), sR2_u = smem_u32(sR2), sBias_u = smem_u32(sBias);
+    const bool mask_mode = (NRES >= 1) && (p.mask_c1 > p.mask_c0);   // res1 = activation whose sign gates [mask_c0, mask_c1)
+    const uint32_t sS_u = smem_u32(sS), sR1_u = smem_u32(sR1), sR2_u = smem_u32(sR2);
     const bool has_bias = a.bias != nullptr;
-    uint32_t it = 0;
-    const int g0 = wg, gs = EPI_WGS;        // first column group and stride of this warp's groups
-    for (long tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x, it++) {
-      const int acc = (int)(it % nacc);
-      const uint32_t acc_phase = (it / nacc) & 1;
-      const uint32_t te = (uint32_t)(p.tile_rev ? a.ntiles - 1 - tile : tile);
-      const uint32_t r = te / (uint32_t)a.tiles_x;
-      const int tx = (int)(te - r * (uint32_t)a.tiles_x);
-      const int n = (int)(r / (uint32_t)a.tiles_y);
-      const int ty = (int)(r - (uint32_t)n * (uint32_t)a.tiles_y);
-      const int y = ty * TILE_H + py, x = tx * TILE_W + px;
-      const bool valid = (y < p.H) && (x < p.W);
-      const int oy = y * p.out_mul + p.out_py[var], ox = x * p.out_mul + p.out_px[var];
-      const long opix = ((long)n * OH + oy) * OW + ox;
-      const int sb = (int)(it % (uint32_t)nbuf);                // staging buffer of this tile
-      const uint32_t sphase = (it / (uint32_t)nbuf) & 1;
-      const uint32_t bS = sS_u + sb * a.epi_bytes, bR1 = sR1_u + sb * a.epi_bytes, bR2 = sR2_u + sb * a.epi_bytes;
+    const int r0 = 16 * wi + (lane >> 2);       // this thread's accumulator rows: r0 and r0 + 8 of the warpgroup's 64
+    const int cq = 2 * (lane & 3);              // and columns 8j + cq, 8j + cq + 1
 
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
-      if constexpr (EPI_MODE == 0) {
-        if (has_loads) mbar_wait(&pre_bar[sb], sphase);                      // pre / residual tiles of this tile landed
-        else if (it >= (uint32_t)nbuf) mbar_wait(&sfree_bar[sb], sphase ^ 1); // stores of tile it-nbuf have read the buffer
+    auto release = [&](int s) {                 // this warp's wgmmas reading stage s have completed
+      __syncwarp();
+      if (lane == 0) {
+        mbar_arrive(&empty_bar[s]);
+        if (pair && rank == 1) mbar_arrive_cluster(&empty_bar[s], 0);
       }
-      const uint32_t t_addr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * acc_stride);
-      if constexpr (EPI_MODE == 3) {
-        // phase 1: D' rows (halo pixels) -> shared memory.  Warpgroup wg holds halo rows wg*128 + q*32 + lane.
-        float* S = reinterpret_cast<float*>(sS);
-        constexpr int SROW = 29;                                   // floats per halo pixel (27 used; odd stride: no bank conflicts)
-        const int hrow = wg * 128 + m;
-        uint32_t r0[16], r1[16];
-        tmem_ld16(t_addr + wg * 32, r0);
-        tmem_ld16(t_addr + wg * 32 + 16, r1);
-        tmem_ld_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tempty_bar[acc]);              // accumulator free for the MMA warp
-        if (hrow < HALO_W * HALO_H) {
-#pragma unroll
-          for (int j = 0; j < 16; j++) S[hrow * SROW + j] = __uint_as_float(r0[j]);
-#pragma unroll
-          for (int j = 0; j < 11; j++) S[hrow * SROW + 16 + j] = __uint_as_float(r1[j]);
+    };
+    mbar_wait(w_bar, 0);
+    int stage = 0;
+    uint32_t phase = 0;
+    uint32_t it = 0;
+
+    if constexpr (EPI_MODE == 3) {
+      // D'[halo pixel][tap * out_nc + c] = A[halo pixel][K] * B'[K][tap * out_nc + c]: every halo pixel against the filters
+      // of ALL taps at once — three 64-row blocks of halo rows (rows >= 180 are never read back; warpgroup 0 takes blocks
+      // 0 and 2, warpgroup 1 block 1), N = 32; the epilogue adds the nine shifted partial results.
+      float acc0[16], acc1[16];
+      float* S = reinterpret_cast<float*>(sS);
+      constexpr int SROW = 29;                                   // floats per halo pixel (27 used; odd stride: no bank conflicts)
+      for (long tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x, it++) {
+        int prev = -1;
+        for (int c = 0; c < a.nloads; c++) {
+          mbar_wait(&full_bar[stage], phase);
+          const uint32_t a_base = sA_u + (uint32_t)stage * a.a_stage_bytes + wg_off;
+          const uint32_t cb = a.chunk64 ? 2u * (uint32_t)c : (uint32_t)c;
+          wgmma_fence();
+          for (int ks = 0; ks < ksteps; ks++) {
+            const uint64_t da = make_desc(a_base + 32u * ks, a_hi);
+            // block 2: warpgroup 0 keeps it; warpgroup 1 issues the same wgmma into acc1 and discards it, so both
+            // warpgroups run one uniform wgmma stream (a wgmma on a divergent path is serialised by the compiler)
+            const uint64_t da2 = make_desc(sA_u + (uint32_t)stage * a.a_stage_bytes + 128u * a_row + 32u * ks, a_hi);
+            const uint64_t db = make_desc(sW_u + (cb + (uint32_t)(ks >> 1)) * b_slot + 32u * (ks & 1), b_hi);
+            const int sc = (c | ks) != 0;
+            if (f16) {
+              wgmma<32, 1, 0>(acc0, da, db, sc);
+              wgmma<32, 1, 0>(acc1, da2, db, sc);
+            } else {
+              wgmma<32, 0, 0>(acc0, da, db, sc);
+              wgmma<32, 0, 0>(acc1, da2, db, sc);
+            }
+          }
+          wgmma_commit();
+          if (prev >= 0) { wgmma_wait<1>(); release(prev); }
+          prev = stage;
+          if (++stage == a.stages) { stage = 0; phase ^= 1; }
         }
-        asm volatile("bar.sync 1, %0;" ::"n"(EPI_WARPS * 32) : "memory");
+        wgmma_wait<0>();
+        fence_regs<16>(acc0);
+        fence_regs<16>(acc1);
+        release(prev);
+        int x0, y0, n;
+        tile_xyz(tile, x0, y0, n);
+        // phase 1: D' rows (halo pixels) -> shared memory
+#pragma unroll
+        for (int blk = 0; blk < 2; blk++) {
+          if (blk == 1 && wg != 0) break;
+          const float* d = blk ? acc1 : acc0;
+          const int hb = blk ? 128 : 64 * wg;
+#pragma unroll
+          for (int h = 0; h < 2; h++) {
+            const int hrow = hb + r0 + 8 * h;
+            if (hrow < HALO_W * HALO_H) {
+#pragma unroll
+              for (int j = 0; j < 4; j++)
+#pragma unroll
+                for (int e = 0; e < 2; e++)
+                  if (8 * j + cq + e < 27) S[hrow * SROW + 8 * j + cq + e] = d[4 * j + 2 * h + e];
+            }
+          }
+        }
+        asm volatile("bar.sync 1, %0;" ::"n"(CONS_WARPS * 32) : "memory");
         // phase 2: output pixel (py, px) of the tile = sum over the nine taps of the partial result of its neighbour
-        if (wg == 0 && valid) {
+        const int m = threadIdx.x;
+        const int py = m >> 3, px = m & 7;
+        const int y = y0 + py, x = x0 + px;
+        if (wg == 0 && y < p.H && x < p.W) {
           float* of = reinterpret_cast<float*>(a.out);
           const long plane = (long)OH * OW;
           const int onc = p.out_nc;
@@ -412,156 +409,133 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
 #pragma unroll
             for (int t9 = 0; t9 < 9; t9++) v += S[((py + t9 / 3) * HALO_W + (px + t9 % 3)) * SROW + t9 * onc + c];
             if (act != DASR_ACT_NONE && p.act_cols > 0) v = (act == DASR_ACT_LRELU) ? fmaxf(v, v * slope) : fmaxf(v, 0.f);
-            of[((long)n * onc + c) * plane + (long)oy * OW + ox] = v * alpha;
+            of[((long)n * onc + c) * plane + (long)y * OW + x] = v * alpha;
           }
         }
-        asm volatile("bar.sync 1, %0;" ::"n"(EPI_WARPS * 32) : "memory");   // S may be overwritten by the next tile
-        continue;
+        asm volatile("bar.sync 1, %0;" ::"n"(CONS_WARPS * 32) : "memory");   // S may be overwritten by the next tile
       }
-      // One 16-column group: registers -> (+bias, +pre) -> act -> scale -> (+residuals) -> bf16 -> staged tile / global.
-      auto process = [&](const uint32_t* rr, int g) {
-        const int cg = g << 4;
-        const int co = co_base + cg;
-        const bool do_act = (act != DASR_ACT_NONE) && (co + 16 <= p.act_cols);
-        float v[16];
-#pragma unroll
-        for (int j = 0; j < 16; j++) v[j] = __uint_as_float(rr[j]);
-        if (has_bias) {
-#pragma unroll
-          for (int j4 = 0; j4 < 4; j4++) {
-            const float4 b4 = lds128f(sBias_u + (cg + 4 * j4) * 4);
-            v[4 * j4 + 0] += b4.x;
-            v[4 * j4 + 1] += b4.y;
-            v[4 * j4 + 2] += b4.z;
-            v[4 * j4 + 3] += b4.w;
+    } else {
+      float acc[ACC_REGS];
+      for (long tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x, it++) {
+        int prev = -1;
+        for (int c = 0; c < a.nloads; c++) {
+          mbar_wait(&full_bar[stage], phase);
+          const uint32_t a_base = sA_u + (uint32_t)stage * a.a_stage_bytes + wg_off;
+          // K step ks of this load reads 32 B at offset 32 * ks of every A row and the 32-channel filter chunk
+          // cb + (ks >> 1) at offset 32 * (ks & 1) of its rows
+          const uint32_t cb = a.chunk64 ? 2u * (uint32_t)c : (uint32_t)c;
+          wgmma_fence();
+#pragma unroll 1
+          for (int tap = 0; tap < ntaps; tap++) {
+            const uint32_t b_addr = sW_u + ((uint32_t)tap * a.nchunks + cb) * b_slot;
+            const int first = (c | tap) == 0;
+            if (f16) issue_tap_rt<1>(nt, acc, a_base + sTap[tap], a_hi, b_addr, b_slot, b_hi, ksteps, first);
+            else issue_tap_rt<0>(nt, acc, a_base + sTap[tap], a_hi, b_addr, b_slot, b_hi, ksteps, first);
           }
+          wgmma_commit();
+          if (prev >= 0) { wgmma_wait<1>(); release(prev); }
+          prev = stage;
+          if (++stage == a.stages) { stage = 0; phase ^= 1; }
         }
+        wgmma_wait<0>();
+        fence_regs<ACC_REGS>(acc);
+        release(prev);
+
+        int x0, y0, n;
+        tile_xyz(tile, x0, y0, n);
+        const int sb = (int)(it % (uint32_t)nbuf);                // staging buffer of this tile
+        const uint32_t sphase = (it / (uint32_t)nbuf) & 1;
+        const uint32_t bS = sS_u + sb * a.epi_bytes, bR1 = sR1_u + sb * a.epi_bytes, bR2 = sR2_u + sb * a.epi_bytes;
         if constexpr (EPI_MODE == 0) {
-          int o0, o1;
-          if (cg < (nb64 << 6)) {             // inside a 64-channel block (128 B rows, SWIZZLE_128B)
-            const int base = (cg >> 6) * EPI_BLK64_BYTES + m * 128;
-            const int c0 = (cg & 63) >> 3;
-            o0 = base + ((c0 ^ sw128) << 4);
-            o1 = base + (((c0 + 1) ^ sw128) << 4);
-          } else {                            // 32-channel tail block (64 B rows, SWIZZLE_64B)
-            const int base = nb64 * EPI_BLK64_BYTES + m * 64;
-            const int c0 = (cg & 31) >> 3;
-            o0 = base + ((c0 ^ sw64) << 4);
-            o1 = base + (((c0 + 1) ^ sw64) << 4);
-          }
-          if constexpr (HAS_PRE) {
-            fma_h16x8(v, lds128(bS + o0), 1.f, f16);
-            fma_h16x8(v + 8, lds128(bS + o1), 1.f, f16);
-          }
-          if (do_act) {
-            if (act == DASR_ACT_LRELU) {
+          if (has_loads) mbar_wait(&pre_bar[sb], sphase);                      // pre / residual tiles of this tile landed
+          else if (it >= (uint32_t)nbuf) mbar_wait(&sfree_bar[sb], sphase ^ 1); // stores of tile it-nbuf have read the buffer
+        }
 #pragma unroll
-              for (int j = 0; j < 16; j++) v[j] = fmaxf(v[j], v[j] * slope);     // 0 < slope < 1
-            } else {
+        for (int h = 0; h < 2; h++) {
+          const int m = 64 * wg + r0 + 8 * h;               // tile pixel
+          const int py = m >> 3, px = m & 7;
+          const int y = y0 + py, x = x0 + px;
+          const bool valid = (y < p.H) && (x < p.W);
+          const int oy = y * p.out_mul + p.out_py[var], ox = x * p.out_mul + p.out_px[var];
+          const long opix = ((long)n * OH + oy) * OW + ox;
 #pragma unroll
-              for (int j = 0; j < 16; j++) v[j] = fmaxf(v[j], 0.f);
-            }
-          }
-          if (scale) {
-#pragma unroll
-            for (int j = 0; j < 16; j++) v[j] *= alpha;
-          }
-          if constexpr (NRES >= 1) {
-            fma_h16x8(v, lds128(bR1 + o0), p.beta1, f16);
-            fma_h16x8(v + 8, lds128(bR1 + o1), p.beta1, f16);
-          }
-          if constexpr (NRES >= 2) {
-            fma_h16x8(v, lds128(bR2 + o0), p.beta2, f16);
-            fma_h16x8(v + 8, lds128(bR2 + o1), p.beta2, f16);
-          }
-          uint4 o[2];
-          pack_h16x16(v, o, f16);
-          sts128(bS + o0, o[0]);
-          sts128(bS + o1, o[1]);
-        } else if (valid) {
-          if (do_act) {
-#pragma unroll
-            for (int j = 0; j < 16; j++) v[j] = (act == DASR_ACT_LRELU) ? fmaxf(v[j], v[j] * slope) : fmaxf(v[j], 0.f);
-          }
-#pragma unroll
-          for (int j = 0; j < 16; j++) v[j] *= alpha;
-          if constexpr (EPI_MODE == 2) {
-            // final layer: first out_nc channels straight to NCHW fp32 (the module boundary layout)
-            float* of = reinterpret_cast<float*>(a.out);
-            const long plane = (long)OH * OW;
-#pragma unroll
-            for (int j = 0; j < 16; j++)
-              if (co + j < p.out_nc) of[((long)n * p.out_nc + co + j) * plane + (long)oy * OW + ox] = v[j];
-          } else {
-            __nv_bfloat16* ob16 = reinterpret_cast<__nv_bfloat16*>(a.out);
-            if (a.res1) {
-              const uint4* rp = reinterpret_cast<const uint4*>(a.res1 + opix * p.res1_cs + p.res1_coff + co);
-              fma_h16x8(v, __ldg(rp), p.beta1, f16);
-              fma_h16x8(v + 8, __ldg(rp + 1), p.beta1, f16);
-            }
-            if (a.res2) {
-              const uint4* rp = reinterpret_cast<const uint4*>(a.res2 + opix * p.res2_cs + p.res2_coff + co);
-              fma_h16x8(v, __ldg(rp), p.beta2, f16);
-              fma_h16x8(v + 8, __ldg(rp + 1), p.beta2, f16);
-            }
-            if (a.mask_src && co + 16 > p.mask_c0 && co < p.mask_c1) {
-              const __nv_bfloat16* mp = a.mask_src + opix * p.mask_cs + p.mask_coff + (co - p.mask_c0);
-#pragma unroll
-              for (int j = 0; j < 16; j++) {
-                int cc = co + j;
-                if (cc >= p.mask_c0 && cc < p.mask_c1) {
-                  float mv = __bfloat162float(mp[j]);
-                  if (!(mv > 0.f)) v[j] *= p.mask_slope;
+          for (int j = 0; j < ACC_REGS / 4; j++) {
+            if (j < (nt >> 3)) {
+              const int cl = 8 * j + cq;                    // channel inside the tile
+              const int co = co_base + cl;
+              float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+              if (has_bias) { v0 += sBias[cl]; v1 += sBias[cl + 1]; }
+              const bool do_act = (act != DASR_ACT_NONE) && (co < p.act_cols);
+              if constexpr (EPI_MODE == 0) {
+                const uint32_t o = staged_off(m, cl, nb64, tail32);
+                if constexpr (HAS_PRE) {
+                  const float2 q = h16x2_to_f2(lds32(bS + o), f16);
+                  v0 += q.x; v1 += q.y;
+                }
+                if (do_act) {
+                  if (act == DASR_ACT_LRELU) { v0 = fmaxf(v0, v0 * slope); v1 = fmaxf(v1, v1 * slope); }   // 0 < slope < 1
+                  else { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+                }
+                v0 *= alpha; v1 *= alpha;
+                if constexpr (NRES >= 1) {
+                  const uint32_t r = lds32(bR1 + o);
+                  if (mask_mode) {
+                    if (co >= p.mask_c0 && co < p.mask_c1) {    // a positive finite bf16 / half is a positive 16-bit integer
+                      if (!((short)(r & 0xFFFF) > 0)) v0 *= p.mask_slope;
+                      if (!((short)(r >> 16) > 0)) v1 *= p.mask_slope;
+                    }
+                  } else {
+                    const float2 q = h16x2_to_f2(r, f16);
+                    v0 = fmaf(p.beta1, q.x, v0); v1 = fmaf(p.beta1, q.y, v1);
+                  }
+                }
+                if constexpr (NRES >= 2) {
+                  const float2 q = h16x2_to_f2(lds32(bR2 + o), f16);
+                  v0 = fmaf(p.beta2, q.x, v0); v1 = fmaf(p.beta2, q.y, v1);
+                }
+                sts32(bS + o, f2_to_h16x2(v0, v1, f16));
+              } else if (valid) {
+                if (do_act) {
+                  v0 = (act == DASR_ACT_LRELU) ? fmaxf(v0, v0 * slope) : fmaxf(v0, 0.f);
+                  v1 = (act == DASR_ACT_LRELU) ? fmaxf(v1, v1 * slope) : fmaxf(v1, 0.f);
+                }
+                v0 *= alpha; v1 *= alpha;
+                if constexpr (EPI_MODE == 2) {
+                  // final layer: first out_nc channels straight to NCHW fp32 (the module boundary layout)
+                  float* of = reinterpret_cast<float*>(a.out);
+                  const long plane = (long)OH * OW;
+                  if (co < p.out_nc) of[((long)n * p.out_nc + co) * plane + (long)oy * OW + ox] = v0;
+                  if (co + 1 < p.out_nc) of[((long)n * p.out_nc + co + 1) * plane + (long)oy * OW + ox] = v1;
+                } else {
+                  if (a.res1) {
+                    const float2 q = h16x2_to_f2(__ldg(reinterpret_cast<const unsigned int*>(a.res1 + opix * p.res1_cs + p.res1_coff + co)), f16);
+                    v0 = fmaf(p.beta1, q.x, v0); v1 = fmaf(p.beta1, q.y, v1);
+                  }
+                  if (a.res2) {
+                    const float2 q = h16x2_to_f2(__ldg(reinterpret_cast<const unsigned int*>(a.res2 + opix * p.res2_cs + p.res2_coff + co)), f16);
+                    v0 = fmaf(p.beta2, q.x, v0); v1 = fmaf(p.beta2, q.y, v1);
+                  }
+                  if (a.mask_src) {
+                    const __nv_bfloat16* mp = a.mask_src + opix * p.mask_cs + p.mask_coff + (co - p.mask_c0);
+                    if (co >= p.mask_c0 && co < p.mask_c1 && !(__bfloat162float(mp[0]) > 0.f)) v0 *= p.mask_slope;
+                    if (co + 1 >= p.mask_c0 && co + 1 < p.mask_c1 && !(__bfloat162float(mp[1]) > 0.f)) v1 *= p.mask_slope;
+                  }
+                  __nv_bfloat16* ob16 = reinterpret_cast<__nv_bfloat16*>(a.out);
+                  *reinterpret_cast<uint32_t*>(ob16 + opix * p.out_cs + p.out_coff + co) = f2_to_h16x2(v0, v1, f16);
                 }
               }
             }
-            uint4 o[2];
-            pack_h16x16(v, o, f16);
-            uint4* op = reinterpret_cast<uint4*>(ob16 + opix * p.out_cs + p.out_coff + co);
-            op[0] = o[0];
-            op[1] = o[1];
           }
         }
-      };
-      auto release_acc = [&]() {
-        // all TMEM reads of this warp for this tile are done: hand the accumulator back early
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-      };
-      // two register sets: the next group's accumulators are in flight while the current group is processed
-      uint32_t ra[16], rb[16];
-      if (g0 < ngroups) tmem_ld16(t_addr + g0 * 16, ra);
-      for (int g = g0; g < ngroups; g += 2 * gs) {
-        tmem_ld_wait();
-        if (g + gs < ngroups) tmem_ld16(t_addr + (g + gs) * 16, rb); else release_acc();
-        process(ra, g);
-        if (g + gs < ngroups) {
-          tmem_ld_wait();
-          if (g + 2 * gs < ngroups) tmem_ld16(t_addr + (g + 2 * gs) * 16, ra); else release_acc();
-          process(rb, g + gs);
+        if constexpr (EPI_MODE == 0) {
+          fence_proxy_async();          // generic-proxy writes of the staged tile -> visible to the TMA engine
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&sfull_bar[sb]);
         }
-      }
-      if (g0 >= ngroups) {
-        // this warpgroup had no column group in the tile (nt == 16): still release the accumulator
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-      }
-      if constexpr (EPI_MODE == 0) {
-        fence_proxy_async();          // generic-proxy writes of the staged tile -> visible to the TMA engine
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&sfull_bar[sb]);
       }
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, (uint32_t)a.tmem_cols);
-  }
+  if (pair) cluster_sync();             // no CTA leaves while its peer may still multicast into it or arrive on its barriers
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -664,69 +638,6 @@ __global__ void pack_filter_tc_batch_kernel(const DasrPackJob* __restrict__ jobs
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
-
-static int pow2_at_least(int v) {
-  int r = 32;
-  while (r < v) r <<= 1;
-  return r;
-}
-
-
-// ---------------------------------------------------------------------------------------------
-// tcgen05.mma issue-rate probe (selftest only): one elected thread issues `iters` groups of 18 MMAs
-// (M=128, N=n, K=16, bf16) whose A descriptors walk 9 tap offsets of a halo tile, commits, waits.
-// Reports SM cycles per MMA.  Used to choose tile shapes; not part of the product path.
-// ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128, 1) mma_rate_kernel(int n, int sbo, int iters, int a_step, long long* out) {
-  // a_step >= 0x10000 encodes the probe mode: bits 16..19 = number of accumulators the MMAs rotate over (independent
-  // accumulate chains), bit 20 = do not wait for completion between the groups of 18 (throughput instead of latency)
-  const int nacc = (a_step >> 16) & 15 ? (a_step >> 16) & 15 : 1;
-  const bool nowait = (a_step >> 20) & 1;
-  a_step &= 0xFFFF;
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  __shared__ uint64_t bar;
-  __shared__ uint32_t tptr;
-  for (int i = threadIdx.x; i < 48 * 1024 / 4; i += blockDim.x) reinterpret_cast<uint32_t*>(smem)[i] = 0;
-  if (threadIdx.x == 0) { mbar_init(&bar, 1); fence_barrier_init(); }
-  fence_proxy_async();
-  if (threadIdx.x < 32) tmem_alloc(&tptr, 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tb = tptr;
-  if (threadIdx.x < 32) {
-    const uint32_t idesc = make_idesc_bf16(128, n);
-    const uint32_t a0 = smem_u32(smem), b0 = smem_u32(smem + 16384);
-    const uint32_t acc_stride = 512u / (uint32_t)nacc;
-    long long t0 = clock64();
-    uint32_t ph = 0;
-    for (int it = 0; it < iters; it++) {
-      if (elect_one()) {
-        int kk = 0;
-#pragma unroll 1
-        for (int tap = 0; tap < 9; tap++) {
-          uint32_t aa = a0 + (uint32_t)(((tap / 3) * 10 + (tap % 3)) * a_step);
-#pragma unroll
-          for (int k = 0; k < 2; k++, kk++)
-            umma_bf16(tb + (uint32_t)(kk % nacc) * acc_stride, make_desc_sw64(aa + k * 32, (uint32_t)sbo),
-                      make_desc_sw64(b0 + k * 32, 512), idesc, 1u);
-        }
-        if (!nowait || it == iters - 1) umma_commit(&bar);
-      }
-      __syncwarp();
-      if (!nowait || it == iters - 1) {
-        mbar_wait(&bar, ph);
-        ph ^= 1;
-      }
-    }
-    long long t1 = clock64();
-    if (threadIdx.x == 0 && blockIdx.x == 0) out[0] = (t1 - t0);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (threadIdx.x < 32) { tc_fence_after(); tmem_dealloc(tb, 512); }
-}
 
 // ---------------------------------------------------------------------------------------------
 // TMA row-rate probe (selftest only): every CTA streams `iters` boxes of [rows x row_bytes] from / to a large
@@ -851,15 +762,201 @@ static int encode_act_map(PFN_encodeTiled enc, CUtensorMap* tm, const void* base
   cuuint64_t gstr[3] = {(cuuint64_t)mul * cs * 2, (cuuint64_t)mul * (mul * W) * cs * 2, (cuuint64_t)(mul * H) * (mul * W) * cs * 2};
   cuuint32_t box[4] = {(cuuint32_t)width, TILE_W, TILE_H, 1};
   cuuint32_t estr[4] = {1, 1, 1, 1};
+  const CUtensorMapSwizzle sw = width == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : (width == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
   CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), gdim, gstr, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, width == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                   (width == 32 && cs > 32) ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B : CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
+                   (width < 64 && cs > width) ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B : CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_error("conv_tc: cuTensorMapEncodeTiled(%s) failed: %d", what, (int)r);
     return DASR_E_LAUNCH;
   }
   return DASR_OK;
+}
+
+// the 64-, 32- and 16-channel maps of one staged-epilogue tensor (slots m[0..2])
+static int encode_staged_maps(PFN_encodeTiled enc, CUtensorMap* m, const void* base, int cs, int nt, int W, int H, int N,
+                              const char* what, int mul = 1) {
+  int rc;
+  if (nt >= 64 && (rc = encode_act_map(enc, &m[0], base, cs, W, H, N, 64, what, mul))) return rc;
+  if ((nt & 32) && (rc = encode_act_map(enc, &m[1], base, cs, W, H, N, 32, what, mul))) return rc;
+  if ((nt & 16) && (rc = encode_act_map(enc, &m[2], base, cs, W, H, N, 16, what, mul))) return rc;
+  return DASR_OK;
+}
+
+static size_t a_stage_bytes_for(const DasrConvTcParams* p, int chunk64) {
+  return (p->a_mode == 0) ? (size_t)(chunk64 ? 2 : 1) * A_STAGE_ROWS * ROW_B : (size_t)p->ntaps * A_TAP_BYTES;
+}
+static const int TC_BAR_BYTES = (2 * MAX_STAGES + 24) * 8 + 256 * 4 + 16;
+
+// Shared-memory plan: staged-epilogue buffers as many (<= 4) as still leave 4 A stages — loads of pre / residual tiles
+// are issued nbuf tiles ahead, which hides their latency — then as many A stages as fit (<= MAX_STAGES).  One buffer
+// (stores of a tile drain before the next tile's epilogue) only when two would leave fewer than 2 A stages.
+// Returns the number of A stages (< 2: does not fit).
+static int tc_plan(int w_bytes, int a_stage, int epi_bytes, int nres_loaded, int epi_mode, int* nbuf_out) {
+  int nbuf = (epi_mode == 0) ? 4 : (epi_mode == 3 ? 1 : 2);
+  int avail = 0;
+  for (;; nbuf--) {
+    const int epi_total = nbuf * epi_bytes * (1 + nres_loaded);
+    avail = SMEM_LIMIT - 1024 /*alignment slack*/ - w_bytes - epi_total - TC_BAR_BYTES;
+    if (nbuf <= 1 || avail >= 4 * a_stage || (nbuf == 2 && avail >= 2 * a_stage)) break;
+  }
+  *nbuf_out = nbuf;
+  int stages = avail > 0 ? avail / a_stage : 0;
+  return stages > MAX_STAGES ? MAX_STAGES : stages;
+}
+
+static int chunk64_allowed() {
+  static int ok = -1;
+  if (ok < 0) {
+    const char* e = getenv("DASR_TC_CHUNK64");
+    ok = (e && e[0] == '0') ? 0 : 1;
+  }
+  return ok;
+}
+
+// pair = 1: (1, 2, 1) clusters, p->nt is the Cout tile of ONE CTA (half of the pair's tile)
+static int conv_tc_launch(const void* in, const void* w, const float* bias, const void* pre, const void* res1, const void* res2,
+                          const void* mask_src, void* out, const DasrConvTcParams* p, void* stream, int pair) {
+  PFN_encodeTiled enc = get_encode();
+  if (!enc) {
+    set_error("conv_tc: cuTensorMapEncodeTiled not available");
+    return DASR_E_NODRIVER;
+  }
+
+  TcKernelArgs a;
+  a.p = *p;
+  a.bias = bias;
+  a.res1 = (const __nv_bfloat16*)res1;
+  a.res2 = (const __nv_bfloat16*)res2;
+  a.mask_src = (const __nv_bfloat16*)mask_src;
+  a.out = out;
+  a.pair = pair;
+  a.nchunks = p->cin / CHUNK;
+  a.n_ntiles = p->cout / p->nt;
+  a.tiles_x = cdiv(p->W, TILE_W);
+  a.tiles_y = cdiv(p->H, TILE_H);
+  a.ntiles = (long)p->N * a.tiles_x * a.tiles_y;
+  a.w_bytes = p->ntaps * a.nchunks * p->nt * ROW_B;
+  // 64-channel A chunks: contiguous input slice whose channel count is a multiple of 64; a pair keeps 32-channel stages,
+  // whose smaller footprint leaves room for the larger filter sets it exists for
+  a.chunk64 = (chunk64_allowed() && !pair && p->a_mode == 0 && p->nchunk_list == 0 && p->cin % (2 * CHUNK) == 0) ? 1 : 0;
+  a.nloads = a.chunk64 ? a.nchunks / 2 : a.nchunks;
+  a.a_stage_bytes = (int)a_stage_bytes_for(p, a.chunk64);
+  a.has_pre = (p->epi_mode == 0 && pre) ? 1 : 0;
+  a.has_res1 = (p->epi_mode == 0 && res1) ? 1 : 0;
+  a.has_res2 = (p->epi_mode == 0 && res2) ? 1 : 0;
+  a.epi_bytes = (p->epi_mode == 0) ? p->nt * 128 * 2 : (p->epi_mode == 3 ? 21504 : 0);   // mode 3: 180 halo pixels x 29 floats
+  int nbuf = 2;
+  const int stages = tc_plan(a.w_bytes, a.a_stage_bytes, a.epi_bytes, a.has_res1 + a.has_res2, p->epi_mode, &nbuf);
+  a.nbuf = nbuf;
+  const int epi_total = nbuf * a.epi_bytes * (1 + a.has_res1 + a.has_res2);
+  if (stages < 2) {
+    set_error("conv_tc: resident filters (%d B) + epilogue tiles (%d B) + 2 A stages do not fit shared memory; use a smaller nt",
+              a.w_bytes, epi_total);
+    return DASR_E_SMEM;
+  }
+  a.stages = stages;
+  const size_t smem = 1024 + (size_t)a.w_bytes + (size_t)stages * a.a_stage_bytes + epi_total + TC_BAR_BYTES;
+
+  CUtensorMap tm_in, tm_w;
+  EpiMaps em;
+  {
+    cuuint64_t gdim[4] = {(cuuint64_t)p->in_cs, (cuuint64_t)p->W, (cuuint64_t)p->H, (cuuint64_t)p->N};
+    cuuint64_t gstr[3] = {(cuuint64_t)p->in_cs * 2, (cuuint64_t)p->W * p->in_cs * 2,
+                          (cuuint64_t)p->H * p->W * p->in_cs * 2};
+    cuuint32_t box[4] = {(cuuint32_t)(a.chunk64 ? 2 * CHUNK : CHUNK), (cuuint32_t)(p->a_mode == 0 ? HALO_W : TILE_W),
+                         (cuuint32_t)(p->a_mode == 0 ? HALO_H : TILE_H), 1};
+    cuuint32_t estr[4] = {1, 1, 1, 1};
+    // a 32-channel chunk is 64 B of a wider pixel row: promoting its L2 fills to 128 B would double the DRAM reads of A
+    CUresult r = enc(&tm_in, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(in), gdim, gstr, box, estr,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, a.chunk64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
+                     (p->in_cs > CHUNK && !a.chunk64) ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B : CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+      set_error("conv_tc: cuTensorMapEncodeTiled(input) failed: %d", (int)r);
+      return DASR_E_LAUNCH;
+    }
+  }
+  {
+    cuuint64_t rows = (cuuint64_t)p->nvar * p->ntaps * a.nchunks * p->cout;
+    cuuint64_t gdim[2] = {CHUNK, rows};
+    cuuint64_t gstr[1] = {ROW_B};
+    cuuint32_t box[2] = {CHUNK, (cuuint32_t)p->nt};
+    cuuint32_t estr[2] = {1, 1};
+    CUresult r = enc(&tm_w, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(w), gdim, gstr, box, estr,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+      set_error("conv_tc: cuTensorMapEncodeTiled(filter) failed: %d", (int)r);
+      return DASR_E_LAUNCH;
+    }
+  }
+  for (int i = 0; i < 12; i++) em.m[i] = tm_in;   // placeholders when unused
+  if (p->epi_mode == 0) {
+    const void* bases[4] = {out, pre, res1, res2};
+    const int css[4] = {p->out_cs, p->pre_cs, p->res1_cs, p->res2_cs};
+    const int used[4] = {1, a.has_pre, a.has_res1, a.has_res2};
+    const char* names[4] = {"output", "pre", "res1", "res2"};
+    if (p->out_mul == 2) {
+      // one output map triple per parity variant (slots 3v..3v+2; no pre / residual maps in this mode)
+      for (int v = 0; v < p->nvar && v < 4; v++) {
+        const char* vb = (const char*)out + ((size_t)p->out_py[v] * (2 * p->W) + p->out_px[v]) * p->out_cs * 2;
+        int rc = encode_staged_maps(enc, &em.m[3 * v], vb, p->out_cs, p->nt, p->W, p->H, p->N, "output", 2);
+        if (rc) return rc;
+      }
+    } else {
+      for (int t = 0; t < 4; t++) {
+        if (!used[t]) continue;
+        int rc = encode_staged_maps(enc, &em.m[3 * t], bases[t], css[t], p->nt, p->W, p->H, p->N, names[t]);
+        if (rc) return rc;
+      }
+    }
+  }
+
+  typedef void (*KernelFn)(const CUtensorMap, const CUtensorMap, const EpiMaps, const TcKernelArgs);
+  static const KernelFn kernels[9] = {
+      conv_tc_kernel<0, false, 0>, conv_tc_kernel<0, false, 1>, conv_tc_kernel<0, false, 2>,
+      conv_tc_kernel<0, true, 0>,  conv_tc_kernel<0, true, 1>,  conv_tc_kernel<0, true, 2>,
+      conv_tc_kernel<1, false, 0>, conv_tc_kernel<2, false, 0>, conv_tc_kernel<3, false, 0>};
+  const int ki = (p->epi_mode == 0) ? (a.has_pre * 3 + a.has_res1 + a.has_res2) : (5 + p->epi_mode);
+  if (p->epi_mode == 0) DASR_REQUIRE(!(a.has_res2 && !a.has_res1), "conv_tc: res2 without res1");
+  static bool attr_set[9] = {false, false, false, false, false, false, false, false, false};
+  if (!attr_set[ki]) {
+    cudaError_t e = cudaFuncSetAttribute(kernels[ki], cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
+    if (e != cudaSuccess) {
+      set_error("conv_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
+      return DASR_E_LAUNCH;
+    }
+    attr_set[ki] = true;
+  }
+  int gy = p->nvar * a.n_ntiles;
+  int gx = num_sms() / gy;
+  if (gx < 1) gx = 1;
+  if ((long)gx > a.ntiles) gx = (int)a.ntiles;
+  // programmatic dependent launch: this kernel's prologue (barrier init, resident filter load) may run while the previous
+  // kernel of the stream drains; every global access that depends on it sits behind griddepcontrol.wait
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(gx, gy, 1);
+  cfg.blockDim = dim3(TCK_THREADS, 1, 1);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = (cudaStream_t)stream;
+  cudaLaunchAttribute attrs[2];
+  attrs[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attrs[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
+  attrs[1].id = cudaLaunchAttributeClusterDimension;
+  attrs[1].val.clusterDim.x = 1;
+  attrs[1].val.clusterDim.y = pair ? 2 : 1;
+  attrs[1].val.clusterDim.z = 1;
+  cfg.attrs = attrs;
+  cfg.numAttrs = pair ? 2 : 1;
+  cudaError_t le = cudaLaunchKernelEx(&cfg, kernels[ki], tm_in, tm_w, em, a);
+  if (le != cudaSuccess) {
+    cudaGetLastError();                 // reported here, not by the next launch's check
+    set_error("conv_tc: launch failed: %s", cudaGetErrorString(le));
+    return DASR_E_LAUNCH;
+  }
+  return check_launch(pair ? "conv_tc2" : "conv_tc");
 }
 
 int dasr_conv_tc(const void* in, const void* w, const float* bias, const void* pre, const void* res1, const void* res2,
@@ -905,177 +1002,65 @@ int dasr_conv_tc(const void* in, const void* w, const float* bias, const void* p
   DASR_REQUIRE((reinterpret_cast<uintptr_t>(in) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0 &&
                    (reinterpret_cast<uintptr_t>(w) & 15) == 0,
                "conv_tc: pointers must be 16-byte aligned");
-  PFN_encodeTiled enc = get_encode();
-  if (!enc) {
-    set_error("conv_tc: cuTensorMapEncodeTiled not available");
-    return DASR_E_NODRIVER;
-  }
+  DasrConvTcParams q = *p;
+  if (p->epi_mode == 0) q.mask_c0 = q.mask_c1 = 0;   // the staged epilogue's mask mode belongs to dasr_conv_tc2
+  return conv_tc_launch(in, w, bias, pre, res1, res2, mask_src, out, &q, stream, 0);
+}
 
-  TcKernelArgs a;
-  a.p = *p;
-  a.bias = bias;
-  a.res1 = (const __nv_bfloat16*)res1;
-  a.res2 = (const __nv_bfloat16*)res2;
-  a.mask_src = (const __nv_bfloat16*)mask_src;
-  a.out = out;
-  a.nchunks = p->cin / CHUNK;
-  a.n_ntiles = p->cout / p->nt;
-  a.tiles_x = cdiv(p->W, TILE_W);
-  a.tiles_y = cdiv(p->H, TILE_H);
-  a.ntiles = (long)p->N * a.tiles_x * a.tiles_y;
-  a.w_bytes = p->ntaps * a.nchunks * p->nt * ROW_B;
-  static int chunk64_ok = -1;
-  if (chunk64_ok < 0) {
-    const char* e = getenv("DASR_TC_CHUNK64");
-    chunk64_ok = (e && e[0] == '0') ? 0 : 1;
+// ---- cluster pair: the two Cout halves of a tile on two SMs of a (1, 2, 1) cluster, A tiles multicast ----
+static int tc2_fits(const DasrConvTcParams* p, int nres) {
+  // one CTA: half of the pair's filters, staged blocks of nt / 2 channels
+  const int half = p->nt / 2;
+  const int w_bytes = 9 * (p->cin / CHUNK) * half * ROW_B;
+  int nbuf;
+  return tc_plan(w_bytes, (int)a_stage_bytes_for(p, 0), half * 128 * 2, nres, 0, &nbuf) >= 2;
+}
+
+int dasr_conv_tc2_supported(const DasrConvTcParams* p) {
+  // plain 3x3 fprop/dgrad geometry, staged bf16 epilogue; pre / residual tensors are announced through their channel
+  // strides (pre_cs, res1_cs, res2_cs > 0), as dasr_conv_tc2 callers fill them
+  if (!p) return 0;
+  if (p->nvar != 1 || p->ntaps != 9 || p->out_mul != 1 || p->epi_mode != 0 || p->a_mode != 0) return 0;
+  if (p->nt % 32 != 0 || p->nt < 32 || p->nt > 256 || p->cout % p->nt != 0 || p->cin % CHUNK != 0 || p->cin <= 0) return 0;
+  return tc2_fits(p, (p->res1_cs > 0 ? 1 : 0) + (p->res2_cs > 0 ? 1 : 0));
+}
+
+int dasr_conv_tc2(const void* in, const void* w, const float* bias, const void* pre, const void* res1, const void* res2,
+                  void* out, const DasrConvTcParams* p, void* stream) {
+  DASR_REQUIRE(p && in && w && out, "conv_tc2: null argument");
+  DASR_REQUIRE(p->nvar == 1 && p->ntaps == 9 && p->out_mul == 1 && p->epi_mode == 0 && p->a_mode == 0,
+               "conv_tc2: plain 3x3 geometry with the staged epilogue only");
+  DASR_REQUIRE(p->nt % 32 == 0 && p->nt >= 32 && p->nt <= 256 && p->cout % p->nt == 0,
+               "conv_tc2: the Cout tile nt must be a multiple of 32 in [32, 256] that divides cout (nt=%d cout=%d)", p->nt, p->cout);
+  DASR_REQUIRE(p->N > 0 && p->H > 0 && p->W > 0, "conv_tc2: bad dims");
+  DASR_REQUIRE((long)p->N * cdiv(p->W, TILE_W) * cdiv(p->H, TILE_H) < (1L << 30), "conv_tc2: too many tiles for 32-bit tile arithmetic");
+  DASR_REQUIRE(p->cin > 0 && p->cin % CHUNK == 0, "conv_tc2: cin must be a multiple of 32 (got %d)", p->cin);
+  if (p->nchunk_list > 0) {
+    DASR_REQUIRE(p->nchunk_list <= 8 && p->nchunk_list * CHUNK == p->cin, "conv_tc2: chunk list must cover cin");
+    for (int i = 0; i < p->nchunk_list; i++)
+      DASR_REQUIRE(p->chunk_off[i] >= 0 && p->chunk_off[i] % 8 == 0 && p->chunk_off[i] + CHUNK <= p->in_cs, "conv_tc2: chunk_off[%d]", i);
+  } else {
+    DASR_REQUIRE(p->in_cs % 8 == 0 && p->in_coff % 8 == 0 && p->in_coff + p->cin <= p->in_cs, "conv_tc2: input slice");
   }
-  // 64-channel A chunks: contiguous input slice whose channel count is a multiple of 64
-  a.chunk64 = (chunk64_ok && p->a_mode == 0 && p->nchunk_list == 0 && p->cin % (2 * CHUNK) == 0) ? 1 : 0;
-  a.nloads = a.chunk64 ? a.nchunks / 2 : a.nchunks;
-  a.a_stage_bytes = (p->a_mode == 0) ? (((a.chunk64 ? 2 : 1) * A_HALO_BYTES + 1023) / 1024 * 1024) : p->ntaps * A_TAP_BYTES;
-  a.acc_stride = (p->epi_mode == 3) ? 64 : pow2_at_least(p->nt);      // mode 3: two M-halves of 32 columns
-  a.nacc = (a.acc_stride <= 128) ? 4 : 2;          // 512 TMEM columns: 4 accumulators up to N = 128, else 2
-  a.tmem_cols = a.nacc * a.acc_stride;
-  if (a.tmem_cols < 32) a.tmem_cols = 32;
-  a.has_pre = (p->epi_mode == 0 && pre) ? 1 : 0;
-  a.has_res1 = (p->epi_mode == 0 && res1) ? 1 : 0;
-  a.has_res2 = (p->epi_mode == 0 && res2) ? 1 : 0;
-  a.epi_bytes = (p->epi_mode == 0) ? p->nt * 128 * 2 : (p->epi_mode == 3 ? 21504 : 0);   // mode 3: 180 halo pixels x 29 floats
-  const int bar_bytes = (2 * MAX_STAGES + 22) * 8 + 256 * 4 + 16;
-  // staged-epilogue buffers: as many (<= 4) as still leave 4 A stages; loads of pre / residual tiles are issued nbuf
-  // tiles ahead, which hides their latency (with 2 the read-modify-write launches are bound by that round trip)
-  int nbuf = (p->epi_mode == 0) ? 4 : (p->epi_mode == 3 ? 1 : 2);
-  int epi_total = 0, avail = 0;
-  for (;; nbuf--) {
-    epi_total = nbuf * a.epi_bytes * (1 + a.has_res1 + a.has_res2);
-    avail = SMEM_LIMIT - 1024 /*alignment slack*/ - a.w_bytes - epi_total - bar_bytes;
-    if (nbuf <= 2 || avail >= 4 * a.a_stage_bytes) break;
-  }
-  a.nbuf = nbuf;
-  int stages = avail / a.a_stage_bytes;
-  if (stages > MAX_STAGES) stages = MAX_STAGES;
-  if (stages < 2) {
-    set_error("conv_tc: resident filters (%d B) + epilogue tiles (%d B) + 2 A stages do not fit shared memory; use a smaller nt",
-              a.w_bytes, epi_total);
+  DASR_REQUIRE(p->out_cs % 8 == 0 && p->out_coff % 8 == 0 && p->out_coff + p->cout <= p->out_cs, "conv_tc2: output slice");
+  DASR_REQUIRE(p->act_cols % 16 == 0, "conv_tc2: act_cols must be a multiple of 16");
+  DASR_REQUIRE(!(res2 && !res1), "conv_tc2: res2 without res1");
+  if (p->mask_c1 > p->mask_c0)
+    DASR_REQUIRE(res1 && !res2 && p->mask_c0 % 16 == 0 && p->mask_c1 % 16 == 0 && p->mask_c1 <= p->cout,
+                 "conv_tc2: mask mode takes the activation as res1 (no res2) and a range of whole 16-channel groups");
+  if (pre) DASR_REQUIRE(p->pre_cs % 8 == 0 && p->pre_coff % 8 == 0 && p->pre_coff + p->cout <= p->pre_cs, "conv_tc2: pre slice");
+  if (res1) DASR_REQUIRE(p->res1_cs % 8 == 0 && p->res1_coff % 8 == 0 && p->res1_coff + p->cout <= p->res1_cs, "conv_tc2: res1 slice");
+  if (res2) DASR_REQUIRE(p->res2_cs % 8 == 0 && p->res2_coff % 8 == 0 && p->res2_coff + p->cout <= p->res2_cs, "conv_tc2: res2 slice");
+  if (!tc2_fits(p, (res1 ? 1 : 0) + (res2 ? 1 : 0))) {
+    set_error("conv_tc2: half filter set + epilogue buffers + 2 A stages do not fit shared memory (nt=%d cin=%d)", p->nt, p->cin);
     return DASR_E_SMEM;
   }
-  a.stages = stages;
-  size_t smem = 1024 + (size_t)a.w_bytes + (size_t)stages * a.a_stage_bytes + epi_total + bar_bytes;
-  // one CTA per SM is assumed by the TMEM allocation (2 x nt columns): make sure two CTAs never co-reside
-  if (smem < 120 * 1024) smem = 120 * 1024;
-
-  CUtensorMap tm_in, tm_w;
-  EpiMaps em;
-  {
-    cuuint64_t gdim[4] = {(cuuint64_t)p->in_cs, (cuuint64_t)p->W, (cuuint64_t)p->H, (cuuint64_t)p->N};
-    cuuint64_t gstr[3] = {(cuuint64_t)p->in_cs * 2, (cuuint64_t)p->W * p->in_cs * 2,
-                          (cuuint64_t)p->H * p->W * p->in_cs * 2};
-    cuuint32_t box[4] = {(cuuint32_t)(a.chunk64 ? 2 * CHUNK : CHUNK), (cuuint32_t)(p->a_mode == 0 ? HALO_W : TILE_W),
-                         (cuuint32_t)(p->a_mode == 0 ? HALO_H : TILE_H), 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    // a 32-channel chunk is 64 B of a wider pixel row: promoting its L2 fills to 128 B doubled the DRAM reads of A
-    // (ncu: dram__bytes_read 311 MB for 234 MB requested by the SMs in a one-chunk launch)
-    CUresult r = enc(&tm_in, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(in), gdim, gstr, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, a.chunk64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                     (p->in_cs > CHUNK && !a.chunk64) ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B : CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-      set_error("conv_tc: cuTensorMapEncodeTiled(input) failed: %d", (int)r);
-      return DASR_E_LAUNCH;
-    }
-  }
-  {
-    cuuint64_t rows = (cuuint64_t)p->nvar * p->ntaps * a.nchunks * p->cout;
-    cuuint64_t gdim[2] = {CHUNK, rows};
-    cuuint64_t gstr[1] = {ROW_B};
-    cuuint32_t box[2] = {CHUNK, (cuuint32_t)p->nt};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(&tm_w, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(w), gdim, gstr, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-      set_error("conv_tc: cuTensorMapEncodeTiled(filter) failed: %d", (int)r);
-      return DASR_E_LAUNCH;
-    }
-  }
-  for (int i = 0; i < 8; i++) em.m[i] = tm_in;   // placeholders when unused
-  if (p->epi_mode == 0) {
-    const void* bases[4] = {out, pre, res1, res2};
-    const int css[4] = {p->out_cs, p->pre_cs, p->res1_cs, p->res2_cs};
-    const int used[4] = {1, a.has_pre, a.has_res1, a.has_res2};
-    const char* names[4] = {"output", "pre", "res1", "res2"};
-    if (p->out_mul == 2) {
-      // one output map pair per parity variant (slots 2v, 2v + 1; no pre / residual maps in this mode)
-      for (int v = 0; v < p->nvar && v < 4; v++) {
-        const char* vb = (const char*)out + ((size_t)p->out_py[v] * (2 * p->W) + p->out_px[v]) * p->out_cs * 2;
-        int rc;
-        if (p->nt >= 64 && (rc = encode_act_map(enc, &em.m[2 * v], vb, p->out_cs, p->W, p->H, p->N, 64, "output", 2))) return rc;
-        if ((p->nt & 32) && (rc = encode_act_map(enc, &em.m[2 * v + 1], vb, p->out_cs, p->W, p->H, p->N, 32, "output", 2))) return rc;
-      }
-    } else
-    for (int t = 0; t < 4; t++) {
-      if (!used[t]) continue;
-      int rc;
-      if (p->nt >= 64 && (rc = encode_act_map(enc, &em.m[2 * t], bases[t], css[t], p->W, p->H, p->N, 64, names[t]))) return rc;
-      if ((p->nt & 32) && (rc = encode_act_map(enc, &em.m[2 * t + 1], bases[t], css[t], p->W, p->H, p->N, 32, names[t]))) return rc;
-    }
-  }
-
-  typedef void (*KernelFn)(const CUtensorMap, const CUtensorMap, const EpiMaps, const TcKernelArgs);
-  static const KernelFn kernels[9] = {
-      conv_tc_kernel<0, false, 0>, conv_tc_kernel<0, false, 1>, conv_tc_kernel<0, false, 2>,
-      conv_tc_kernel<0, true, 0>,  conv_tc_kernel<0, true, 1>,  conv_tc_kernel<0, true, 2>,
-      conv_tc_kernel<1, false, 0>, conv_tc_kernel<2, false, 0>, conv_tc_kernel<3, false, 0>};
-  const int ki = (p->epi_mode == 0) ? (a.has_pre * 3 + a.has_res1 + a.has_res2) : (5 + p->epi_mode);
-  if (p->epi_mode == 0) DASR_REQUIRE(!(a.has_res2 && !a.has_res1), "conv_tc: res2 without res1");
-  static bool attr_set[9] = {false, false, false, false, false, false, false, false, false};
-  if (!attr_set[ki]) {
-    cudaError_t e = cudaFuncSetAttribute(kernels[ki], cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
-    if (e != cudaSuccess) {
-      set_error("conv_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-      return DASR_E_LAUNCH;
-    }
-    attr_set[ki] = true;
-  }
-  int gy = p->nvar * a.n_ntiles;
-  int gx = num_sms() / gy;
-  if (gx < 1) gx = 1;
-  if ((long)gx > a.ntiles) gx = (int)a.ntiles;
-  // programmatic dependent launch: this kernel's prologue (barrier init, TMEM allocation, resident filter load) may run
-  // while the previous kernel of the stream drains; every global access that depends on it sits behind griddepcontrol.wait
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(gx, gy, 1);
-  cfg.blockDim = dim3(TCK_THREADS, 1, 1);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = (cudaStream_t)stream;
-  cudaLaunchAttribute attrs[1];
-  attrs[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attrs[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-  cfg.attrs = attrs;
-  cfg.numAttrs = 1;
-  cudaError_t le = cudaLaunchKernelEx(&cfg, kernels[ki], tm_in, tm_w, em, a);
-  if (le != cudaSuccess) {
-    set_error("conv_tc: launch failed: %s", cudaGetErrorString(le));
-    return DASR_E_LAUNCH;
-  }
-  return check_launch("conv_tc");
+  DasrConvTcParams q = *p;
+  q.nt = p->nt / 2;                     // per CTA; grid.y = cout / (nt / 2), consecutive CTAs form the clusters
+  return conv_tc_launch(in, w, bias, pre, res1, res2, nullptr, out, &q, stream, 1);
 }
 
 // selftest-only probe (declared in selftest.cu, not in the public header)
-int dasr_probe_mma_rate(int n, int sbo, int iters, int a_step, double* cycles_per_mma) {
-  long long* d;
-  if (cudaMalloc(&d, 8) != cudaSuccess) return DASR_E_LAUNCH;
-  cudaFuncSetAttribute(mma_rate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024);
-  mma_rate_kernel<<<num_sms(), 128, 64 * 1024>>>(n, sbo, iters, a_step, d);
-  long long h = 0;
-  cudaError_t e = cudaMemcpy(&h, d, 8, cudaMemcpyDeviceToHost);
-  cudaFree(d);
-  if (e != cudaSuccess) { set_error("probe: %s", cudaGetErrorString(e)); return DASR_E_LAUNCH; }
-  *cycles_per_mma = (double)h / ((double)iters * 18.0);
-  return DASR_OK;
-}
-
-
 int dasr_probe_tma_rate(int row_elems, int rows_per_box, int cs, int store, double* cycles_per_box) {
   PFN_encodeTiled enc = get_encode();
   if (!enc) return DASR_E_NODRIVER;

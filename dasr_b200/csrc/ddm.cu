@@ -1,5 +1,5 @@
 // Domain-distance map (DDM): per-pixel average of the discriminator's patch scores over the receptive fields that cover
-// the pixel — sm_100a, fp64, HBM-bound (two separable gather passes, no atomics).
+// the pixel — sm_90a, fp64, HBM-bound (two separable gather passes, no atomics).
 //
 // Replaces (reference, codes/DSN): receptive_cal.py:34-43 `weights_matrix` (a numpy double loop that scatter-adds every
 // patch score into its receptive-field window) and :55-60 `getWeights` (sum / count), called by

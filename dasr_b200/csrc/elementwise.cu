@@ -959,7 +959,7 @@ int dasr_log_loss(const float* x, int one_minus, float eps, float* loss, float* 
 int dasr_prelu_fwd(const float* z, const float* slope, float* y, long n, void* stream) {
   DASR_REQUIRE(z && slope && y && n > 0, "prelu_fwd: bad arguments");
   int blocks = (int)((n + 1023) / 1024);
-  if (blocks > 4 * 148) blocks = 4 * 148;
+  if (blocks > 4 * num_sms()) blocks = 4 * num_sms();
   prelu_fwd_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(z, slope, y, n);
   return check_launch("prelu_fwd");
 }
@@ -977,7 +977,7 @@ int dasr_prelu_fwd_bf16(const void* z, const float* slope, void* y, long n, void
   DASR_REQUIRE(z && slope && y && n > 0 && n % 8 == 0, "prelu_fwd_bf16: n must be a multiple of 8");
   long n8 = n / 8;
   int blocks = (int)((n8 + 255) / 256);
-  if (blocks > 8 * 148) blocks = 8 * 148;
+  if (blocks > 8 * num_sms()) blocks = 8 * num_sms();
   prelu_fwd_bf16x8_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>((const uint4*)z, slope, (uint4*)y, n8);
   return check_launch("prelu_fwd_bf16");
 }
@@ -996,21 +996,21 @@ int dasr_cast_bf16_f32(const void* src, void* dst, long n, int to_bf16, void* st
   DASR_REQUIRE(src && dst && n > 0 && n % 8 == 0, "cast: n must be a multiple of 8");
   long n8 = n / 8;
   int blocks = (int)((n8 + 255) / 256);
-  if (blocks > 8 * 148) blocks = 8 * 148;
+  if (blocks > 8 * num_sms()) blocks = 8 * num_sms();
   cast_bf16_f32_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(src, dst, n8, to_bf16);
   return check_launch("cast");
 }
 int dasr_sigmoid_fwd(const float* x, float* y, long n, void* stream) {
   DASR_REQUIRE(x && y && n > 0, "sigmoid_fwd: bad arguments");
   int blocks = (int)((n + 1023) / 1024);
-  if (blocks > 4 * 148) blocks = 4 * 148;
+  if (blocks > 4 * num_sms()) blocks = 4 * num_sms();
   sigmoid_fwd_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(x, y, n);
   return check_launch("sigmoid_fwd");
 }
 int dasr_sigmoid_bwd(const float* y, const float* dy, float* dx, long n, void* stream) {
   DASR_REQUIRE(y && dy && dx && n > 0, "sigmoid_bwd: bad arguments");
   int blocks = (int)((n + 1023) / 1024);
-  if (blocks > 4 * 148) blocks = 4 * 148;
+  if (blocks > 4 * num_sms()) blocks = 4 * num_sms();
   sigmoid_bwd_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(y, dy, dx, n);
   return check_launch("sigmoid_bwd");
 }

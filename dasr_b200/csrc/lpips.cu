@@ -1,4 +1,4 @@
-// LPIPS (learned perceptual metric, AlexNet trunk) support kernels — sm_100a, fp32 NHWC, HBM-bound.
+// LPIPS (learned perceptual metric, AlexNet trunk) support kernels — sm_90a, fp32 NHWC, HBM-bound.
 //
 // Replaces (reference, codes/PerceptualSimilarity): nn.MaxPool2d(3, 2) of torchvision's alexnet.features
 // (models/pretrained_networks.py:57-96), util.normalize_tensor (util/util.py: x / (sqrt(sum_c x^2) + 1e-10)),

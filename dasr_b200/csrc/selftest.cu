@@ -1,7 +1,7 @@
 // Standalone GPU self-test / micro-benchmark of the C-ABI library (no Python, no torch).
 // Usage: selftest [check] [bench]      (default: both)
 // `check` compares every conv kernel with a CPU double-precision loop nest on small shapes;
-// `bench` times the RRDB-shaped tcgen05 convs at BASELINE config 2 size (16 x 256 x 256).
+// `bench` times the RRDB-shaped tensor-core convs at BASELINE config 2 size (16 x 256 x 256).
 // Test infrastructure only — nothing here is on the product path.
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -22,9 +22,7 @@
     }                                                                              \
   } while (0)
 
-extern "C" int dasr_probe_mma_rate(int n, int sbo, int iters, int a_step, double* cycles_per_mma);
 extern "C" int dasr_probe_tma_rate(int row_elems, int rows_per_box, int cs, int store, double* cycles_per_box);
-extern "C" int dasr_probe_mma2_rate(int n, int iters, double* cycles_per_mma);
 static unsigned long long rng_state = 0x1234567ULL;
 static inline unsigned rnd() {
   rng_state = rng_state * 6364136223846793005ULL + 1442695040888963407ULL;
@@ -193,7 +191,7 @@ static inline float h16_to_float(__nv_bfloat16 x) {
   return __half2float(h);
 }
 
-// tcgen05 conv vs CPU reference. kind 0 fprop, 1 dgrad, 2 upsample-fused
+// tensor-core (wgmma) conv vs CPU reference. kind 0 fprop, 1 dgrad, 2 upsample-fused
 // epi: 0 none, 1 = act+res1+mask (direct-store epilogue), 2 = staged epilogue with pre + act_cols + res1 + res2, 3 = NCHW fp32 out
 static void test_tc(int N, int H, int W, int cin, int cout, int nt, int kind, int a_mode, int epi) {
   char name[200];
@@ -243,14 +241,14 @@ static void test_tc(int N, int H, int W, int cin, int cout, int nt, int kind, in
       if (c < act_cols) v = v > 0 ? v : v * slope;
       ref[i] = alpha * v + beta1 * res1[i] + beta2 * res1[(i + gn) % ref.size()];
     }
-  if (epi == 7)      // CTA-pair dgrad form: acc + bias + pre, then the LeakyReLU-backward gate on the last 32 channels
+  if (epi == 7)      // cluster-pair dgrad form: acc + bias + pre, then the LeakyReLU-backward gate on the last 32 channels
     for (size_t i = 0; i < ref.size(); i++) {
       int c = (int)(i % gn);
       double v = ref[i] + msk[i];
       if (c >= gn - 32 && !(res1[i] > 0.f)) v *= mslope;
       ref[i] = v;
     }
-  if (epi == 4)      // CTA-pair kernel: bias + LeakyReLU on the first act_cols channels + scale, no pre / residual tiles
+  if (epi == 4)      // cluster pair: bias + LeakyReLU on the first act_cols channels + scale, no pre / residual tiles
     for (size_t i = 0; i < ref.size(); i++) {
       int c = (int)(i % gn);
       double v = ref[i];
@@ -311,7 +309,7 @@ static void test_tc(int N, int H, int W, int cin, int cout, int nt, int kind, in
     rc |= dasr_conv_tc2(din, dwp, db, dmsk, dres, nullptr, dout, &p, 0);
   } else if (epi == 4)
     rc |= dasr_conv_tc2(din, dwp, db, nullptr, nullptr, nullptr, dout, &p, 0);
-  else if (epi == 5)      // CTA-pair kernel with the full staged-epilogue contract of epi 2
+  else if (epi == 5)      // cluster pair with the full staged-epilogue contract of epi 2
     rc |= dasr_conv_tc2(din, dwp, db, dmsk, gn <= 96 ? dres : nullptr, dres2, dout, &p, 0);
   else
     rc |= dasr_conv_tc(din, dwp, db, epi == 2 ? dmsk : nullptr, (epi == 1 || (epi == 2 && gn <= 96)) ? dres : nullptr, dres2,
@@ -451,7 +449,7 @@ static void bench_tc(int N, int H, int W, int cin, int cout, int nt, int kind, i
 // partial sums accumulated IN PLACE (pre == out), activation on the first 32 channels only.
 // in_cs / out_cs = 0: both operands are channel slices of ONE 256-channel buffer (the dense-block layout of the engine);
 // otherwise the input is a dense [N,H,W,in_cs] tensor and the output / partial-sum tile a dense [N,H,W,out_cs] tensor
-// (what a slab-planar activation layout would look like to the kernel).  pair = 1: CTA-pair kernel (dasr_conv_tc2).
+// (what a slab-planar activation layout would look like to the kernel).  pair = 1: cluster pair (dasr_conv_tc2).
 static void bench_tc_fused(int N, int H, int W, int cin, int cout, int nt, int with_pre, int iters, int in_cs = 0, int out_cs = 0,
                            int pair = 0) {
   const int cs = 256;
@@ -543,30 +541,6 @@ int main(int argc, char** argv) {
           }
       return 0;
     }
-    if (!strcmp(argv[i], "mmarate")) {
-      int ns[] = {32, 64, 96, 128, 192, 256};
-      // latency of a dependent accumulate chain (wait after every 18 MMAs, one accumulator) vs throughput (no waits), and
-      // 1 / 2 / 4 independent accumulators the MMAs rotate over
-      for (int nowait = 0; nowait <= 1; nowait++)
-        for (int nacc : {1, 2, 4})
-          for (int n : ns) {
-            if (n * nacc > 512) continue;
-            double c = 0;
-            int rc = dasr_probe_mma_rate(n, 640, 200, 64 | (nacc << 16) | (nowait << 20), &c);
-            printf("mma_rate M128 N%-3d K16 accumulators=%d %s : %7.1f cycles/MMA  (N/2=%d) rc=%d\n", n, nacc,
-                   nowait ? "back-to-back" : "wait/18     ", c, n / 2, rc);
-          }
-      return 0;
-    }
-    if (!strcmp(argv[i], "mma2rate")) {     // cta_group::2: M=256 per instruction, two pixel tiles
-      for (int n : {64, 96, 128, 160, 192, 256}) {
-        double c = 0;
-        int rc = dasr_probe_mma2_rate(n, 200, &c);
-        printf("mma2_rate M256 N%-3d K16 cta_group::2 back-to-back : %7.1f cycles/MMA  (%.1f per 128-pixel tile) rc=%d %s\n", n, c, c / 2,
-               rc, rc ? dasr_last_error() : "");
-      }
-      return 0;
-    }
     if (!strcmp(argv[i], "fused")) {
       bench_tc_fused(16, 256, 256, 64, 192, 96, 0, 10);
       bench_tc_fused(16, 256, 256, 32, 160, 160, 1, 10);
@@ -587,7 +561,7 @@ int main(int argc, char** argv) {
       bench_tc_fused(16, 256, 256, 64, 64, 64, 1, 10, 64, 64);
       bench_tc_fused(16, 256, 256, 32, 128, 128, 1, 10, 32, 128);
       bench_tc_fused(16, 256, 256, 64, 192, 96, 0, 10, 64, 192);
-      // CTA-pair kernel: dense-block launch 1
+      // cluster pair: dense-block launch 1
       bench_tc_fused(16, 256, 256, 64, 192, 192, 0, 10, 0, 0, 1);
       bench_tc_fused(16, 256, 256, 64, 192, 192, 0, 10, 64, 192, 1);
       bench_tc_fused(16, 256, 256, 32, 128, 128, 0, 10, 0, 0, 1);
@@ -635,7 +609,7 @@ int main(int argc, char** argv) {
     test_wgrad_tc(3, 32, 24, 160, 32);
     test_wgrad_tc(2, 32, 16, 192, 64);
     test_wgrad_tc(1, 48, 40, 64, 64);
-    // tcgen05: validation path first (one aligned tile per tap), then shifted-descriptor halo path
+    // tensor-core conv: validation path first (one aligned tile per tap), then shifted-descriptor halo path
     for (int am = 1; am >= 0; am--) {
       test_tc(1, 16, 8, 32, 32, 32, 0, am, 0);
       test_tc(2, 32, 32, 64, 32, 32, 0, am, 0);
@@ -654,15 +628,15 @@ int main(int argc, char** argv) {
       }
       test_tc(1, 24, 24, 160, 32, 160, 1, am, 1);      // dgrad conv4-like: K=32 -> N=160
       test_tc(1, 16, 16, 192, 64, 96, 1, am, 0);       // dgrad conv5-like: K=64 -> N=192 split 2x96
-      if (am == 0) {                                   // CTA-pair kernel (cta_group::2): dense-block launch 1 and conv5's dgrad
-        test_tc(1, 16, 8, 64, 192, 192, 0, 0, 4);      // one tile: odd tail (the peer CTA runs an empty tile)
+      if (am == 0) {                                   // cluster-pair launch (dasr_conv_tc2): dense-block launch 1 and conv5's dgrad
+        test_tc(1, 16, 8, 64, 192, 192, 0, 0, 4);      // one tile: both CTAs of the cluster take it (one Cout half each)
         test_tc(1, 19, 11, 64, 192, 192, 0, 0, 4);     // ragged, 4 tiles
         test_tc(2, 32, 16, 64, 192, 192, 0, 0, 4);
-        test_tc(4, 96, 64, 64, 192, 192, 0, 0, 4);     // 192 tiles: pairs take a second iteration, ring wrap-around
+        test_tc(4, 96, 64, 64, 192, 192, 0, 0, 4);     // 192 tiles: several tiles per cluster, A-stage ring wrap-around
         test_tc(1, 24, 16, 32, 128, 128, 0, 0, 4);     // one chunk, two 64-channel blocks
         test_tc(1, 16, 16, 192, 64, 192, 1, 0, 4);     // dgrad conv5-like: K=64 -> N=192
-        test_tc(1, 20, 13, 96, 64, 64, 0, 0, 5);       // pair kernel, staged epilogue with pre + res1 + res2, ragged, 3 chunks
-        test_tc(3, 48, 40, 64, 64, 64, 0, 0, 5);       // several iterations per pair (ring wrap with loads)
+        test_tc(1, 20, 13, 96, 64, 64, 0, 0, 5);       // cluster pair, staged epilogue with pre + res1 + res2, ragged, 3 chunks
+        test_tc(3, 48, 40, 64, 64, 64, 0, 0, 5);       // several tiles per cluster (epilogue ring wrap with loads)
         test_tc(2, 40, 24, 32, 128, 128, 0, 0, 5);     // pre only, two blocks per tile
         test_tc(1, 32, 24, 64, 192, 192, 0, 0, 5);     // pre only, three blocks per tile
         test_tc(4, 96, 64, 32, 64, 64, 0, 0, 5);       // 192 tiles, pre + two residuals

@@ -1,8 +1,9 @@
-// tcgen05 / TMA / mbarrier PTX wrappers and tile constants shared by the tensor-core kernels (sm_100a).
+// wgmma / TMA / mbarrier PTX wrappers and tile constants shared by the tensor-core kernels (sm_90a).
 #pragma once
 #include <cuda.h>
 #include "common.cuh"
 #include <cuda_fp16.h>
+#include "wgmma.cuh"
 
 namespace dasr {
 
@@ -12,7 +13,6 @@ constexpr int CHUNK = 32;                      // channels per K chunk (64 B row
 constexpr int ROW_B = CHUNK * 2;               // 64
 constexpr int A_HALO_BYTES = HALO_H * HALO_W * ROW_B;   // 11520
 constexpr int A_TAP_BYTES = TILE_H * TILE_W * ROW_B;    // 8192 (a_mode 1: one aligned tile per tap)
-constexpr int TC_THREADS = 352;   // warp 0 A/B TMA, warp 1 MMA, warps 2..9 epilogue (two warpgroups), warp 10 epilogue TMA
 constexpr int MAX_STAGES = 8;
 constexpr int SMEM_LIMIT = 226 * 1024;  // 227 KB opt-in max minus the kernel's 1 KB static allocation
 
@@ -65,17 +65,6 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(
@@ -86,26 +75,30 @@ __device__ __forceinline__ bool elect_one() {
   return pred != 0;
 }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::f16 (bf16 in, fp32 accumulate)
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
+// ---- warpgroup MMA (wgmma) synchronisation ----
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across a wgmma fence or wait
+template <int R>
+__device__ __forceinline__ void fence_regs(float* d) {
+#pragma unroll
+  for (int i = 0; i < R; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
-// all previously issued MMAs of this thread arrive on `bar` when complete (implies fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// ---- CTA-pair (cta_group::2) forms: two SMs of a TPC execute one M=256 MMA; each CTA holds 128 rows of A and half of
-// the N rows of B in its own shared memory, and gets its 128 x N accumulator rows in its own TMEM.  The leader CTA
-// (cluster rank 0) issues; barriers are signalled across the pair through shared::cluster addresses. ----
-constexpr uint32_t PEER_BIT_MASK = 0xFEFFFFFFu;   // shared::cluster address of the SAME offset in the even (leader) CTA
 
+// sm_90 shared-memory matrix descriptor: [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [62,64) layout
+// (1 = SWIZZLE_128B, 2 = SWIZZLE_64B).  K-major swizzled operands ignore LBO (1); MN-major ones use it as the stride
+// between swizzle-width groups of the M / N index.  The swizzle is a function of the shared-memory address bits, as it is
+// for the TMA writes, so a start address shifted by whole 64 B / 128 B rows (a conv tap) reads the tile TMA wrote.
+constexpr uint64_t DESC_SW128 = (uint64_t)1 << 62;
+constexpr uint64_t DESC_SW64 = (uint64_t)2 << 62;
+__device__ __forceinline__ uint64_t desc_hi(uint32_t lbo, uint32_t sbo, uint64_t layout) {
+  return ((uint64_t)((lbo >> 4) & 0x3FFF) << 16) | ((uint64_t)((sbo >> 4) & 0x3FFF) << 32) | layout;
+}
+__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint64_t hi) { return hi | (uint64_t)((smem_addr >> 4) & 0x3FFF); }
+
+// ---- thread-block clusters ----
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -114,98 +107,24 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
 __device__ __forceinline__ void cluster_sync() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-__device__ __forceinline__ void tmem_alloc2(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
+// arrive on the barrier at the same shared-memory offset in cluster CTA `rank`
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
+  uint32_t remote;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(rank));
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
 }
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma2_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                           uint32_t accumulate) {
+// TMA load written to the same shared-memory offset of every CTA in `mask`; each destination's barrier at `bar`'s offset
+// receives the bytes it got
+__device__ __forceinline__ void tma_load_4d_mc(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2,
+                                               int c3, uint16_t mask) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// all MMAs issued so far by this thread arrive (once) on the barrier at this shared-memory offset in BOTH CTAs of the pair
-__device__ __forceinline__ void umma2_commit_mc(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(smem_u32(bar)), "h"((uint16_t)3)
-      : "memory");
-}
-// arrive on the LEADER CTA's copy of a barrier (from either CTA)
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & PEER_BIT_MASK) : "memory");
-}
-// TMA load into THIS CTA's shared memory whose transaction bytes complete on the LEADER CTA's barrier
-__device__ __forceinline__ void tma2_load_4d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar) & PEER_BIT_MASK), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tma2_load_2d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar) & PEER_BIT_MASK), "r"(c0), "r"(c1)
+      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4, %5, %6}], [%2], %7;"
+      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "h"(mask)
       : "memory");
 }
 // programmatic dependent launch: wait for the prerequisite grid's memory / let the dependent grid start its prologue
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp gets row (lane base + i), columns c..c+31
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// K-major, SWIZZLE_64B shared-memory operand descriptor (cute::UMMA::SmemDescriptor bit layout):
-//   [0,14) start>>4 | [16,30) LBO>>4 (unused for swizzled K-major, 1) | [32,46) SBO>>4 |
-//   [46,48) version=1 (sm_100) | [49,52) base offset=0 | [61,64) layout type (4 = SWIZZLE_64B)
-__device__ __forceinline__ uint64_t make_desc_sw64(uint32_t smem_addr, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)4 << 61;
-  return d;
-}
-// cute::UMMA::InstrDescriptor: c_format F32 (1) @4, a/b format BF16 (1) @7/@10, K-major both,
-// n_dim = N>>3 @17, m_dim = M>>4 @24
-__host__ __device__ inline uint32_t make_idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// same with the 16-bit operand type selectable: f16 != 0 -> a/b format F16 (0) (IEEE half operands, fp32 accumulate:
-// three more mantissa bits than bf16 at the same tensor-core rate)
-__host__ __device__ inline uint32_t make_idesc_16(int M, int N, int f16) {
-  const uint32_t fmt = f16 ? 0u : 1u;
-  return (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
 
 // TMA store / bulk-group helpers (epilogue)
 __device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, const void* src, int c0, int c1, int c2, int c3) {

@@ -1,20 +1,19 @@
 // Filter gradients of ALL FIVE convs of a ResidualDenseBlock_5C (reference: autograd of block.py:262-278) in one
-// tcgen05 launch + one reduction.
+// wgmma launch + one reduction (sm_90a).
 //
-// dasr_conv3x3_wgrad_tc handles one conv per launch with N = 32 output channels per MMA (a tcgen05.mma costs ~72 cycles
-// for any N <= 96) and only 512 pixel tiles per launch at the training shape, i.e. 3.5 tiles per CTA before each CTA
-// writes a 147 KB partial.  Here the five gradients are one block-triangular GEMM per tap,
+// dasr_conv3x3_wgrad_tc handles one conv per launch and only 512 pixel tiles per launch at the training shape, i.e. ~4
+// tiles per CTA before each CTA writes a 147 KB partial.  Here the five gradients are one block-triangular GEMM per tap,
 //     dW[tap][ci 0:192][col 0:192] = sum_p X[p + tap][ci] * dY[p][col],   cols = [g1 g2 g3 g4 | g5 (64)],
-// of which conv k needs rows ci < 64 + 32 (k - 1).  It is cut into 7 jobs, each a (row tile, column range, tap range)
-// whose accumulators fit TMEM (taps x columns <= 512):
-//     rows   0:128 x cols g1..g4 (N = 128) x taps {0-2}, {3-5}, {6-8}
-//     rows   0:128 x cols g5     (N =  64) x taps {0-4}, {5-8}
-//     rows 128:192 x cols g4, g5 (N =  96) x taps {0-4}, {5-8}
-// The 148 CTAs are divided among the jobs in proportion to their per-tile cost (max of MMA time and the ~32 B/clk
-// shared-memory ingest of the tiles); a CTA walks every nsplit-th pixel tile of its job and writes ONE partial.
+// of which conv k needs rows ci < 64 + 32 (k - 1).  It is cut into 11 jobs, each a (row tile, column range, tap range)
+// whose accumulators fit the registers of the two consumer warpgroups (<= 128 fp32 per thread):
+//     rows   0:128 x cols g1..g4 (N = 128) x taps {0-1}, {2-3}, {4-5}, {6-7}, {8}
+//     rows   0:128 x cols g5     (N =  64) x taps {0-3}, {4-7}, {8}
+//     rows 128:192 x cols g4, g5 (N =  96) x taps {0-3}, {4-7}, {8}   (64 rows: the warpgroups split the taps)
+// The CTAs are divided among the jobs in proportion to their per-tile cost (MMA work + shared-memory ingest of the
+// tiles); a CTA walks every nsplit-th pixel tile of its job and writes ONE partial.
 // Operands are the MN-major tiles of wgrad_tc.cu: X = (16+2)x(8+2) halo tiles of up to four 32-channel chunks
-// (LBO = chunk slot stride, SBO = 640 B, a tap is a start-address shift), dY = 16x8 tiles of up to six 32-channel
-// groups (LBO = 8 KB, SBO = 512 B).
+// (LBO = chunk slot stride, SBO = 640 B, a tap is a start-address shift), dY = 16x8 tiles of up to four 32-channel
+// groups (one N = 32 wgmma each, SBO = 512 B).
 #include <string.h>
 #include "tc_common.cuh"
 
@@ -26,9 +25,9 @@ constexpr int B_GROUP = TILE_H * TILE_W * ROW_B;    // 8192: one 32-channel dY t
 constexpr int MAX_COLG = 4;                         // column groups per job (N <= 128)
 constexpr int STAGE_BYTES = 4 * A_SLOT + MAX_COLG * B_GROUP;   // 81920
 constexpr int STAGES = 2;
-constexpr int THREADS = 192;                        // warp 0 TMA, warp 1 MMA, warps 2..5 epilogue
+constexpr int THREADS = 288;                        // warps 0..7 two consumer warpgroups, warp 8 TMA
 constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + 256;
-constexpr int MAX_JOBS = 8;
+constexpr int MAX_JOBS = 12;
 
 struct Job {
   int nchunk;               // 32-channel X chunks (rows = 32 * nchunk <= 128)
@@ -57,9 +56,76 @@ struct Lut {
   int cin[5], cout[5];
 };
 
-__device__ __forceinline__ uint64_t desc_mn_sw64(uint32_t addr, uint32_t lbo, uint32_t sbo) {
-  return (uint64_t)((addr >> 4) & 0x3FFF) | ((uint64_t)((lbo >> 4) & 0x3FFF) << 16) | ((uint64_t)((sbo >> 4) & 0x3FFF) << 32) |
-         ((uint64_t)1 << 46) | ((uint64_t)4 << 61);
+// Consumer warpgroup g of a job with NG column groups: 128-row jobs give warpgroup g rows 64g..64g+63 and every tap;
+// 64-row jobs give both warpgroups all rows and split the taps (local taps g, g + 2, ...).  At most MAXU taps each.
+template <int MAXU, int NG>
+__device__ __forceinline__ void rdb_consume(const Job& jb, int split, const Args& a, uint8_t* smem, uint64_t* full_bar,
+                                            uint64_t* empty_bar, int warp, int lane) {
+  const int g = warp >> 2;
+  const bool half_rows = jb.nchunk == 2;
+  const int u0 = half_rows ? g : 0, ustep = half_rows ? 2 : 1;     // local taps u0, u0 + ustep, ...
+  const int nu = (jb.ntap - u0 + ustep - 1) / ustep;
+  const uint32_t row_off = half_rows ? 0u : 2u * g * A_SLOT;
+  const uint64_t a_hi = desc_hi(A_SLOT, HALO_W * ROW_B, DESC_SW64);
+  const uint64_t b_hi = desc_hi(B_GROUP, TILE_W * ROW_B, DESC_SW64);
+  float acc[MAXU][NG][16];
+  int stage = 0;
+  uint32_t phase = 0;
+  int prev = -1;
+  bool first = true;
+  for (int tile = split; tile < a.ntiles; tile += jb.nsplit) {
+    mbar_wait(&full_bar[stage], phase);
+    const uint32_t a0 = smem_u32(smem + stage * STAGE_BYTES) + row_off;
+    const uint32_t b0 = smem_u32(smem + stage * STAGE_BYTES) + 4u * A_SLOT;
+    wgmma_fence();
+#pragma unroll
+    for (int u = 0; u < MAXU; u++) {
+      if (u < nu) {
+        const int tap = jb.tap0 + u0 + u * ustep;
+        const uint32_t at = a0 + (uint32_t)(((tap / 3) * HALO_W + (tap % 3)) * ROW_B);
+#pragma unroll
+        for (int ks = 0; ks < 8; ks++)            // 16 pixels (two tile rows) per MMA
+#pragma unroll
+          for (int c = 0; c < NG; c++)
+            wgmma<32, 0, 1>(acc[u][c], make_desc(at + ks * 2 * HALO_W * ROW_B, a_hi),
+                            make_desc(b0 + c * B_GROUP + ks * 2 * TILE_W * ROW_B, b_hi), (first && ks == 0) ? 0 : 1);
+      }
+    }
+    wgmma_commit();
+    if (prev >= 0) {
+      wgmma_wait<1>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+    }
+    prev = stage;
+    first = false;
+    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+  }
+  wgmma_wait<0>();
+#pragma unroll
+  for (int u = 0; u < MAXU; u++)
+#pragma unroll
+    for (int c = 0; c < NG; c++) fence_regs<16>(acc[u][c]);
+  // epilogue (once): rows 16 * (warp & 3) + lane / 4 (+ 8) of this warpgroup's 64, columns 8j + 2 * (lane & 3) (+ 1)
+  const int rows = 32 * jb.nchunk, ncol = 32 * NG;
+  float* dst = a.part + jb.part_off + (size_t)split * jb.ntap * rows * ncol;
+  const int cq = 2 * (lane & 3);
+#pragma unroll
+  for (int u = 0; u < MAXU; u++) {
+    if (u >= nu) break;
+    const int t = u0 + u * ustep;
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      const int row = (half_rows ? 0 : 64 * g) + 16 * (warp & 3) + (lane >> 2) + 8 * h;
+#pragma unroll
+      for (int c = 0; c < NG; c++)
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+          const float2 v = first ? make_float2(0.f, 0.f) : make_float2(acc[u][c][4 * j + 2 * h], acc[u][c][4 * j + 2 * h + 1]);
+          *reinterpret_cast<float2*>(dst + ((size_t)t * rows + row) * ncol + c * 32 + 8 * j + cq) = v;
+        }
+    }
+  }
 }
 
 __global__ void __launch_bounds__(THREADS, 1)
@@ -70,8 +136,6 @@ wgrad_rdb_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
-  uint64_t* done_bar = bars + 2 * STAGES;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   int ji = 0;
@@ -79,26 +143,20 @@ wgrad_rdb_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
     if ((int)blockIdx.x >= a.job[j].cta0) ji = j;
   const Job& jb = a.job[ji];
   const int split = (int)blockIdx.x - jb.cta0;
-  const int ncol = 32 * jb.ncolg;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tm_x);
     tma_prefetch_desc(&tm_ga);
     tma_prefetch_desc(&tm_gb);
-    for (int s = 0; s < STAGES; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(done_bar, 1);
+    for (int s = 0; s < STAGES; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_ptr, 512u);
-  // chunk slots a job never loads are still read by the M = 128 MMAs (rows that are never written out): keep them finite
+  // chunk slots a job never loads are still read by the M = 64 wgmmas (rows that are never written out): keep them finite
   for (int i = threadIdx.x; i < STAGES * STAGE_BYTES / 16; i += THREADS) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
   fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -114,67 +172,12 @@ wgrad_rdb_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    // D fp32, A/B bf16, both operands MN-major, M = 128, N = ncol
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(ncol >> 3) << 17) | ((128u >> 4) << 24);
-    int stage = 0;
-    uint32_t phase = 0;
-    bool first = true;
-    for (int tile = split; tile < a.ntiles; tile += jb.nsplit) {
-      mbar_wait(&full_bar[stage], phase);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t a0 = smem_u32(smem + stage * STAGE_BYTES);
-        const uint32_t b0 = a0 + 4 * A_SLOT;
-#pragma unroll 1
-        for (int t = 0; t < jb.ntap; t++) {
-          const int tap = jb.tap0 + t;
-          const uint32_t at = a0 + (uint32_t)(((tap / 3) * HALO_W + (tap % 3)) * ROW_B);
-          const uint32_t d = tmem_base + (uint32_t)(t * ncol);
-#pragma unroll
-          for (int ks = 0; ks < 8; ks++) {          // 16 pixels (two tile rows) per MMA
-            const uint64_t da = desc_mn_sw64(at + ks * 2 * HALO_W * ROW_B, A_SLOT, HALO_W * ROW_B);
-            const uint64_t db = desc_mn_sw64(b0 + ks * 2 * TILE_W * ROW_B, B_GROUP, TILE_W * ROW_B);
-            umma_bf16(d, da, db, idesc, (uint32_t)!(first && ks == 0));
-          }
-        }
-        umma_commit(&empty_bar[stage]);
-      }
-      __syncwarp();
-      first = false;
-      if (++stage == STAGES) { stage = 0; phase ^= 1; }
-    }
-    if (elect_one()) umma_commit(done_bar);
-    __syncwarp();
+  } else if (jb.ncolg == 4) {
+    rdb_consume<2, 4>(jb, split, a, smem, full_bar, empty_bar, warp, lane);
+  } else if (jb.ncolg == 2) {
+    rdb_consume<4, 2>(jb, split, a, smem, full_bar, empty_bar, warp, lane);
   } else {
-    // epilogue (once): lane = X channel (row) of this job
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    const int rows = 32 * jb.nchunk;
-    mbar_wait(done_bar, 0);
-    tc_fence_after();
-    const bool any = split < a.ntiles;
-    float* dst = a.part + jb.part_off + (size_t)split * jb.ntap * rows * ncol;
-    for (int t = 0; t < jb.ntap; t++)
-      for (int g = 0; g < jb.ncolg; g++) {
-        uint32_t rr[32];
-        tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(t * ncol + g * 32), rr);
-        tmem_ld_wait();
-        if (row < rows) {
-          float4* o = reinterpret_cast<float4*>(dst + ((size_t)t * rows + row) * ncol + g * 32);
-#pragma unroll
-          for (int j = 0; j < 8; j++)
-            o[j] = any ? make_float4(__uint_as_float(rr[4 * j]), __uint_as_float(rr[4 * j + 1]), __uint_as_float(rr[4 * j + 2]),
-                                     __uint_as_float(rr[4 * j + 3]))
-                       : make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-      }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512u);
+    rdb_consume<2, 3>(jb, split, a, smem, full_bar, empty_bar, warp, lane);
   }
 }
 
@@ -215,36 +218,42 @@ struct Plan {
 };
 
 // nf = 64, gc = 32 dense block.  X buffer channels: x 0:64, x1..x4 64:192.  dY buffer A: g1..g4 at ga_coff + 0..127; B: g5.
+static const int NJOBS = 11;
+
 static void make_plan(Plan* pl, int ntiles, int ga_coff, int gb_coff) {
   Args& a = pl->a;
   const int nsm = num_sms();
-  // (row tile, col group list, tap0, ntap, relative cost per tile)
+  // (row tile, col group list, tap0, ntap); relative cost per tile = MMA work + shared-memory ingest of its tiles
   struct Spec { int m; int g0, ng; int tap0, ntap; int cost; };
-  const Spec specs[7] = {
-      {0, 0, 4, 0, 3, 2560}, {0, 0, 4, 3, 3, 2560}, {0, 0, 4, 6, 3, 2560},   // rows 0:128 x g1..g4, ingest bound
-      {0, 4, 2, 0, 5, 2880}, {0, 4, 2, 5, 4, 2304},                          // rows 0:128 x g5
-      {1, 3, 3, 0, 5, 2880}, {1, 3, 3, 5, 4, 2304}};                         // rows 128:192 x g4, g5
+  Spec specs[NJOBS] = {
+      {0, 0, 4, 0, 2, 0}, {0, 0, 4, 2, 2, 0}, {0, 0, 4, 4, 2, 0}, {0, 0, 4, 6, 2, 0}, {0, 0, 4, 8, 1, 0},   // rows 0:128 x g1..g4
+      {0, 4, 2, 0, 4, 0}, {0, 4, 2, 4, 4, 0}, {0, 4, 2, 8, 1, 0},                                           // rows 0:128 x g5
+      {1, 3, 3, 0, 4, 0}, {1, 3, 3, 4, 4, 0}, {1, 3, 3, 8, 1, 0}};                                          // rows 128:192 x g4, g5
+  for (int j = 0; j < NJOBS; j++) {
+    const int nchunk = specs[j].m == 0 ? 4 : 2;
+    specs[j].cost = 4 * nchunk * specs[j].ntap * specs[j].ng + 12 * nchunk + 8 * specs[j].ng;
+  }
   int total = 0;
-  for (int j = 0; j < 7; j++) total += specs[j].cost;
-  int ctas[7], used = 0;
-  for (int j = 0; j < 7; j++) {
+  for (int j = 0; j < NJOBS; j++) total += specs[j].cost;
+  int ctas[NJOBS], used = 0;
+  for (int j = 0; j < NJOBS; j++) {
     ctas[j] = (int)((long)nsm * specs[j].cost / total);
     if (ctas[j] < 1) ctas[j] = 1;
     if (ctas[j] > ntiles) ctas[j] = ntiles;
     used += ctas[j];
   }
-  for (int j = 0; used < nsm && j < 7; j = (j + 1) % 7) {      // hand out the rounding remainder
+  for (int j = 0; used < nsm && j < NJOBS; j = (j + 1) % NJOBS) {      // hand out the rounding remainder
     if (ctas[j] < ntiles) { ctas[j]++; used++; }
     else {
       bool room = false;
-      for (int q = 0; q < 7; q++) room |= ctas[q] < ntiles;
+      for (int q = 0; q < NJOBS; q++) room |= ctas[q] < ntiles;
       if (!room) break;
     }
   }
-  a.njobs = 7;
+  a.njobs = NJOBS;
   long off = 0;
   int cta0 = 0;
-  for (int j = 0; j < 7; j++) {
+  for (int j = 0; j < NJOBS; j++) {
     Job& jb = a.job[j];
     const Spec& s = specs[j];
     if (s.m == 0) {

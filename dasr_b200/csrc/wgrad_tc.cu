@@ -1,95 +1,32 @@
-// tcgen05 filter-gradient (wgrad) kernel for the 3x3 s1 p1 convolutions of the RRDB generator.
+// wgmma filter-gradient (wgrad) kernel for the 3x3 s1 p1 convolutions of the RRDB generator (sm_90a).
 //
 //   dW[tap][ci][co] = sum over pixels p of  X[p + tap][ci] * dY[p][co]            (reference: autograd of
 //   nn.Conv2d in codes/SRN/models/modules/block.py:142-143 — ResidualDenseBlock_5C / RRDBNet convs)
 //
-// GEMM view per tap:  D[M = 128 input channels, N = 32 output channels] += A[M, K] * B[N, K]^T with K = pixels.
+// GEMM view per tap:  D[M = 64 input channels, N = 32 output channels] += A[M, K] * B[N, K]^T with K = pixels.
 // Both operands are "MN-major" for the tensor core: the NHWC tiles already in shared memory have the channel
 // (M resp. N) index contiguous and the pixel (K) index as the row:
-//   A: the SAME (16+2)x(8+2) halo tiles the forward kernel uses — four 32-channel chunks side by side (LBO = chunk
+//   A: the SAME (16+2)x(8+2) halo tiles the forward kernel uses — two 32-channel chunks side by side (LBO = chunk
 //      slot stride), 8-pixel K groups one tile row apart (SBO = 640 B); a tap is a start-address shift.
 //   B: the 16x8 dY tile, 32 channels (SBO = 512 B).
-// One CTA owns (128-channel M tile, 32-channel N slice) and walks its share of the pixel tiles, accumulating all
-// 9 taps in TMEM (9 x 32 fp32 columns) for its whole lifetime; a single epilogue at the end writes the partial
-// [tap*cin + ci][co] block, and the deterministic split-K reduce of conv_f32.cu produces the OIHW gradient.
+// One CTA owns (64-channel M tile, 32-channel N slice) and walks its share of the pixel tiles; its consumer warpgroup
+// holds the 64 input channels x 9 taps x 32 output channels in registers (144 per thread: one warpgroup per CTA keeps
+// the whole register file available) for the CTA's whole lifetime, and writes the partial [tap*cin + ci][co] block once
+// at the end; the deterministic split-K reduce below produces the OIHW gradient.
 #include <cuda.h>
-#include "common.cuh"
+#include "tc_common.cuh"
 
 namespace dasr {
 
 namespace wg {
 
-constexpr int TILE_H = 16, TILE_W = 8, HALO_H = 18, HALO_W = 10;
-constexpr int ROW_B = 64;                                // 32 bf16 channels
 constexpr int A_SLOT = 12288;                            // one 32-channel halo tile (11520 B) rounded to 1 KB
-constexpr int A_HALO_BYTES = HALO_H * HALO_W * ROW_B;    // 11520
 constexpr int B_BYTES = TILE_H * TILE_W * ROW_B;         // 8192
-constexpr int STAGE_BYTES = 4 * A_SLOT + B_BYTES;        // 57344
-constexpr int STAGES = 3;
-constexpr int THREADS = 192;                             // warp 0 TMA, warp 1 MMA, warps 2..5 epilogue
+constexpr int MCHUNKS = 2;                               // 32-channel chunks per M tile
+constexpr int STAGE_BYTES = MCHUNKS * A_SLOT + B_BYTES;  // 32768
+constexpr int STAGES = 4;
+constexpr int THREADS = 160;                             // warps 0..3 consumer warpgroup, warp 4 TMA
 constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + 256;
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  while (!mbar_try_wait(bar, parity)) {
-  }
-}
-__device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void umma(uint32_t d, uint64_t a, uint64_t b, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d), "l"(a), "l"(b), "r"(idesc), "r"(acc)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-
-// MN-major, SWIZZLE_64B operand descriptor: [0,14) start>>4 | [16,30) LBO>>4 (stride between 32-element MN groups)
-// | [32,46) SBO>>4 (stride between 8-row K groups) | version 1 @46 | layout type 4 (SWIZZLE_64B) @61
-__device__ __forceinline__ uint64_t desc_mn_sw64(uint32_t addr, uint32_t lbo, uint32_t sbo) {
-  return (uint64_t)((addr >> 4) & 0x3FFF) | ((uint64_t)((lbo >> 4) & 0x3FFF) << 16) | ((uint64_t)((sbo >> 4) & 0x3FFF) << 32) |
-         ((uint64_t)1 << 46) | ((uint64_t)4 << 61);
-}
 
 struct Args {
   int N, H, W;
@@ -108,36 +45,26 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant_
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
   uint64_t* full_bar = bars;             // [STAGES]
   uint64_t* empty_bar = bars + STAGES;   // [STAGES]
-  uint64_t* done_bar = bars + 2 * STAGES;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int mtile = blockIdx.y / a.nslices, nslice = blockIdx.y - mtile * a.nslices;
-  const int chunk0 = mtile * 4;                                   // first 32-channel chunk of this M tile
+  const int chunk0 = mtile * MCHUNKS;                             // first 32-channel chunk of this M tile
   int nvalid = (a.cin - chunk0 * 32 + 31) / 32;                    // chunks of this M tile that exist
-  nvalid = nvalid > 4 ? 4 : nvalid;
+  nvalid = nvalid > MCHUNKS ? MCHUNKS : nvalid;
 
   if (threadIdx.x == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tm_x)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tm_dy)) : "memory");
-    for (int s = 0; s < STAGES; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(done_bar, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    tma_prefetch_desc(&tm_x);
+    tma_prefetch_desc(&tm_dy);
+    for (int s = 0; s < STAGES; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 4); }
+    fence_barrier_init();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr)), "r"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  // chunk slots this CTA never loads must not hold NaN bit patterns (0 * NaN would poison real rows? no: rows are
-  // independent, but keep the accumulators finite for tidy partials): zero them once
+  // chunk slots this CTA never loads are still read by the M = 64 wgmmas (rows that are never written out): keep the
+  // accumulators finite
   for (int i = threadIdx.x; i < STAGES * STAGE_BYTES / 16; i += THREADS) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+  fence_proxy_async();
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
+  if (warp == 4) {
     if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -149,86 +76,61 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant_
         mbar_expect_tx(&full_bar[stage], (uint32_t)(nvalid * A_HALO_BYTES + B_BYTES));
         for (int c = 0; c < nvalid; c++)
           tma_load_4d(st + c * A_SLOT, &tm_x, &full_bar[stage], a.x_coff + (chunk0 + c) * 32, x0 - 1, y0 - 1, n);
-        tma_load_4d(st + 4 * A_SLOT, &tm_dy, &full_bar[stage], a.dy_coff + nslice * 32, x0, y0, n);
+        tma_load_4d(st + MCHUNKS * A_SLOT, &tm_dy, &full_bar[stage], a.dy_coff + nslice * 32, x0, y0, n);
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    // instruction descriptor: D fp32, A/B bf16, BOTH operands MN-major, N = 32, M = 128
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((32u >> 3) << 17) | ((128u >> 4) << 24);
+  } else {
+    const uint64_t a_hi = desc_hi(A_SLOT, HALO_W * ROW_B, DESC_SW64);
+    const uint64_t b_hi = desc_hi(B_BYTES, TILE_W * ROW_B, DESC_SW64);
+    float acc[9][16];
     int stage = 0;
     uint32_t phase = 0;
+    int prev = -1;
     bool first = true;
     for (int tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x) {
       mbar_wait(&full_bar[stage], phase);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      if (elect_one()) {
-        const uint32_t a0 = smem_u32(smem + stage * STAGE_BYTES);
-        const uint32_t b0 = a0 + 4 * A_SLOT;
-#pragma unroll 1
-        for (int tap = 0; tap < 9; tap++) {
-          const uint32_t at = a0 + (uint32_t)(((tap / 3) * HALO_W + (tap % 3)) * ROW_B);
-          const uint32_t d = tmem_base + (uint32_t)(tap * 32);
+      const uint32_t a0 = smem_u32(smem + stage * STAGE_BYTES);
+      const uint32_t b0 = a0 + MCHUNKS * A_SLOT;
+      wgmma_fence();
 #pragma unroll
-          for (int ks = 0; ks < 8; ks++) {          // 16 pixels (two tile rows) per MMA
-            const uint64_t da = desc_mn_sw64(at + ks * 2 * HALO_W * ROW_B, A_SLOT, HALO_W * ROW_B);
-            const uint64_t db = desc_mn_sw64(b0 + ks * 2 * TILE_W * ROW_B, 0, TILE_W * ROW_B);
-            umma(d, da, db, idesc, (uint32_t)!(first && ks == 0));
-          }
-        }
-        umma_commit(&empty_bar[stage]);
+      for (int tap = 0; tap < 9; tap++) {
+        const uint32_t at = a0 + (uint32_t)(((tap / 3) * HALO_W + (tap % 3)) * ROW_B);
+#pragma unroll
+        for (int ks = 0; ks < 8; ks++)            // 16 pixels (two tile rows) per MMA
+          wgmma<32, 0, 1>(acc[tap], make_desc(at + ks * 2 * HALO_W * ROW_B, a_hi), make_desc(b0 + ks * 2 * TILE_W * ROW_B, b_hi),
+                          (first && ks == 0) ? 0 : 1);
       }
-      __syncwarp();
+      wgmma_commit();
+      if (prev >= 0) {
+        wgmma_wait<1>();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      }
+      prev = stage;
       first = false;
       if (++stage == STAGES) { stage = 0; phase ^= 1; }
     }
-    if (elect_one()) umma_commit(done_bar);
-    __syncwarp();
-  } else {
-    // epilogue (once): lane = input channel of this M tile, 9 x 32 columns = taps x output channels
-    const int q = warp & 3;
-    const int ci = mtile * 128 + q * 32 + lane;
-    mbar_wait(done_bar, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const bool any = (int)blockIdx.x < a.ntiles;
-    float* dst = a.part + (size_t)blockIdx.x * 9 * a.cin * a.cout;
-    for (int tap = 0; tap < 9; tap++) {
-      uint32_t rr[32];
-      tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(tap * 32), rr);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      if (ci < a.cin) {
-        float4* o = reinterpret_cast<float4*>(dst + ((size_t)tap * a.cin + ci) * a.cout + nslice * 32);
+    wgmma_wait<0>();
 #pragma unroll
-        for (int j = 0; j < 8; j++)
-          o[j] = any ? make_float4(__uint_as_float(rr[4 * j]), __uint_as_float(rr[4 * j + 1]), __uint_as_float(rr[4 * j + 2]),
-                                   __uint_as_float(rr[4 * j + 3]))
-                     : make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int tap = 0; tap < 9; tap++) fence_regs<16>(acc[tap]);
+    // epilogue (once): rows ci = 16 * warp + lane / 4 (+ 8), columns co = 8j + 2 * (lane & 3) (+ 1)
+    float* dst = a.part + (size_t)blockIdx.x * 9 * a.cin * a.cout;
+    const int cq = 2 * (lane & 3);
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      const int ci = mtile * 64 + 16 * warp + (lane >> 2) + 8 * h;
+      if (ci < a.cin) {
+#pragma unroll
+        for (int tap = 0; tap < 9; tap++)
+#pragma unroll
+          for (int j = 0; j < 4; j++) {
+            float2 v = first ? make_float2(0.f, 0.f) : make_float2(acc[tap][4 * j + 2 * h], acc[tap][4 * j + 2 * h + 1]);
+            *reinterpret_cast<float2*>(dst + ((size_t)tap * a.cin + ci) * a.cout + nslice * 32 + 8 * j + cq) = v;
+          }
       }
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
-  }
-}
-
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static PFN_encodeTiled get_encode() {
-  static PFN_encodeTiled fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<PFN_encodeTiled>(ptr);
-  }
-  return fn;
 }
 
 static int splits_for(int ntiles, int gy) {
@@ -261,8 +163,8 @@ using namespace dasr;
 extern "C" {
 
 size_t dasr_conv3x3_wgrad_tc_workspace(int N, int H, int W, int cin, int cout) {
-  int ntiles = N * cdiv(H, wg::TILE_H) * cdiv(W, wg::TILE_W);
-  int gy = cdiv(cin, 128) * (cout / 32);
+  int ntiles = N * cdiv(H, TILE_H) * cdiv(W, TILE_W);
+  int gy = cdiv(cin, 32 * wg::MCHUNKS) * (cout / 32);
   return (size_t)wg::splits_for(ntiles, gy) * 9 * cin * cout * 4 + 256;
 }
 
@@ -276,19 +178,19 @@ int dasr_conv3x3_wgrad_tc(const void* x, int x_cs, int x_coff, const void* dy, i
                    dy_coff + cout <= dy_cs,
                "wgrad_tc: channel slices");
   DASR_REQUIRE(workspace_bytes >= dasr_conv3x3_wgrad_tc_workspace(N, H, W, cin, cout), "wgrad_tc: workspace too small");
-  wg::PFN_encodeTiled enc = wg::get_encode();
+  PFN_encodeTiled enc = get_encode();
   if (!enc) {
     set_error("wgrad_tc: cuTensorMapEncodeTiled not available");
     return DASR_E_NODRIVER;
   }
   wg::Args a;
   a.N = N; a.H = H; a.W = W; a.cin = cin; a.cout = cout; a.x_coff = x_coff; a.dy_coff = dy_coff;
-  a.tiles_x = cdiv(W, wg::TILE_W);
-  a.tiles_y = cdiv(H, wg::TILE_H);
+  a.tiles_x = cdiv(W, TILE_W);
+  a.tiles_y = cdiv(H, TILE_H);
   a.ntiles = N * a.tiles_x * a.tiles_y;
   a.nslices = cout / 32;
   a.part = (float*)workspace;
-  const int gy = cdiv(cin, 128) * a.nslices;
+  const int gy = cdiv(cin, 32 * wg::MCHUNKS) * a.nslices;
   const int gx = wg::splits_for(a.ntiles, gy);
   CUtensorMap tmx, tmy;
   for (int t = 0; t < 2; t++) {
@@ -296,7 +198,7 @@ int dasr_conv3x3_wgrad_tc(const void* x, int x_cs, int x_coff, const void* dy, i
     const int cs = t ? dy_cs : x_cs;
     cuuint64_t gdim[4] = {(cuuint64_t)cs, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
     cuuint64_t gstr[3] = {(cuuint64_t)cs * 2, (cuuint64_t)W * cs * 2, (cuuint64_t)H * W * cs * 2};
-    cuuint32_t box[4] = {32, (cuuint32_t)(t ? wg::TILE_W : wg::HALO_W), (cuuint32_t)(t ? wg::TILE_H : wg::HALO_H), 1};
+    cuuint32_t box[4] = {32, (cuuint32_t)(t ? TILE_W : HALO_W), (cuuint32_t)(t ? TILE_H : HALO_H), 1};
     cuuint32_t estr[4] = {1, 1, 1, 1};
     CUresult r = enc(t ? &tmy : &tmx, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), gdim, gstr, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_64B,

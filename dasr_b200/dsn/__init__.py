@@ -1,1 +1,1 @@
-"""B200 drop-in for the reference's codes/DSN modules (`model.py`, `loss.py`) and its training iteration."""
+"""H100 drop-in for the reference's codes/DSN modules (`model.py`, `loss.py`) and its training iteration."""

@@ -1,5 +1,5 @@
 """Mixed-precision De_resnet (DSN/model.py:25-55): the 3->64 stem and the sixteen 64->64 3x3 convs of the residual
-trunk on the tcgen05 kernels (bf16 activations, fp32 accumulation; fprop + dgrad = dasr_conv_tc, filter gradients =
+trunk on the wgmma kernels (bf16 activations, fp32 accumulation; fprop + dgrad = dasr_conv_tc, filter gradients =
 dasr_conv3x3_wgrad_tc), residual adds fused in the conv epilogues (forward: conv2 + x; backward: dgrad(conv1) + skip
 gradient); the stride-2 tail, the 64->3 output conv and the sigmoid stay on the fp32 kernels (seqnet).  fp32 master
 weights, fp32 filter gradients.  Opt-in: De_resnet.precision = 'bf16' or DASR_B200_TRAIN_PRECISION=bf16."""
@@ -14,7 +14,8 @@ BF = torch.bfloat16
 
 
 def _pair(nf):
-    """64 -> 64 trunk convs on the CTA-pair kernel: 64 instead of 84 cycles per MMA (DASR_B200_PAIR=0 switches back)."""
+    """64 -> 64 trunk convs on the cluster pair (the activation tile is read once for both Cout halves; DASR_B200_PAIR=0
+    switches back)."""
     return _engine.PAIR_MODE and nf % 64 == 0 and nf <= 256
 
 

@@ -1,4 +1,4 @@
-"""Drop-in for /root/reference/codes/DSN/loss.py: generator_loss / discriminator_loss (loss.py:11-41) and
+"""Drop-in for codes/DSN/loss.py: generator_loss / discriminator_loss (loss.py:11-41) and
 GeneratorLoss (loss.py:44-107) with the VGG16 perceptual term (loss.py:118-129) on dasr_b200 kernels."""
 import os
 import warnings
@@ -46,7 +46,7 @@ def discriminator_loss(reals, fakes, wasserstein=False, grad_penalties=None, wei
     if weights is None:
         weights = [1.0 / len(fakes)] * len(fakes)
     if wasserstein:
-        raise NotImplementedError('WGAN-GP (double backward through D) is not on the B200 path')
+        raise NotImplementedError('WGAN-GP (double backward through D) is not on the H100 path')
     loss = 0.0
     for real, fake, weight in zip(reals, fakes, weights):
         loss = loss + weight * (_LogLoss.apply(real, False) + _LogLoss.apply(fake, True))
@@ -149,5 +149,5 @@ class GeneratorLoss(nn.Module):
 
     def filter_wavelet_LL(self, x, norm=True):
         if not norm:
-            raise NotImplementedError('un-normalised LL band is not on the B200 path')
+            raise NotImplementedError('un-normalised LL band is not on the H100 path')
         return haar_split(x, True)[0]            # LL * 0.5  (loss.py:101-107)

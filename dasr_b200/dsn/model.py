@@ -1,4 +1,4 @@
-"""Drop-in for /root/reference/codes/DSN/model.py on the dasr_b200 kernels: same class names, constructor
+"""Drop-in for codes/DSN/model.py on the dasr_b200 kernels: same class names, constructor
 arguments, state_dict keys and error behaviour; every forward/backward is C-ABI CUDA (no CPU fallback).
 
   De_resnet / Generator / ResidualBlock   model.py:7-55,213-224   3x3 convs + one-slope PReLU + sigmoid
@@ -90,7 +90,7 @@ class De_resnet(_SeqNet):
         # like the reference (model.py:33-52), any other scale leaves `down_sample` undefined and forward raises
         self.block_output = nn.Conv2d(64, 3, kernel_size=3, padding=1)
 
-    precision = None     # None -> DASR_B200_TRAIN_PRECISION or 'fp32'; 'bf16' = tcgen05 trunk (dsn/engine_bf16.py)
+    precision = None     # None -> DASR_B200_TRAIN_PRECISION or 'fp32'; 'bf16' = wgmma trunk (dsn/engine_bf16.py)
 
     def _tail_spec(self):
         s = []
@@ -169,7 +169,7 @@ class NLayerDiscriminator(_SeqNet):
     def __init__(self, input_nc, ndf=64, n_layers=3, norm_layer='Instance', kw=4, padw=1, stride=2):
         super().__init__()
         if norm_layer.lower() == 'batch':
-            raise NotImplementedError('NLayerDiscriminator with BatchNorm is not on the B200 path')
+            raise NotImplementedError('NLayerDiscriminator with BatchNorm is not on the H100 path')
         if norm_layer.lower() != 'instance':
             raise NotImplementedError('Norm layer [{:s}] not recognized'.format(norm_layer))
         seq = [nn.Conv2d(input_nc, ndf, kernel_size=kw, stride=stride, padding=padw), nn.LeakyReLU(0.2, True)]
@@ -244,7 +244,7 @@ class Discriminator(nn.Module):
 
     def forward(self, x, y=None):
         if y is not None:
-            raise NotImplementedError('relativistic (ragan) discriminator scores are not on the B200 path')
+            raise NotImplementedError('relativistic (ragan) discriminator scores are not on the H100 path')
         if self.filter is not None:
             x = self.filter(x)
         x = self.net(x)
@@ -254,8 +254,8 @@ class Discriminator(nn.Module):
 
     def filter_wavelet(self, x, norm=True):
         if not norm:
-            raise NotImplementedError('un-normalised wavelet bands are not on the B200 path')
+            raise NotImplementedError('un-normalised wavelet bands are not on the H100 path')
         _, hc = haar_split(x, True)              # band-major cat(LH, HL, HH) * 0.5 + 0.5  (model.py:106-117)
         if self.cs.lower() == 'cat':
             return hc
-        raise NotImplementedError('Wavelet format [{:s}] not on the B200 path'.format(self.cs))
+        raise NotImplementedError('Wavelet format [{:s}] not on the H100 path'.format(self.cs))

@@ -1,4 +1,4 @@
-"""Drop-in for /root/reference/codes/DSN/receptive_cal.py (and codes/SRN/utils/receptive_cal.py): receptive-field
+"""Drop-in for codes/DSN/receptive_cal.py (and codes/SRN/utils/receptive_cal.py): receptive-field
 bookkeeping + the domain-distance map (DDM) of create_dataset_modified.py:14-24, with the O(patch x rf^2) numpy
 scatter (`weights_matrix`, receptive_cal.py:34-43) replaced by the dasr_ddm gather kernels.
 

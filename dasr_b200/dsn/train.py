@@ -1,4 +1,4 @@
-"""The training iteration of /root/reference/codes/DSN/train.py:204-264 as a function (the reference has it inline
+"""The training iteration of codes/DSN/train.py:204-264 as a function (the reference has it inline
 in a script).  Both gradients are taken with the D weights of the forward pass, then both Adam steps are applied
 (train.py steps D before back-propagating the G loss through it, which PyTorch >= 1.5 rejects; see
 oracle/dsn_oracle.py)."""

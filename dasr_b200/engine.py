@@ -9,7 +9,7 @@ SURVEY.md §3.3, H4); kernel-layout copies are derived per call (training) or ca
 
 precision:
   'fp32' — CUDA-core fp32 kernels everywhere (the 1e-3 rel-Linf parity mode; also the training mode)
-  'bf16' — tcgen05 bf16 kernels, fp32 accumulate (inference performance mode)
+  'bf16' — wgmma bf16 kernels, fp32 accumulate (inference performance mode)
 """
 import math
 import os
@@ -53,7 +53,7 @@ class RRDBLayout:
         self.n_up = 1 if upscale == 3 else int(math.log(upscale, 2))
         self.up_factor = 3 if upscale == 3 else 2
         if self.up_factor != 2:
-            raise NotImplementedError('RRDBNet upscale=3 (nearest x3 upconv) is not supported by the B200 path')
+            raise NotImplementedError('RRDBNet upscale=3 (nearest x3 upconv) is not supported by the H100 path')
         self.n_rdb = 3 * nb
         self.i_fea = 0
         self.i_rdb0 = 1                               # conv index of RDB r conv k: 1 + 5*r + (k-1)
@@ -222,7 +222,7 @@ def rrdb_backward_f32(ctx, params, dout, need_dx=False):
     return dx, grads
 
 
-# ---- bf16 tcgen05 inference -----------------------------------------------------------------------
+# ---- bf16 wgmma inference -----------------------------------------------------------------------
 
 _TC_W_BUDGET = 150 * 1024   # resident-filter bytes per CTA that still leaves >= 5 halo stages
 
@@ -320,9 +320,7 @@ def _fused_rdb_filters(cache, params, L, r, nf):
 #   SCHED2 (round 1):  1: x -> x1 | p2 p3 p4 p5   2: x1 -> x2 | p3   3: x2 -> x3 | p4   4: x1,x3 -> x4 | p5   5: x2,x4 -> out
 #                      34 x 64 B per pixel of DRAM traffic, 9 chunk-passes of MMAs
 #   SCHED3 (round 2):  1: x -> x1 | p2 p3 p4 p5   2: x1 -> x2        3: x1,x2 -> x3 | p4   4: x3 -> x4      5: x1..x4 -> out
-#                      30 x 64 B per pixel, 11 chunk-passes.  The launches are HBM-bound once they run on CTA pairs
-#                      (64 cycles per MMA K-step instead of 84: tools/sched_search.py, profiles/r2_summary.md), so trading
-#                      partial-sum bytes for MMA passes pays: every partial sum is now written once and read once.
+#                      30 x 64 B per pixel, 11 chunk-passes: every partial sum is written once and read once.
 SCHED2 = ((('x',), (1, 2, 3, 4, 5)), ((1,), (2, 3)), ((2,), (3, 4)), ((1, 3), (4, 5)), ((2, 4), (5,)))
 SCHED3 = ((('x',), (1, 2, 3, 4, 5)), ((1,), (2,)), ((1, 2), (3, 4)), ((3,), (4,)), ((1, 2, 3, 4), (5,)))
 # 4: like 3, but conv5's product with x moves from launch 1 (as a 64-channel partial sum: one slab written, one read back) to
@@ -476,7 +474,8 @@ TILE_REV = os.environ.get('DASR_B200_TILE_REV', '1') != '0'
 def _rdb_stage1(b, w, bias, out, nf, tile_rev=False):
     """Launch 1 of a dense block: x (K = nf) against the stacked filters of conv1..5 (N = 4*GC + nf = 192), LeakyReLU on the
     first GC columns (= x1).  One CTA cannot keep the 192-wide filter set resident, so the single-CTA kernel runs it as
-    two Cout tiles of 96; the CTA-pair kernel splits the filters over the two SMs of a TPC and issues M=256, N=192."""
+    two Cout tiles of 96 that each load the activation tile; the cluster pair splits the filters over two SMs and
+    multicasts one load of the activation tile into both."""
     if PAIR_STAGE1 and nf == 64 and GC == 32:
         ops.conv_tc(View(b, nf, 0), w, bias, out, act=ACT_LRELU, slope=0.2, act_cols=GC, pair=True, tile_rev=tile_rev)
     else:
@@ -484,7 +483,7 @@ def _rdb_stage1(b, w, bias, out, nf, tile_rev=False):
 
 
 def _last_layer(h0, out, w, i, cache, wk, bk, hk, dtype):
-    """HR_conv1 (nf -> out_nc <= 3 channels, NCHW fp32 out).  An MMA costs the same 84 cycles for N = 16 as for N = 128, so
+    """HR_conv1 (nf -> out_nc <= 3 channels, NCHW fp32 out).  An N = 16 MMA uses a small fraction of the tensor core, so
     the nine taps go into GEMM-N: one pass over the halo tile gives every halo pixel's product with all 27 (tap, channel)
     filter rows, the epilogue adds the nine shifted partial results (8 MMAs per pixel tile instead of 36)."""
     out_nc = w.shape[0]
@@ -496,15 +495,15 @@ def _last_layer(h0, out, w, i, cache, wk, bk, hk, dtype):
 
 
 def rrdb_forward_bf16(x, params, nb, upscale=4, cache=None, fused=True, half=False):
-    """tcgen05 bf16 forward (inference).  NCHW fp32 in -> NCHW fp32 out; bf16 NHWC in between.
+    """wgmma bf16 forward (inference).  NCHW fp32 in -> NCHW fp32 out; bf16 NHWC in between.
 
     fused=True : dense-block N-fusion.  Each RDB runs 5 launches; launch j reads one or two 32-channel chunks ONCE
-                 and produces conv j's output plus partial sums of later convs of the block (a tcgen05.mma of
-                 N <= 128 costs the same ~84 cycles as N = 32).  Partial sums live IN PLACE in the channel slots the
+                 and produces conv j's output plus partial sums of later convs of the block (one wide-N wgmma
+                 instead of several N = 32 ones on the same A tile).  Partial sums live IN PLACE in the channel slots the
                  finished activations will occupy (bf16), so the only extra state is a 64-channel slot for conv5.
                  DASR_B200_SCHED=3 (default) / 2: engine.SCHED3 / SCHED2; =1: every launch carries all later partial sums.
     fused=False: one launch per conv over the growing concat (the straightforward restatement).
-    half=True  : IEEE half instead of bf16 for filters, activations and partial sums (tcgen05 kind::f16 with F16 operands:
+    half=True  : IEEE half instead of bf16 for filters, activations and partial sums (wgmma with F16 operands:
                  same rate, 11 instead of 8 significand bits).  RRDBNet activations stay far inside half's range
                  (|x| < 6.5e4); meant for inference, where it brings PSNR / SSIM within 3 decimals of the fp32 path.
     """
@@ -608,16 +607,16 @@ def rrdb_forward_bf16(x, params, nb, upscale=4, cache=None, fused=True, half=Fal
     del cur
     out_nc = Wt(L.i_hr1).shape[0]
     out = _empty((N, out_nc, h, w), x)
-    # last layer: Cout 3 -> one 16-wide UMMA N tile, epilogue writes the 3 real channels straight to NCHW fp32
+    # last layer: Cout 3 -> one 16-wide wgmma N tile, epilogue writes the 3 real channels straight to NCHW fp32
     _last_layer(h0, out, Wt(L.i_hr1), L.i_hr1, cache, wk, bk, hk, bf)
     _mark('tc_end')
     return out
 
 
-# ---- bf16 tcgen05 training (mixed precision: bf16 activations/gradients, fp32 accumulation, fp32 filter grads) ----
+# ---- bf16 wgmma training (mixed precision: bf16 activations/gradients, fp32 accumulation, fp32 filter grads) ----
 
 def rrdb_forward_bf16_train(x, params, nb, upscale=4, cache=None):
-    """Forward of the mixed-precision training mode: the dense-block N-fused tcgen05 schedule of the inference path,
+    """Forward of the mixed-precision training mode: the dense-block N-fused wgmma schedule of the inference path,
     but every RDB keeps its own buffer (the backward needs x, x1..x4)."""
     _need_cuda(x, 'RRDBNet')
     L = RRDBLayout(nb, params[0].shape[0], upscale)
@@ -688,9 +687,9 @@ def _side_stream(device):
 
 
 def rrdb_backward_bf16(ctx, params, dout, cache=None, flat=None):
-    """Backward of the mixed-precision mode: input gradients (dgrad) on the tcgen05 kernel (3x3 conv with flipped,
+    """Backward of the mixed-precision mode: input gradients (dgrad) on the wgmma kernel (3x3 conv with flipped,
     transposed filters; gradient contributions of a dense block accumulate in place in one bf16 buffer), filter
-    gradients on the tcgen05 wgrad kernel (MN-major operands straight from the NHWC tiles, fp32 TMEM accumulation).  Returns fp32 grads."""
+    gradients on the wgmma wgrad kernel (MN-major operands straight from the NHWC tiles, fp32 register accumulation).  Returns fp32 grads."""
     from .ops import TC_DGRAD
     L = ctx['L']
     nf = L.nf
@@ -727,7 +726,7 @@ def rrdb_backward_bf16(ctx, params, dout, cache=None, flat=None):
     dev = dout
 
     def wgrad(xv, gv, i, cin_real=None, cout_real=None, bias=True):
-        """filter + bias gradient of conv i on the tcgen05 wgrad kernel (zero-padded channel chunks are cut off)"""
+        """filter + bias gradient of conv i on the wgmma wgrad kernel (zero-padded channel chunks are cut off)"""
         xv, gv = ops.as_view(xv), ops.as_view(gv)
         if cin_real is None and cout_real is None:
             ops.conv3x3_wgrad_tc(xv, gv, gW(i))
@@ -779,8 +778,8 @@ def rrdb_backward_bf16(ctx, params, dout, cache=None, flat=None):
     overlap = fused_wgrad and os.environ.get('DASR_B200_BWD_OVERLAP', '1') == '1'
     pair_dgrad = PAIR_MODE and nf == 64 and GC == 32 and os.environ.get('DASR_B200_PAIR_DGRAD', '0') == '1'
     # DASR_B200_FUSE_MASK=1: LeakyReLU backward of x1..x4 inside the epilogue of the dgrad launch that completes each slot (pair
-    # kernel, activation in the res1 slot): 276 launches less per step, same step time (27.13 vs 27.17 ms: the K = 32 dgrads are
-    # a little slower on the pair kernel), gradients within 4e-3 rel-L2 of the unfused ones (one rounding instead of two) -> off
+    # kernel, activation in the res1 slot): 276 launches less per step, gradients within 4e-3
+    # rel-L2 of the unfused ones (one rounding instead of two) -> off by default
     fuse_mask = PAIR_STAGE1 and nf == 64 and GC == 32 and os.environ.get('DASR_B200_FUSE_MASK', '0') == '1'
     nset = 2 if overlap else 1
     GBs = [_empty((N, H, W, CS), dev, bf) for _ in range(nset)]
@@ -842,7 +841,7 @@ def rrdb_backward_bf16(ctx, params, dout, cache=None, flat=None):
 
         def reductions(b=b, GB=GB, g_x5=g_x5, c1=c1, c5=c5, r=r):
             # bias gradients of conv1..4 in one reduction (their masked output gradients are the final x1..x4 slices of GB),
-            # conv5's, and all five filter gradients of the block: one tcgen05 launch + one reduction
+            # conv5's, and all five filter gradients of the block: one wgmma launch + one reduction
             ops.bias_grad(View(GB, 4 * GC, nf), flat[b_off[c1]:b_off[c1] + 4 * GC])
             if fused_wgrad:
                 if overlap:
@@ -915,7 +914,7 @@ class _TrainGraphs:
 
 
 class RRDBNetFunctionBF16(torch.autograd.Function):
-    """Mixed-precision training node (tcgen05 fprop + dgrad + wgrad); graphs = None runs eagerly."""
+    """Mixed-precision training node (wgmma fprop + dgrad + wgrad); graphs = None runs eagerly."""
 
     @staticmethod
     def forward(ctx, x, nb, upscale, cache, graphs, arena, *params):
@@ -1190,7 +1189,7 @@ def _vgg_pair_nt(k_ch, n_ch):
 
 
 def vgg_forward_bf16(x, params, mean, std, feature_layer=34, save=False, cache=None):
-    """VGG19 features on the tcgen05 conv (bf16 activations/filters, fp32 accumulate).  Filters of the 256/512-channel
+    """VGG19 features on the wgmma conv (bf16 activations/filters, fp32 accumulate).  Filters of the 256/512-channel
     layers do not fit shared memory whole, so those layers run as Cout/nt column tiles (grid.y) of 16..64 channels."""
     _need_cuda(x, 'VGGFeatureExtractor')
     plan = vgg_plan(feature_layer)

@@ -3,7 +3,7 @@
 Marks `codes/SRN` and `codes/DSN` of a reference checkout for the dasr_b200 import overlay (dasr_b200/overlay.py) and
 makes the overlay start with every interpreter, so that `python Auto_Reproduce.py --dataset ... --artifact ...` — which
 shells out to `cd ./DSN; sh auto_reproduce_launcher_*.sh` and `cd ./SRN; python train.py -opt ...`
-(Auto_Reproduce.py:38-40) — runs the B200 modules without a single edit in the checkout's sources.
+(Auto_Reproduce.py:38-40) — runs the H100 modules without a single edit in the checkout's sources.
 
   * writes `<codes>/SRN/.dasr_b200` ("SRN") and `<codes>/DSN/.dasr_b200` ("DSN")  — the only files added to the checkout;
   * interpreter hook, one of

@@ -1,4 +1,4 @@
-"""Run one of the reference's entry scripts on the B200 path without touching the reference checkout:
+"""Run one of the reference's entry scripts on the H100 path without touching the reference checkout:
 
     python -m dasr_b200.launch /path/to/DASR/codes/SRN/test.py  -opt options/test/test_sr.json
     python -m dasr_b200.launch /path/to/DASR/codes/SRN/train.py -opt options/train/train_DASR_auto_reproduce_realsr.json

@@ -164,7 +164,7 @@ class PNetLin(nn.Module):
     def __init__(self, pnet_type='alex', pnet_rand=False, pnet_tune=False, use_dropout=True, spatial=False, version='0.1', lpips=True):
         super().__init__()
         if pnet_type != 'alex' or spatial or version != '0.1' or not lpips or pnet_tune:
-            raise NotImplementedError('LPIPS on the B200 path: net-lin / alex / v0.1, non-spatial, frozen trunk')
+            raise NotImplementedError('LPIPS on the H100 path: net-lin / alex / v0.1, non-spatial, frozen trunk')
         self.pnet_type, self.version = pnet_type, version
         self.chns = [64, 192, 384, 256, 256]
         self.scaling_layer = ScalingLayer()
@@ -206,7 +206,7 @@ class PerceptualLoss(nn.Module):
                  lin_weights=None, trunk_weights=None):
         super().__init__()
         if model != 'net-lin' or net != 'alex' or spatial or colorspace.lower() != 'rgb':
-            raise NotImplementedError("LPIPS on the B200 path: model='net-lin', net='alex', colorspace='rgb', spatial=False")
+            raise NotImplementedError("LPIPS on the H100 path: model='net-lin', net='alex', colorspace='rgb', spatial=False")
         self.spatial, self.use_gpu, self.gpu_ids = spatial, use_gpu, gpu_ids
         self.net = PNetLin()
         allow = os.environ.get('DASR_B200_ALLOW_RANDOM_VGG', '0') == '1'

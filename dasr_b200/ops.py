@@ -181,7 +181,7 @@ def conv2d_wgrad_f32(inp, dout, dw, db, k, stride, pad, ups=1, accumulate=False)
 
 
 def conv3x3_wgrad_tc(x, dy, dw, accumulate=False):
-    """tcgen05 filter gradient of a 3x3 s1 p1 conv: x, dy = Views of bf16 NHWC buffers (channels % 32 == 0), dw fp32 OIHW."""
+    """wgmma filter gradient of a 3x3 s1 p1 conv: x, dy = Views of bf16 NHWC buffers (channels % 32 == 0), dw fp32 OIHW."""
     x, dy = as_view(x), as_view(dy)
     N, H, W, _ = x.t.shape
     lib = _lib.load()
@@ -235,7 +235,7 @@ def pack_filter_f32(w, for_dgrad=False):
 
 
 # --------------------------------------------------------------------------------------------------
-# tcgen05 bf16 conv
+# wgmma bf16 conv
 # --------------------------------------------------------------------------------------------------
 
 TC_PACK_F16 = 0x100        # DASR_TC_PACK_F16
@@ -261,10 +261,10 @@ def pack_filter_tc(w, kind, dtype=torch.bfloat16):
 def conv_tc(inp, w_packed, bias, out, kind=TC_FPROP, nt=None, act=ACT_NONE, slope=0.2, alpha=1.0, act_cols=None,
             pre=None, res1=None, beta1=0.0, res2=None, beta2=0.0, mask=None, mask_c0=0, mask_c1=0, mask_slope=0.2,
             a_mode=0, nchw_out=None, cout=None, tile_rev=False, chunks=None, pair=None, tapn=False):
-    """tcgen05 3x3 conv on NHWC bf16 channel slices; chunks = optional list of 32-channel chunk offsets of `inp`'s buffer; `inp`/`out`/`pre`/`res*`/`mask` are Views (or tensors).
+    """wgmma 3x3 conv on NHWC bf16 channel slices; chunks = optional list of 32-channel chunk offsets of `inp`'s buffer; `inp`/`out`/`pre`/`res*`/`mask` are Views (or tensors).
     v = alpha*act(acc + bias + pre) + beta1*res1 + beta2*res2, activation on the first `act_cols` channels only.
     nchw_out: fp32 NCHW tensor — the launch writes its first nchw_out.shape[1] channels there (last layer).
-    pair: True = run on the CTA-pair kernel (dasr_conv_tc2: cta_group::2, filters split over two SMs, 64-cycle MMAs;
+    pair: True = run on the CTA-pair kernel (dasr_conv_tc2: 2-CTA cluster, filters split over two SMs, activation tiles multicast;
           plain 3x3 geometry, cout % 64 == 0, no mask; `nt` is ignored)."""
     inp = as_view(inp)
     N, H, W, _ = inp.t.shape

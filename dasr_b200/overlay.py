@@ -82,6 +82,6 @@ def activate():
 
 def _drop_in_defaults():
     """Defaults of the drop-in entry points (this overlay, dasr_b200.launch): reference scripts train in the mixed-precision
-    mode (tcgen05 fprop / dgrad / wgrad, tf32 side nets; 31 ms vs 490 ms per DASR step).  The library default stays the exact
+    mode (wgmma fprop / dgrad / wgrad, tf32 side nets).  The library default stays the exact
     fp32 mode; DASR_B200_TRAIN_PRECISION=fp32 selects it for a script, too."""
     os.environ.setdefault('DASR_B200_TRAIN_PRECISION', 'bf16')

@@ -327,7 +327,7 @@ def compile_sequence(mods, prefix, training, out_channels=None):
         elif isinstance(m, (nn.LeakyReLU, nn.ReLU)):
             raise NotImplementedError('a free-standing activation (not after a conv / norm / linear) is not on the path')
         else:
-            raise NotImplementedError('module %s (%s) is not on the B200 path' % (full, m.__class__.__name__))
+            raise NotImplementedError('module %s (%s) is not on the H100 path' % (full, m.__class__.__name__))
     return layers
 
 

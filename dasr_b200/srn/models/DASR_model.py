@@ -78,7 +78,7 @@ class DASR_Model(BaseModel):
         if self.is_train:
             self.cri_gan = L.GANLoss(train_opt['gan_type'], 1.0, 0.0).to(self.device)
             if train_opt['gan_type'] == 'wgan-gp':
-                raise NotImplementedError('wgan-gp gradient penalty (double backward) is not on the B200 path')
+                raise NotImplementedError('wgan-gp gradient penalty (double backward) is not on the H100 path')
 
         self.netG = networks.define_G(opt).to(self.device)
         if self.is_train:

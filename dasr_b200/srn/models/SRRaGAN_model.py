@@ -52,7 +52,7 @@ class SRRaGANModel(BaseModel):
             else:
                 self.netF = networks.define_F(opt, use_bn=False).to(self.device)
             if train_opt['gan_type'] == 'wgan-gp':
-                raise NotImplementedError('wgan-gp gradient penalty (double backward) is not on the B200 path')
+                raise NotImplementedError('wgan-gp gradient penalty (double backward) is not on the H100 path')
             self.cri_gan = L.GANLoss(train_opt['gan_type'], 1.0, 0.0).to(self.device)
             self.l_gan_w = train_opt['gan_weight']
             self.D_update_ratio = train_opt['D_update_ratio'] or 1

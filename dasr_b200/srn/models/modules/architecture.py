@@ -1,7 +1,7 @@
 """Networks of the SRN hot path with the reference's class names, constructor signatures and
 state_dict keys (codes/SRN/models/modules/architecture.py), running on dasr_b200 kernels.
 
-  RRDBNet               architecture.py:174-205   -> engine.RRDBNetFunction (fp32 train) / rrdb_forward_bf16 (tcgen05)
+  RRDBNet               architecture.py:174-205   -> engine.RRDBNetFunction (fp32 train) / rrdb_forward_bf16 (wgmma)
   NLayerDiscriminator   architecture.py:983-1024  -> engine.NLayerDFunction
   VGGFeatureExtractor   architecture.py:1060-1088 -> engine.VGGFunction
   GaussianFilter / FilterLow / FilterHigh  :1177-1243 -> dwfilter kernel
@@ -22,7 +22,7 @@ def _precision(module_default):
 
 
 class _GraphedForward:
-    """One inference forward captured into a CUDA graph (the tcgen05 path launches ~350-2800 small kernels per
+    """One inference forward captured into a CUDA graph (the wgmma path launches ~350-2800 small kernels per
     forward; replaying a graph removes the per-launch host cost).  Inputs are copied into a static buffer; the
     result is returned as a fresh tensor."""
 
@@ -55,7 +55,7 @@ class RRDBNet(nn.Module):
                  act_type='leakyrelu', mode='CNA', upsample_mode='upconv'):
         super().__init__()
         if norm_type is not None:
-            raise NotImplementedError('RRDBNet with norm layers is not on the B200 path (all shipped configs use norm_type null)')
+            raise NotImplementedError('RRDBNet with norm layers is not on the H100 path (all shipped configs use norm_type null)')
         if upsample_mode != 'upconv':
             raise NotImplementedError('upsample mode [{:s}] is not found'.format(upsample_mode))
         if act_type != 'leakyrelu':
@@ -96,7 +96,7 @@ class RRDBNet(nn.Module):
         need_grad = torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in params))
         if need_grad:
             tp = self.train_precision or os.environ.get('DASR_B200_TRAIN_PRECISION', 'fp32')
-            if tp == 'bf16':      # mixed precision: tcgen05 fprop / dgrad / wgrad, fp32 accumulation, fp32 filter gradients
+            if tp == 'bf16':      # mixed precision: wgmma fprop / dgrad / wgrad, fp32 accumulation, fp32 filter gradients
                 graphs = None
                 if os.environ.get('DASR_B200_GRAPH', '1') != '0' and x.is_cuda and not x.requires_grad:
                     # the graphs hold raw parameter addresses: re-capture if any parameter storage moved (.to(), .float(), ...)
@@ -111,7 +111,7 @@ class RRDBNet(nn.Module):
         prec = self.precision or _precision('bf16')
         if prec in ('bf16', 'bf16_layer', 'fp16', 'fp16_layer'):
             # 'bf16' / 'fp16' = dense-block N-fused launches (bf16 is the default); '*_layer' = one launch per conv;
-            # fp16 = IEEE half operands on the same tcgen05 kernels (3 more significand bits, same speed)
+            # fp16 = IEEE half operands on the same wgmma kernels (3 more significand bits, same speed)
             fn = lambda t: engine.rrdb_forward_bf16(t, params, self.nb, self.upscale, self._pack_cache,
                                                     fused=not prec.endswith('_layer'), half=prec.startswith('fp16'))
             if os.environ.get('DASR_B200_GRAPH', '1') == '0' or not x.is_cuda or engine.PROFILE is not None:
@@ -139,7 +139,7 @@ class NLayerDiscriminator(nn.Module):
     def __init__(self, input_nc, ndf=64, n_layers=3, norm_layer=nn.InstanceNorm2d):
         super().__init__()
         if norm_layer is not nn.InstanceNorm2d:
-            raise NotImplementedError('NLayerDiscriminator: only InstanceNorm2d is on the B200 path')
+            raise NotImplementedError('NLayerDiscriminator: only InstanceNorm2d is on the H100 path')
         kw, padw = 4, 1
         seq = [B.Conv2d(input_nc, ndf, kernel_size=kw, stride=2, padding=padw), nn.LeakyReLU(0.2, True)]
         nf_mult = 1
@@ -182,7 +182,7 @@ class VGGFeatureExtractor(nn.Module):
     def __init__(self, feature_layer=34, use_bn=False, use_input_norm=True, device=torch.device('cpu'), weights=None):
         super().__init__()
         if use_bn:
-            raise NotImplementedError('VGG19-BN feature extractor is not on the B200 path')
+            raise NotImplementedError('VGG19-BN feature extractor is not on the H100 path')
         self.use_input_norm = use_input_norm
         self.feature_layer = feature_layer
         mean = torch.Tensor([0.485, 0.456, 0.406]).view(1, 3, 1, 1).to(device)
@@ -194,7 +194,7 @@ class VGGFeatureExtractor(nn.Module):
         for _, v in self.features.named_parameters():
             v.requires_grad = False
         self._pack_cache = engine._PackCache()
-        self.precision = None          # None -> DASR_B200_TRAIN_PRECISION or 'fp32'; 'bf16' = tcgen05 convs
+        self.precision = None          # None -> DASR_B200_TRAIN_PRECISION or 'fp32'; 'bf16' = wgmma convs
 
     def _load_pretrained(self, weights):
         sd = None

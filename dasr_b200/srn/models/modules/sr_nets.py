@@ -90,7 +90,7 @@ class SRResNet(_Compiled):
         else:
             raise NotImplementedError('upsample mode [{:s}] is not found'.format(upsample_mode))
         if upscale == 3:
-            raise NotImplementedError('SRResNet upscale=3 is not supported by the B200 path')
+            raise NotImplementedError('SRResNet upscale=3 is not supported by the H100 path')
         upsampler = [upsample_block(nf, nf, act_type=act_type) for _ in range(n_upscale)]
         HR_conv0 = B.conv_block(nf, nf, kernel_size=3, norm_type=None, act_type=act_type)
         HR_conv1 = B.conv_block(nf, out_nc, kernel_size=3, norm_type=None, act_type=None)

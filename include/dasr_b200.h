@@ -1,5 +1,5 @@
 /*
- * dasr_b200 — C ABI of the B200-native DASR SRN hot path.
+ * dasr_b200 — C ABI of the H100-native (sm_90a) DASR SRN hot path.
  *
  * The reference (ShuhangGu/DASR, codes/SRN) has no FFI layer: its hot path is a chain of
  * torch.nn library calls (cuDNN/ATen).  Each entry point below replaces one such call site; the
@@ -13,7 +13,7 @@
  *
  * Two arithmetic modes exist for every convolution:
  *   *_f32 : CUDA-core fp32 FMA, fp32 storage     (the 1e-3 rel-Linf parity gate, BASELINE north_star)
- *   *_tc  : tcgen05.mma bf16 x bf16 -> fp32 TMEM accumulators, bf16 storage (the performance path)
+ *   *_tc  : wgmma bf16 x bf16 -> fp32 register accumulators, bf16 storage (the performance path)
  */
 #ifndef DASR_B200_H
 #define DASR_B200_H
@@ -99,8 +99,8 @@ int dasr_conv2d_wgrad_bf16(const void* in_bf16, const void* dout_bf16, float* dw
                            const DasrConvF32Params* p, int accumulate, void* workspace, size_t workspace_bytes,
                            void* stream);
 
-/* tcgen05 filter gradient of a 3x3 s1 p1 conv on bf16 NHWC channel slices (cin, cout multiples of 32):
- * dW[co][ci][dy][dx] (fp32 OIHW) = sum_pixels x[p + tap][ci] * dy[p][co], fp32 accumulation in TMEM, deterministic
+/* wgmma filter gradient of a 3x3 s1 p1 conv on bf16 NHWC channel slices (cin, cout multiples of 32):
+ * dW[co][ci][dy][dx] (fp32 OIHW) = sum_pixels x[p + tap][ci] * dy[p][co], fp32 accumulation in registers, deterministic
  * split-K reduction.  Replaces autograd's weight gradient of the RRDB convs (block.py:142-143, 262-278). */
 size_t dasr_conv3x3_wgrad_tc_workspace(int N, int H, int W, int cin, int cout);
 int dasr_conv3x3_wgrad_tc(const void* x_bf16, int x_cs, int x_coff, const void* dy_bf16, int dy_cs, int dy_coff,
@@ -116,7 +116,7 @@ int dasr_pack_filter_f32(const float* w_oihw, float* w_packed, int cout, int cin
                          int for_dgrad, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * tcgen05 bf16 3x3 (and 2x2 sub-pixel) convolution — the RRDB hot kernel.
+ * wgmma bf16 3x3 (and 2x2 sub-pixel) convolution — the RRDB hot kernel.
  * Replaces: ResidualDenseBlock_5C.conv1..5 (block.py:262-286), RRDB / ShortcutBlock residuals
  * (block.py:305-309, 103-105), LR_conv / upconv / HR_conv0 (architecture.py:182-201).
  *
@@ -145,7 +145,7 @@ typedef struct {
   float beta1; int res1_cs, res1_coff;
   float beta2; int res2_cs, res2_coff;
   int mask_cs, mask_coff, mask_c0, mask_c1; float mask_slope;
-  int a_mode;                  /* 0 = one halo tile per chunk + shifted UMMA descriptors (fast);
+  int a_mode;                  /* 0 = one halo tile per chunk + shifted wgmma descriptors (fast);
                                   1 = one aligned TMA tile per tap (validation path) */
   int epi_mode;                /* 0 = staged: tile -> swizzled shared memory -> TMA store; pre/res tiles arrive by TMA
                                       (also the sub-pixel out_mul=2 variants without pre / residual inputs: one strided
@@ -174,10 +174,10 @@ int dasr_conv_tc(const void* in_bf16, const void* w_packed_bf16, const float* bi
                  const void* res1_bf16, const void* res2_bf16, const void* mask_src_bf16,
                  void* out /* bf16 NHWC, or fp32 NCHW in epi_mode 2 */, const DasrConvTcParams* p, void* stream);
 
-/* The same convolution on a CTA PAIR (tcgen05 cta_group::2, csrc/conv_tc2.cu): the two SMs of a TPC each keep half of
- * the filter rows resident and each load the A tile of their own pixel tile; one M=256 instruction feeds both tensor
- * cores (measured: 64 cycles per K step and pixel tile for N <= 128, N/2 above, against 84 / N/2+5 on one CTA), and a
- * filter set twice as large fits (dense-block launch 1: K = 64, N = 192).
+/* The same convolution on a CTA PAIR (csrc/conv_tc.cu): a (1, 2, 1) thread-block cluster whose two CTAs take the two
+ * Cout halves of the same pixel tiles; each keeps half of the filter rows resident and the leader's TMA multicasts every
+ * activation tile into both, so a filter set twice as large fits (dense-block launch 1: K = 64, N = 192) and the
+ * activations are read once per pair.
  * Supported: plain 3x3 geometry (dasr_conv_tc_setup kind 0/1), epi_mode 0; `nt` = Cout tile of a CTA pair (multiple of
  * 32, <= 256, divides cout; grid.y walks the tiles — VGG's 256/512-channel layers run as tiles of 32..128); pre / res1 /
  * res2 as in dasr_conv_tc (nullable).  dasr_conv_tc2_supported answers for the loads announced by pre_cs / res1_cs /
@@ -242,7 +242,7 @@ int dasr_upsample2x_fwd(const void* src, void* dst, int N, int H, int W, int C, 
 /* dst = a*x + b*y on channel slices (gradient accumulation across concat consumers) */
 int dasr_axpby(const void* x, const void* y, void* dst, long npix, int C, int x_cs, int x_coff,
                int y_cs, int y_coff, int d_cs, int d_coff, float a, float b, int is_bf16, void* stream);
-/* Filter gradients of all five convs of one ResidualDenseBlock_5C (nf 64, gc 32) in one tcgen05 launch + one
+/* Filter gradients of all five convs of one ResidualDenseBlock_5C (nf 64, gc 32) in one wgmma launch + one
  * deterministic reduction (mixed-precision training).  xbuf: bf16 NHWC, channels [x 0:64 | x1..x4 64:192];
  * ga: bf16 NHWC holding the (LeakyReLU-masked) output gradients of conv1..4 in channels [ga_coff, ga_coff+128);
  * gb: output gradient of conv5 in channels [gb_coff, gb_coff+64); dw[k]: OIHW fp32 [32|64][64+32k][3][3]. */

@@ -1,7 +1,7 @@
 """CPU oracle for the DSN (domain-gap-aware down-sampling network) training path, BASELINE configs[4] —
 TEST INFRASTRUCTURE ONLY (same rules as srn_oracle.py: nothing under ``dasr_b200/`` may import it).
 
-A plain-PyTorch (CPU, fp32) restatement of /root/reference/codes/DSN: ``De_resnet`` (model.py:25-55,213-224),
+A plain-PyTorch (CPU, fp32) restatement of <DASR checkout>/codes/DSN: ``De_resnet`` (model.py:25-55,213-224),
 ``Discriminator``/``DiscriminatorBasic`` (model.py:60-118,173-210), ``generator_loss``/``discriminator_loss``/
 ``GeneratorLoss`` (loss.py:11-41,44-107) with ``PerceptualLossVGG16`` (loss.py:118-129) and the training
 iteration of train.py:204-264.

@@ -1,7 +1,7 @@
-"""Generate tests/golden/*.pt by running the UNMODIFIED reference (/root/reference/codes/SRN) on CPU.
+"""Generate tests/golden/*.pt by running the UNMODIFIED reference (<DASR checkout>/codes/SRN) on CPU.
 
-Run here (the container that has /root/reference); the fixtures it writes are committed so the GPU box
-(which has no /root/reference) can check against them.  Test infrastructure only.
+Run where a checkout of the original project exists (DASR_REFERENCE = its root directory); the fixtures it writes
+are committed, so the tests need no checkout.  Test infrastructure only.
 
     python oracle/gen_golden.py
 
@@ -17,7 +17,7 @@ from collections import OrderedDict
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-REF = '/root/reference/codes'
+REF = os.path.join(os.environ.get('DASR_REFERENCE', 'DASR'), 'codes')   # a ShuhangGu/DASR checkout
 sys.path.insert(0, os.path.join(HERE, 'ref_stubs'))
 sys.path.insert(0, os.path.join(REF, 'SRN'))
 sys.path.insert(0, REF)

@@ -1,11 +1,11 @@
-"""Generate tests/golden/ddm.pt from the UNMODIFIED reference /root/reference/codes/DSN/receptive_cal.py (pure numpy) and
+"""Generate tests/golden/ddm.pt from the UNMODIFIED reference <DASR checkout>/codes/DSN/receptive_cal.py (pure numpy) and
 create_dataset_modified.py:14-24's handler logic.  Test infrastructure only.   python oracle/gen_golden_ddm.py"""
 import os
 import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-sys.path.insert(0, '/root/reference/codes/DSN')
+sys.path.insert(0, os.path.join(os.environ.get('DASR_REFERENCE', 'DASR'), 'codes', 'DSN'))   # a ShuhangGu/DASR checkout
 sys.path.insert(0, ROOT)
 import numpy as np  # noqa: E402
 import torch  # noqa: E402

@@ -1,4 +1,4 @@
-"""Generate tests/golden/dsn_*.pt by running the UNMODIFIED reference DSN modules (/root/reference/codes/DSN:
+"""Generate tests/golden/dsn_*.pt by running the UNMODIFIED reference DSN modules (<DASR checkout>/codes/DSN:
 model.py, loss.py) on CPU.  Separate from gen_golden.py because DSN's top-level module names (`model`, `loss`,
 `utils`) collide with the SRN package names.  Test infrastructure only.
 
@@ -15,7 +15,7 @@ from collections import OrderedDict
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-REF = '/root/reference/codes'
+REF = os.path.join(os.environ.get('DASR_REFERENCE', 'DASR'), 'codes')   # a ShuhangGu/DASR checkout
 sys.path.insert(0, os.path.join(HERE, 'ref_stubs'))
 sys.path.insert(0, REF)
 sys.path.insert(0, os.path.join(REF, 'DSN'))

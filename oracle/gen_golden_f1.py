@@ -12,7 +12,7 @@ from collections import OrderedDict
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-REF = '/root/reference/codes'
+REF = os.path.join(os.environ.get('DASR_REFERENCE', 'DASR'), 'codes')   # a ShuhangGu/DASR checkout
 sys.path.insert(0, os.path.join(HERE, 'ref_stubs'))
 sys.path.insert(0, os.path.join(REF, 'SRN'))
 sys.path.insert(0, REF)

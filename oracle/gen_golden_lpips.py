@@ -1,5 +1,5 @@
 """Generate tests/golden/lpips_alex.pt from the UNMODIFIED reference LPIPS network
-(/root/reference/codes/PerceptualSimilarity/models/networks_basic.py: PNetLin(pnet_type='alex')) on CPU.
+(<DASR checkout>/codes/PerceptualSimilarity/models/networks_basic.py: PNetLin(pnet_type='alex')) on CPU.
 The AlexNet trunk gets synthetic weights (no torchvision checkpoint offline); the five linear layers are the reference's
 own weights/v0.1/alex.pth (stored in the fixture: 1152 floats).  Test infrastructure only."""
 import os
@@ -7,7 +7,7 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-REF = '/root/reference/codes'
+REF = os.path.join(os.environ.get('DASR_REFERENCE', 'DASR'), 'codes')   # a ShuhangGu/DASR checkout
 sys.path.insert(0, os.path.join(HERE, 'ref_stubs'))
 sys.path.insert(0, REF)
 sys.path.insert(0, ROOT)

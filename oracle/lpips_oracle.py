@@ -1,7 +1,7 @@
 """CPU oracle for LPIPS v0.1 (AlexNet trunk, linear calibration) — TEST INFRASTRUCTURE ONLY; prepared for the next row of
 SURVEY.md §8f (feature_criterion "LPIPS" of three shipped DASR configs and the validation metric).
 
-Restates /root/reference/codes/PerceptualSimilarity: models/util.py:26-44 (PerceptualLoss.forward with normalize=True),
+Restates <DASR checkout>/codes/PerceptualSimilarity: models/util.py:26-44 (PerceptualLoss.forward with normalize=True),
 networks_basic.py:27-107 (PNetLin, ScalingLayer, NetLinLayer in eval mode), pretrained_networks.py:57-96 (AlexNet
 slices relu1..relu5), util.normalize_tensor (eps 1e-10) and the spatial average.  Pinned by tests/golden/lpips_alex.pt
 (oracle/gen_golden_lpips.py drives the reference's PNetLin with synthetic AlexNet conv weights — the torchvision

@@ -5,7 +5,7 @@ Nothing under ``dasr_b200/`` may import this module: only ``tests/``, ``__graft_
 ``bench.py``'s cpu-baseline / ``--impl reference`` legs use it, and only as the checker / CPU baseline.
 
 Pinning: every function below is checked against outputs of the *imported reference itself*
-(``/root/reference/codes/SRN``) through the fixtures in ``tests/golden/`` produced by
+(``<DASR checkout>/codes/SRN``) through the fixtures in ``tests/golden/`` produced by
 ``oracle/gen_golden.py`` (see tests/test_oracle_golden.py).  Exceptions, stated as the task demands:
   * ``haar_split``: the reference calls ``pytorch_wavelets.DWTForward(J=1, wave='haar', mode='reflect')``
     (DASR_model.py:15,56,442-452), a third-party package that is neither vendored nor installed and

@@ -15,7 +15,7 @@ os.environ.setdefault('DASR_B200_ALLOW_RANDOM_VGG', '1')
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box with -m gpu)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on an H100 with -m gpu)')
 
 
 def pytest_collection_modifyitems(config, items):
@@ -37,5 +37,15 @@ def golden():
     import torch
 
     def load(name):
-        return torch.load(os.path.join(GOLDEN, name), weights_only=False)
+        # fixtures above 1 MB are stored as a skeleton NAME.pt plus NAME.partK.pt files, each {key path: tensor}
+        obj = torch.load(os.path.join(GOLDEN, name), weights_only=False)
+        k = 1
+        while os.path.exists(os.path.join(GOLDEN, '%s.part%d.pt' % (name[:-3], k))):
+            for path, t in torch.load(os.path.join(GOLDEN, '%s.part%d.pt' % (name[:-3], k)), weights_only=False).items():
+                o = obj
+                for key in path[:-1]:
+                    o = o[key]
+                o[path[-1]] = t
+            k += 1
+        return obj
     return load

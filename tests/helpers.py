@@ -83,8 +83,7 @@ def as_good_as_reference(got, ref, truth, tol=1e-3):
       3. isolated LeakyReLU kink flips: a pre-activation within fp32 rounding of zero takes the other slope in two correct
          fp32 implementations (among ~1e7 activations it happens to a few), which moves the gradients downstream of that one
          element by up to ~1e-2 of the maximum while everything else agrees to 1e-6.  tools/debug_f1b.py shows torch's own
-         GPU operators, our kernels and the CPU reference each hit by it on different sub-chains
-         (profiles/r2_kink_flips.txt).  Accepted: rel-L2 error vs truth < 5e-3 and rel-L-inf < 5e-2."""
+         GPU operators, our kernels and the CPU reference each hit by it on different sub-chains.  Accepted: rel-L2 error vs truth < 5e-3 and rel-L-inf < 5e-2."""
     got, ref, truth = got.detach().double().cpu(), ref.detach().double().cpu(), truth.detach().double().cpu()
     if float((got - ref).abs().max() / ref.abs().max().clamp_min(1e-30)) < tol:
         return True

@@ -1,6 +1,6 @@
 """Data-parallel equivalence on real GPUs (SURVEY §4 iv, §8e): a 2-rank DASR_Model step with B_local crops per rank
 (torchrun, NCCL) must produce the gradients and post-Adam weights of a single-GPU step on the concatenated batch.
-Needs 2 GPUs (`gpurun --gpus 2`); skipped on a single-GPU box."""
+Needs 2 GPUs; skipped on a single-GPU machine."""
 import os
 import subprocess
 import sys

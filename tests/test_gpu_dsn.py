@@ -59,7 +59,7 @@ def test_de_resnet_vs_golden(golden):
 
 
 def test_de_resnet_mixed_precision_vs_golden(golden):
-    """tcgen05 trunk (bf16 activations, fp32 accumulate / master weights / filter gradients) against the fp32 reference:
+    """wgmma trunk (bf16 activations, fp32 accumulate / master weights / filter gradients) against the fp32 reference:
     output within bf16 tolerance, every parameter gradient within 15 % rel-L2 (bf16 activation gradients through 6 layers)."""
     from dasr_b200.dsn.model import De_resnet
     g = golden('dsn_de_resnet.pt')

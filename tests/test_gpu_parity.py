@@ -1,6 +1,6 @@
 """GPU parity tests: the CUDA path (through the C ABI) against the CPU oracle and the committed golden
 fixtures generated from the reference.  Tolerances: fp32 mode 1e-3 relative L-inf (BASELINE north_star;
-measured ~1e-6), bf16 tcgen05 mode 3e-2 relative L-inf on activations (operand rounding, SURVEY H2)."""
+measured ~1e-6), bf16 wgmma mode 3e-2 relative L-inf on activations (operand rounding, SURVEY H2)."""
 import numpy as np
 import pytest
 import torch
@@ -108,7 +108,7 @@ def test_rrdbnet_bf16_translation_property():
 
 
 def test_rrdbnet_bf16_training_gradients_vs_oracle():
-    """Mixed-precision training mode (tcgen05 fprop + dgrad, fp32-accumulated wgrad on bf16 activations): gradients
+    """Mixed-precision training mode (wgmma fprop + dgrad, fp32-accumulated wgrad on bf16 activations): gradients
     agree with the fp32 oracle to bf16 accuracy (relative L2 error per tensor; tolerance 0.12: bf16 activation gradients through 17 convs; the wgrad kernel itself is exact)."""
     nb = 1
     sd = O.synth_state_dict(O.rrdbnet_shapes(nb=nb), 131, 0.3)
@@ -211,7 +211,7 @@ def test_vgg19_vs_golden(golden):
 
 
 def test_vgg19_bf16_tensor_core_path_vs_golden(golden):
-    """Mixed-precision perceptual-loss network (tcgen05 convs, bf16 activations): features and input gradient
+    """Mixed-precision perceptual-loss network (wgmma convs, bf16 activations): features and input gradient
     against the fp32 reference within bf16 tolerances (rel-L2; 16 stacked bf16 layers)."""
     from dasr_b200.srn.models.modules.architecture import VGGFeatureExtractor
     g = golden('vgg19.pt')
@@ -238,7 +238,7 @@ def test_vgg19_bf16_tensor_core_path_vs_golden(golden):
 
 @pytest.mark.parametrize('cin,cout,h,w', [(64, 128, 20, 12), (256, 256, 9, 17), (512, 512, 8, 8), (32, 64, 16, 8)])
 def test_conv_tc_wide_channel_tiles(cin, cout, h, w):
-    """tcgen05 fprop / dgrad with the filters split in Cout tiles (VGG19 widths) against torch fp32 convs on the
+    """wgmma fprop / dgrad with the filters split in Cout tiles (VGG19 widths) against torch fp32 convs on the
     same bf16-rounded operands."""
     import torch.nn.functional as F
     from dasr_b200 import engine, ops

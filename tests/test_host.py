@@ -209,25 +209,55 @@ def test_dsn_modules_match_reference_state_dict_layout():
         net(torch.zeros(1, 3, 16, 16))
 
 
+def _stub_checkout(root):
+    """A stand-in for a DASR `codes/` tree: the SRN and DSN directories hold their own `models` / `options` / `utils` and
+    `model` / `loss` modules (which must lose against the mirrors) and small entry scripts with the import statements of
+    the real ones.  `codes/Auto_Reproduce.py` starts the stages the way the real one does (`cd ./DSN; sh ...`,
+    `cd ./SRN; python train.py -opt ...`)."""
+    srn, dsn = root / 'SRN', root / 'DSN'
+    for pkg in ('models', 'options', 'utils'):
+        (srn / pkg).mkdir(parents=True)
+        (srn / pkg / '__init__.py').write_text("ORIGIN = 'checkout'\n")
+    (srn / 'options' / 'options.py').write_text("ORIGIN = 'checkout'\n")
+    (srn / 'utils' / 'util.py').write_text("ORIGIN = 'checkout'\n")
+    dsn.mkdir()
+    for mod in ('model', 'loss'):
+        (dsn / (mod + '.py')).write_text("ORIGIN = 'checkout'\n")
+    (srn / 'test.py').write_text(
+        "import sys\n"
+        "import torch\n"
+        "import options.options as option\n"
+        "import utils.util as util\n"
+        "from models import create_model\n"
+        "opt = option.dict_to_nonedict(option.parse(sys.argv[sys.argv.index('-opt') + 1], is_train=False))\n"
+        "model = create_model(opt)\n"
+        "model.feed_data({'LR': torch.rand(1, 3, 16, 16)}, need_HR=False)\n"
+        "model.test()\n")
+    (srn / 'train.py').write_text(
+        "import options.options as option\n"
+        "import utils.util as util\n"
+        "import models\n"
+        "print('SRN stage:', option.__file__, util.__file__, models.__file__)\n")
+    (dsn / 'train.py').write_text(
+        "import model\n"
+        "import loss\n"
+        "print('DSN stage:', model.__file__, loss.__file__)\n")
+    (dsn / 'auto_reproduce_launcher_realsr.sh').write_text('"%s" train.py --per_type VGG --filter wavelet\n' % sys.executable)
+    (root / 'Auto_Reproduce.py').write_text(
+        "import os\n"
+        "os.system('cd ./DSN; sh auto_reproduce_launcher_realsr.sh')\n"
+        "os.system('cd ./SRN; \"%s\" train.py -opt options/train/train_DASR.json')\n" % sys.executable)
+    return srn, dsn
+
+
 def test_reference_test_py_runs_unchanged_through_the_launcher(tmp_path):
-    """Drop-in boundary: the reference's own codes/SRN/test.py, executed unchanged by dasr_b200.launch, parses its JSON,
-    builds its dataset/dataloader with the reference's data/ package, creates the model through the mirror and reaches
-    the first kernel call — which must refuse loudly on this GPU-less host (no CPU fallback).  Skipped where the
-    reference checkout is absent (the GPU box)."""
+    """Drop-in boundary: an SRN entry script whose own directory holds `models` / `options` / `utils` packages, run by
+    dasr_b200.launch, parses its JSON with the mirrored options, creates the model through the mirror and reaches the
+    first kernel call — which must refuse loudly on a host without a GPU (no CPU fallback)."""
     import json
-    import subprocess
-    import sys
-    import numpy as np
-    import pytest
-    ref = '/root/reference/codes/SRN/test.py'
-    if not os.path.exists(ref):
-        pytest.skip('reference checkout not present')
-    cv2 = pytest.importorskip('cv2')
-    rng = np.random.RandomState(0)
+    srn, _ = _stub_checkout(tmp_path / 'codes')
     (tmp_path / 'LR').mkdir()
     (tmp_path / 'HR').mkdir()
-    cv2.imwrite(str(tmp_path / 'LR' / 'a.png'), (rng.rand(16, 16, 3) * 255).astype(np.uint8))
-    cv2.imwrite(str(tmp_path / 'HR' / 'a.png'), (rng.rand(64, 64, 3) * 255).astype(np.uint8))
     opt = {'name': 'dropin_test', 'suffix': None, 'model': 'sr', 'scale': 4, 'gpu_ids': None, 'chop': False, 'val_lpips': False,
            'save_RealorFake': False,
            'datasets': {'test_1': {'name': 'toy', 'mode': 'LRHR', 'dataroot_HR': str(tmp_path / 'HR'), 'dataroot_LR': str(tmp_path / 'LR')}},
@@ -236,28 +266,22 @@ def test_reference_test_py_runs_unchanged_through_the_launcher(tmp_path):
                          'gc': 32, 'group': 1}}
     cfg = tmp_path / 'test.json'
     cfg.write_text(json.dumps(opt))
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    env = dict(os.environ, PYTHONPATH=os.pathsep.join([root, os.path.join(root, 'oracle', 'ref_stubs')]), CUDA_VISIBLE_DEVICES='')
-    r = subprocess.run([sys.executable, '-m', 'dasr_b200.launch', ref, '-opt', str(cfg)], cwd=str(tmp_path), env=env,
+    env = dict(os.environ, PYTHONPATH=os.pathsep.join([ROOT, os.path.join(ROOT, 'oracle', 'ref_stubs')]), CUDA_VISIBLE_DEVICES='')
+    r = subprocess.run([sys.executable, '-m', 'dasr_b200.launch', str(srn / 'test.py'), '-opt', str(cfg)], cwd=str(tmp_path), env=env,
                        capture_output=True, text=True, timeout=600)
     err = r.stderr + r.stdout
     assert r.returncode != 0
-    assert 'dasr_b200/srn/models/SR_model.py' in err, err[-2000:]          # the mirror, not the reference's models package
+    assert 'dasr_b200/srn/models/SR_model.py' in err, err[-2000:]          # the mirror, not the checkout's models package
     assert 'no CPU fallback exists' in err, err[-2000:]
 
 
 def test_auto_reproduce_resolves_to_the_mirrors_after_install(tmp_path):
-    """`python -m dasr_b200.install <codes>` + the unmodified Auto_Reproduce.py (Auto_Reproduce.py:38-40 shells out to
-    `cd ./DSN; sh auto_reproduce_launcher_<dataset>.sh` and `cd ./SRN; python train.py -opt ...`): both child scripts must
-    import the dasr_b200 mirrors although their own directory is first on sys.path.  The stages stop at the datasets
-    (no data here); the overlay log records which imports were redirected for which script directory."""
-    import shutil
-    import pytest
-    ref = '/root/reference/codes'
-    if not os.path.exists(os.path.join(ref, 'Auto_Reproduce.py')):
-        pytest.skip('reference checkout not present')
+    """`python -m dasr_b200.install <codes>` + an Auto_Reproduce.py that shells out to `cd ./DSN; sh ...` and
+    `cd ./SRN; python train.py -opt ...`: both child scripts must import the dasr_b200 mirrors although their own directory
+    (holding modules of the same names) is first on sys.path.  The overlay log records which imports were redirected for
+    which script directory."""
     codes = tmp_path / 'codes'
-    shutil.copytree(ref, str(codes), ignore=shutil.ignore_patterns('*.tar', '*.png', '*.jpg', '*.pyc', '__pycache__', '*.gif'))
+    srn, dsn = _stub_checkout(codes)
     from dasr_b200 import install
     import io
     buf = io.StringIO()
@@ -269,11 +293,12 @@ def test_auto_reproduce_resolves_to_the_mirrors_after_install(tmp_path):
     r = subprocess.run([sys.executable, 'Auto_Reproduce.py', '--dataset', 'realsr', '--artifact', 'tdrealsr'], cwd=str(codes), env=env,
                        capture_output=True, text=True, timeout=900)
     text = log.read_text() if log.exists() else ''
-    dsn_dir, srn_dir = str(codes / 'DSN'), str(codes / 'SRN')
+    dsn_dir, srn_dir = str(dsn), str(srn)
     for name in ('model', 'loss'):
         assert any(l.startswith(name + ' -> ') and 'dasr_b200/dsn/' in l and dsn_dir in l for l in text.splitlines()), (name, text, r.stderr[-3000:])
     for name in ('options', 'utils', 'models'):
         assert any(l.startswith(name + ' -> ') and 'dasr_b200/srn/' in l and srn_dir in l for l in text.splitlines()), (name, text, r.stderr[-3000:])
+    assert 'DSN stage:' in r.stdout and 'SRN stage:' in r.stdout and os.path.join(srn_dir, 'models') not in r.stdout, r.stdout[-2000:]
     # an unmarked directory is left alone
     install.uninstall(str(codes), out=buf)
     assert not (codes / 'SRN' / '.dasr_b200').exists()

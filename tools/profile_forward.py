@@ -1,6 +1,6 @@
 """One RRDBNet-23 bf16 forward (BASELINE configs[1] shape) between cudaProfilerStart/Stop, for ncu:
    ncu --profile-from-start off --metrics gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum \
-       --clock-control none --csv --log-file gpurun_out/launches.csv python tools/profile_forward.py
+       --clock-control none --csv --log-file profiling/launches.csv python tools/profile_forward.py
 """
 import os
 import sys

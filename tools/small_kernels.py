@@ -1,10 +1,10 @@
-"""Workload for the per-kernel ncu pass over everything that is NOT the tcgen05 conv (VERDICT r1 weak #8): one DASR train step
+"""Workload for the per-kernel ncu pass over everything that is NOT the wgmma conv (VERDICT r1 weak #8): one DASR train step
 in the fp32 parity mode and one in the mixed-precision mode (configs[2], no CUDA graphs), one DSN iteration in each mode
 (configs[4]), an LPIPS loss forward / backward, a BatchNorm discriminator forward / backward, a domain-distance map.
 
   DASR_B200_GRAPH=0 ncu --metrics gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum \\
-      --clock-control none --csv --log-file gpurun_out/r2_small_kernels.csv python tools/small_kernels.py
-  python tools/summarize_small_kernels.py gpurun_out/r2_small_kernels.csv > profiles/r2_small_kernels.md
+      --clock-control none --csv --log-file profiling/small_kernels.csv python tools/small_kernels.py
+  python tools/summarize_small_kernels.py profiling/small_kernels.csv
 """
 import os
 import sys
