@@ -49,6 +49,7 @@ class ConvTcParams(C.Structure):
         ('a_mode', C.c_int), ('epi_mode', C.c_int), ('act_cols', C.c_int),
         ('pre_cs', C.c_int), ('pre_coff', C.c_int), ('out_nc', C.c_int), ('tile_rev', C.c_int),
         ('nchunk_list', C.c_int), ('chunk_off', C.c_int * 8), ('f16', C.c_int),
+        ('map_mode', C.c_int), ('map_scale', C.c_float), ('map_stride', C.c_int),
     ]
 
 
@@ -77,6 +78,8 @@ SYMBOLS = {
     'dasr_conv_tc': (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.POINTER(ConvTcParams), _vp]),
     'dasr_conv_tc2_supported': (_i, [C.POINTER(ConvTcParams)]),
     'dasr_conv_tc2': (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, C.POINTER(ConvTcParams), _vp]),
+    'dasr_conv_tc_map': (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.POINTER(ConvTcParams), _vp]),
+    'dasr_conv_tc2_map': (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.POINTER(ConvTcParams), _vp]),
     'dasr_conv_tc_setup': (_i, [C.POINTER(ConvTcParams), _i]),
     'dasr_pack_filter_tc_bytes': (_sz, [_i, _i, _i]),
     'dasr_pack_filter_tc': (_i, [_vp, _vp, _i, _i, _i, _vp]),
@@ -85,6 +88,7 @@ SYMBOLS = {
     'dasr_act_bwd': (_i, [_vp, _vp, _l, _i, _i, _i, _i, _i, _f, _i, _vp]),
     'dasr_upsample2x_bwd': (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
     'dasr_axpby': (_i, [_vp, _vp, _vp, _l, _i, _i, _i, _i, _i, _i, _i, _f, _f, _i, _vp]),
+    'dasr_map_axpby': (_i, [_vp, _vp, _vp, _vp, _l, _i, _i, _i, _i, _i, _i, _i, _f, _f, _vp]),
     'dasr_maxpool2_fwd': (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
     'dasr_maxpool2_bwd': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     'dasr_maxpool2_fwd_bf16': (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),

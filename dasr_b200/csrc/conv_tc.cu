@@ -59,6 +59,8 @@ struct TcKernelArgs {
   int has_pre, has_res1, has_res2;
   int nbuf;          // staged-epilogue tile buffers (2..4): pre / residual tiles are requested nbuf tiles ahead
   int pair;          // 1: launched as (1, 2, 1) clusters, A tiles multicast by the leader (rank 0)
+  const float* map;  // weight map [N][H][W] fp32 (image stride p.map_stride), MAP != 0 only
+  const float* map_w;// MAP 1: the map channel's filter taps [9][cout] fp32
 };
 
 __device__ __forceinline__ float2 h16x2_to_f2(uint32_t u, int f16) {
@@ -125,7 +127,9 @@ __device__ __forceinline__ void issue_tap_rt(int nt, float* acc, uint32_t a_addr
 }
 
 // EPI_MODE / HAS_PRE / NRES are compile-time so that each instantiation carries only its own epilogue code.
-template <int EPI_MODE, bool HAS_PRE, int NRES>
+// MAP (staged epilogue only): 0 = no weight map; DASR_MAP_CHANNEL = one more input channel map_scale * map convolved with
+// the 3x3 taps map_w, added before the activation; DASR_MAP_SCALE = v = map * (alpha * act(...) + beta1 * res1) + beta2 * res2.
+template <int EPI_MODE, bool HAS_PRE, int NRES, int MAP = 0>
 __global__ void __launch_bounds__(TCK_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ CUtensorMap tmap_w,
                const __grid_constant__ EpiMaps em, const TcKernelArgs a) {
@@ -458,6 +462,18 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
           const bool valid = (y < p.H) && (x < p.W);
           const int oy = y * p.out_mul + p.out_py[var], ox = x * p.out_mul + p.out_px[var];
           const long opix = ((long)n * OH + oy) * OW + ox;
+          // the map around this pixel (zero outside the image): the 3x3 neighbourhood, or the pixel's own value
+          float mv[MAP == DASR_MAP_CHANNEL ? 9 : 1];
+          if constexpr (MAP == DASR_MAP_CHANNEL) {
+            const float* mp = a.map + (long)n * p.map_stride;
+#pragma unroll
+            for (int t = 0; t < 9; t++) {
+              const int yy = y + t / 3 - 1, xx = x + t % 3 - 1;
+              mv[t] = (yy >= 0 && yy < p.H && xx >= 0 && xx < p.W) ? p.map_scale * __ldg(mp + (long)yy * p.W + xx) : 0.f;
+            }
+          } else if constexpr (MAP == DASR_MAP_SCALE) {
+            mv[0] = valid ? __ldg(a.map + (long)n * p.map_stride + (long)y * p.W + x) : 0.f;
+          }
 #pragma unroll
           for (int j = 0; j < ACC_REGS / 4; j++) {
             if (j < (nt >> 3)) {
@@ -471,6 +487,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
                 if constexpr (HAS_PRE) {
                   const float2 q = h16x2_to_f2(lds32(bS + o), f16);
                   v0 += q.x; v1 += q.y;
+                }
+                if constexpr (MAP == DASR_MAP_CHANNEL) {
+                  const float* wa = a.map_w + co;
+#pragma unroll
+                  for (int t = 0; t < 9; t++) {
+                    v0 = fmaf(mv[t], __ldg(wa + t * p.cout), v0);
+                    v1 = fmaf(mv[t], __ldg(wa + t * p.cout + 1), v1);
+                  }
                 }
                 if (do_act) {
                   if (act == DASR_ACT_LRELU) { v0 = fmaxf(v0, v0 * slope); v1 = fmaxf(v1, v1 * slope); }   // 0 < slope < 1
@@ -489,6 +513,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
                     v0 = fmaf(p.beta1, q.x, v0); v1 = fmaf(p.beta1, q.y, v1);
                   }
                 }
+                if constexpr (MAP == DASR_MAP_SCALE) { v0 *= mv[0]; v1 *= mv[0]; }
                 if constexpr (NRES >= 2) {
                   const float2 q = h16x2_to_f2(lds32(bR2 + o), f16);
                   v0 = fmaf(p.beta2, q.x, v0); v1 = fmaf(p.beta2, q.y, v1);
@@ -693,6 +718,9 @@ int dasr_conv_tc_setup(DasrConvTcParams* p, int kind) {
   if (!p) return DASR_E_BADARG;
   p->nchunk_list = 0;
   p->f16 = 0;
+  p->map_mode = 0;
+  p->map_scale = 0.f;
+  p->map_stride = 0;
   if (kind == 0 || kind == 1) {
     p->nvar = 1;
     p->ntaps = 9;
@@ -817,7 +845,8 @@ static int chunk64_allowed() {
 
 // pair = 1: (1, 2, 1) clusters, p->nt is the Cout tile of ONE CTA (half of the pair's tile)
 static int conv_tc_launch(const void* in, const void* w, const float* bias, const void* pre, const void* res1, const void* res2,
-                          const void* mask_src, void* out, const DasrConvTcParams* p, void* stream, int pair) {
+                          const void* mask_src, void* out, const DasrConvTcParams* p, void* stream, int pair,
+                          const float* map = nullptr, const float* map_w = nullptr) {
   PFN_encodeTiled enc = get_encode();
   if (!enc) {
     set_error("conv_tc: cuTensorMapEncodeTiled not available");
@@ -832,6 +861,8 @@ static int conv_tc_launch(const void* in, const void* w, const float* bias, cons
   a.mask_src = (const __nv_bfloat16*)mask_src;
   a.out = out;
   a.pair = pair;
+  a.map = map;
+  a.map_w = map_w;
   a.nchunks = p->cin / CHUNK;
   a.n_ntiles = p->cout / p->nt;
   a.tiles_x = cdiv(p->W, TILE_W);
@@ -915,13 +946,18 @@ static int conv_tc_launch(const void* in, const void* w, const float* bias, cons
   }
 
   typedef void (*KernelFn)(const CUtensorMap, const CUtensorMap, const EpiMaps, const TcKernelArgs);
-  static const KernelFn kernels[9] = {
+  static const KernelFn kernels[12] = {
       conv_tc_kernel<0, false, 0>, conv_tc_kernel<0, false, 1>, conv_tc_kernel<0, false, 2>,
       conv_tc_kernel<0, true, 0>,  conv_tc_kernel<0, true, 1>,  conv_tc_kernel<0, true, 2>,
-      conv_tc_kernel<1, false, 0>, conv_tc_kernel<2, false, 0>, conv_tc_kernel<3, false, 0>};
-  const int ki = (p->epi_mode == 0) ? (a.has_pre * 3 + a.has_res1 + a.has_res2) : (5 + p->epi_mode);
+      conv_tc_kernel<1, false, 0>, conv_tc_kernel<2, false, 0>, conv_tc_kernel<3, false, 0>,
+      // weight-map variants (dasr_conv_tc_map / dasr_conv_tc2_map)
+      conv_tc_kernel<0, false, 0, DASR_MAP_CHANNEL>, conv_tc_kernel<0, false, 2, DASR_MAP_SCALE>,
+      conv_tc_kernel<0, true, 2, DASR_MAP_SCALE>};
+  int ki = (p->epi_mode == 0) ? (a.has_pre * 3 + a.has_res1 + a.has_res2) : (5 + p->epi_mode);
+  if (p->map_mode == DASR_MAP_CHANNEL) ki = 9;
+  else if (p->map_mode == DASR_MAP_SCALE) ki = 10 + a.has_pre;
   if (p->epi_mode == 0) DASR_REQUIRE(!(a.has_res2 && !a.has_res1), "conv_tc: res2 without res1");
-  static bool attr_set[9] = {false, false, false, false, false, false, false, false, false};
+  static bool attr_set[12] = {false, false, false, false, false, false, false, false, false, false, false, false};
   if (!attr_set[ki]) {
     cudaError_t e = cudaFuncSetAttribute(kernels[ki], cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
     if (e != cudaSuccess) {
@@ -959,8 +995,9 @@ static int conv_tc_launch(const void* in, const void* w, const float* bias, cons
   return check_launch(pair ? "conv_tc2" : "conv_tc");
 }
 
-int dasr_conv_tc(const void* in, const void* w, const float* bias, const void* pre, const void* res1, const void* res2,
-                 const void* mask_src, void* out, const DasrConvTcParams* p, void* stream) {
+static int conv_tc_run(const void* in, const void* w, const float* bias, const void* pre, const void* res1, const void* res2,
+                       const void* mask_src, void* out, const DasrConvTcParams* p, void* stream, const float* map,
+                       const float* map_w) {
   DASR_REQUIRE(p && in && w && out, "conv_tc: null argument");
   DASR_REQUIRE(p->N > 0 && p->H > 0 && p->W > 0, "conv_tc: bad dims");
   DASR_REQUIRE((long)p->N * cdiv(p->W, TILE_W) * cdiv(p->H, TILE_H) < (1L << 30), "conv_tc: too many tiles for 32-bit tile arithmetic");
@@ -1004,7 +1041,42 @@ int dasr_conv_tc(const void* in, const void* w, const float* bias, const void* p
                "conv_tc: pointers must be 16-byte aligned");
   DasrConvTcParams q = *p;
   if (p->epi_mode == 0) q.mask_c0 = q.mask_c1 = 0;   // the staged epilogue's mask mode belongs to dasr_conv_tc2
-  return conv_tc_launch(in, w, bias, pre, res1, res2, mask_src, out, &q, stream, 0);
+  return conv_tc_launch(in, w, bias, pre, res1, res2, mask_src, out, &q, stream, 0, map, map_w);
+}
+
+int dasr_conv_tc(const void* in, const void* w, const float* bias, const void* pre, const void* res1, const void* res2,
+                 const void* mask_src, void* out, const DasrConvTcParams* p, void* stream) {
+  DASR_REQUIRE(p, "conv_tc: null argument");
+  DasrConvTcParams q = *p;
+  q.map_mode = 0;                       // the weight map belongs to dasr_conv_tc_map
+  return conv_tc_run(in, w, bias, pre, res1, res2, mask_src, out, &q, stream, nullptr, nullptr);
+}
+
+// the weight-map operand: checks shared by dasr_conv_tc_map and dasr_conv_tc2_map
+static int check_map(const DasrConvTcParams* p, const void* pre, const void* res1, const void* res2, const float* map,
+                     const float* map_w, const char* who) {
+  DASR_REQUIRE(p->map_mode == DASR_MAP_CHANNEL || p->map_mode == DASR_MAP_SCALE, "%s: map_mode must be DASR_MAP_CHANNEL or "
+               "DASR_MAP_SCALE (got %d)", who, p->map_mode);
+  DASR_REQUIRE(p->epi_mode == 0 && p->out_mul == 1 && p->nvar == 1 && p->ntaps == 9 && p->a_mode == 0,
+               "%s: the weight map needs the plain 3x3 geometry (dasr_conv_tc_setup kind 0) and the staged epilogue", who);
+  DASR_REQUIRE(map && (reinterpret_cast<uintptr_t>(map) & 3) == 0, "%s: map must be a non-null fp32 pointer", who);
+  DASR_REQUIRE(p->map_stride >= p->W && (long)p->map_stride >= (long)p->H * p->W,
+               "%s: map image stride %d is below H*W = %ld", who, p->map_stride, (long)p->H * p->W);
+  DASR_REQUIRE(p->mask_c1 <= p->mask_c0, "%s: no dgrad mask together with the weight map", who);
+  if (p->map_mode == DASR_MAP_CHANNEL)
+    DASR_REQUIRE(map_w && (reinterpret_cast<uintptr_t>(map_w) & 3) == 0 && !pre && !res1 && !res2,
+                 "%s: DASR_MAP_CHANNEL needs the map channel's filter taps (map_w) and takes no pre / residual inputs", who);
+  else
+    DASR_REQUIRE(res1 && res2, "%s: DASR_MAP_SCALE needs res1 and res2", who);
+  return DASR_OK;
+}
+
+int dasr_conv_tc_map(const void* in, const void* w, const float* bias, const void* pre, const void* res1, const void* res2,
+                     const float* map, const float* map_w, void* out, const DasrConvTcParams* p, void* stream) {
+  DASR_REQUIRE(p, "conv_tc_map: null argument");
+  const int rc = check_map(p, pre, res1, res2, map, map_w, "conv_tc_map");
+  if (rc) return rc;
+  return conv_tc_run(in, w, bias, pre, res1, res2, nullptr, out, p, stream, map, map_w);
 }
 
 // ---- cluster pair: the two Cout halves of a tile on two SMs of a (1, 2, 1) cluster, A tiles multicast ----
@@ -1025,8 +1097,8 @@ int dasr_conv_tc2_supported(const DasrConvTcParams* p) {
   return tc2_fits(p, (p->res1_cs > 0 ? 1 : 0) + (p->res2_cs > 0 ? 1 : 0));
 }
 
-int dasr_conv_tc2(const void* in, const void* w, const float* bias, const void* pre, const void* res1, const void* res2,
-                  void* out, const DasrConvTcParams* p, void* stream) {
+static int conv_tc2_run(const void* in, const void* w, const float* bias, const void* pre, const void* res1, const void* res2,
+                        void* out, const DasrConvTcParams* p, void* stream, const float* map, const float* map_w) {
   DASR_REQUIRE(p && in && w && out, "conv_tc2: null argument");
   DASR_REQUIRE(p->nvar == 1 && p->ntaps == 9 && p->out_mul == 1 && p->epi_mode == 0 && p->a_mode == 0,
                "conv_tc2: plain 3x3 geometry with the staged epilogue only");
@@ -1057,7 +1129,23 @@ int dasr_conv_tc2(const void* in, const void* w, const float* bias, const void* 
   }
   DasrConvTcParams q = *p;
   q.nt = p->nt / 2;                     // per CTA; grid.y = cout / (nt / 2), consecutive CTAs form the clusters
-  return conv_tc_launch(in, w, bias, pre, res1, res2, nullptr, out, &q, stream, 1);
+  return conv_tc_launch(in, w, bias, pre, res1, res2, nullptr, out, &q, stream, 1, map, map_w);
+}
+
+int dasr_conv_tc2(const void* in, const void* w, const float* bias, const void* pre, const void* res1, const void* res2,
+                  void* out, const DasrConvTcParams* p, void* stream) {
+  DASR_REQUIRE(p, "conv_tc2: null argument");
+  DasrConvTcParams q = *p;
+  q.map_mode = 0;                       // the weight map belongs to dasr_conv_tc2_map
+  return conv_tc2_run(in, w, bias, pre, res1, res2, out, &q, stream, nullptr, nullptr);
+}
+
+int dasr_conv_tc2_map(const void* in, const void* w, const float* bias, const void* pre, const void* res1, const void* res2,
+                      const float* map, const float* map_w, void* out, const DasrConvTcParams* p, void* stream) {
+  DASR_REQUIRE(p, "conv_tc2_map: null argument");
+  const int rc = check_map(p, pre, res1, res2, map, map_w, "conv_tc2_map");
+  if (rc) return rc;
+  return conv_tc2_run(in, w, bias, pre, res1, res2, out, p, stream, map, map_w);
 }
 
 // selftest-only probe (declared in selftest.cu, not in the public header)

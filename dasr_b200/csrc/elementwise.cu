@@ -218,6 +218,18 @@ __global__ void axpby_kernel(const T* __restrict__ x, const T* __restrict__ y, T
   st<T>(d + pp * d_cs + d_coff + c, v);
 }
 
+__global__ void map_axpby_kernel(const float* __restrict__ x, const float* __restrict__ map, const float* __restrict__ y,
+                                 float* __restrict__ d, long npix, int C, int x_cs, int x_coff, int y_cs, int y_coff,
+                                 int d_cs, int d_coff, float a, float b) {
+  long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= npix * C) return;
+  long pp = i / C;
+  int c = (int)(i - pp * C);
+  float v = map[pp] * (x ? a * x[pp * x_cs + x_coff + c] : a);
+  if (y) v += b * y[pp * y_cs + y_coff + c];
+  d[pp * d_cs + d_coff + c] = v;
+}
+
 __global__ void maxpool2_fwd_kernel(const float* __restrict__ in, float* __restrict__ out, int N, int H, int W, int C) {
   const int OH = H / 2, OW = W / 2;
   long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -827,6 +839,16 @@ int dasr_axpby(const void* x, const void* y, void* dst, long npix, int C, int x_
     axpby_kernel<float><<<cdiv(total, 256), 256, 0, (cudaStream_t)stream>>>(
         (const float*)x, (const float*)y, (float*)dst, npix, C, x_cs, x_coff, y_cs, y_coff, d_cs, d_coff, a, b);
   return check_launch("axpby");
+}
+
+int dasr_map_axpby(const float* x, const float* map, const float* y, float* dst, long npix, int C, int x_cs, int x_coff,
+                   int y_cs, int y_coff, int d_cs, int d_coff, float a, float b, void* stream) {
+  DASR_REQUIRE(npix > 0 && C > 0 && map && dst && d_coff + C <= d_cs && (!x || x_coff + C <= x_cs) && (!y || y_coff + C <= y_cs),
+               "map_axpby: bad arguments");
+  const long total = npix * C;
+  map_axpby_kernel<<<cdiv(total, 256), 256, 0, (cudaStream_t)stream>>>(x, map, y, dst, npix, C, x_cs, x_coff, y_cs, y_coff,
+                                                                       d_cs, d_coff, a, b);
+  return check_launch("map_axpby");
 }
 
 int dasr_bias_grad(const void* dout, float* db, long npix, int C, int cs, int coff, int is_bf16, int accumulate,

@@ -71,6 +71,50 @@ def _rdb_cin(nf, k):
     return nf + (k - 1) * GC
 
 
+def _rrdb_tail(bufs, r, nf):
+    """conv5 epilogue of dense block r of an RRDB chain: x5*0.2 + x, and for the last block of an RRDB
+    (x5*0.2 + x)*0.2 + x_rrdb (block.py:286,309)."""
+    b = bufs[r]
+    if r % 3 == 2:
+        return dict(alpha=0.04, res1=View(b, nf, 0), beta1=0.2, res2=View(bufs[r - 2], nf, 0), beta2=1.0)
+    return dict(alpha=0.2, res1=View(b, nf, 0), beta1=1.0)
+
+
+def _rdb_f32(b, dst, r, L, pk, Bs, tail):
+    """fp32 dense block r: conv1..4 (+LeakyReLU) into the concat buffer b, conv5 -> dst with the epilogue `tail`."""
+    nf = L.nf
+    for k in range(1, 5):
+        ci = L.rdb_conv(r, k)
+        ops.conv2d_f32(View(b, _rdb_cin(nf, k), 0), pk(ci), Bs(ci), View(b, GC, nf + (k - 1) * GC), 3, 1, 1,
+                       act=ACT_LRELU, slope=0.2)
+    ci = L.rdb_conv(r, 5)
+    ops.conv2d_f32(View(b, nf + 4 * GC, 0), pk(ci), Bs(ci), dst, 3, 1, 1, **tail)
+
+
+def _trunk_tail_f32(trunk, fea, L, params, pk, Bs):
+    """fea + LR_conv(trunk) -> nearest-x2 upconvs -> HR_conv0 -> HR_conv1 (fp32).  Returns (out NCHW, ups, h0)."""
+    x = fea
+    N, H, W, nf = fea.shape
+    lr = _empty((N, H, W, nf), x)
+    ops.conv2d_f32(trunk, pk(L.i_lr), Bs(L.i_lr), lr, 3, 1, 1, res1=fea, beta1=1.0)   # fea + LR_conv(...)  block.py:103-105
+    ups = [lr]
+    cur, h, w = lr, H, W
+    for u in range(L.n_up):
+        h, w = 2 * h, 2 * w
+        nxt = _empty((N, h, w, nf), x)
+        ops.conv2d_f32(cur, pk(L.i_up0 + u), Bs(L.i_up0 + u), nxt, 3, 1, 1, ups=2, act=ACT_LRELU)
+        ups.append(nxt)
+        cur = nxt
+    h0 = _empty((N, h, w, nf), x)
+    ops.conv2d_f32(cur, pk(L.i_hr0), Bs(L.i_hr0), h0, 3, 1, 1, act=ACT_LRELU)
+    out_nc = params[2 * L.i_hr1].shape[0]
+    o = _empty((N, h, w, out_nc), x)
+    ops.conv2d_f32(h0, pk(L.i_hr1), Bs(L.i_hr1), o, 3, 1, 1)
+    out = _empty((N, out_nc, h, w), x)
+    ops.nhwc_to_nchw(o, out)
+    return out, ups, h0
+
+
 def rrdb_forward_f32(x, params, nb, upscale=4, save=False):
     """fp32 forward.  Returns (out NCHW fp32, ctx or None)."""
     _need_cuda(x, 'RRDBNet')
@@ -95,36 +139,8 @@ def rrdb_forward_f32(x, params, nb, upscale=4, save=False):
         bufs = [rot[i % 3] for i in range(n_rdb + 1)]
     ops.axpby(fea, 1.0, None, 0.0, View(bufs[0], nf, 0))
     for r in range(n_rdb):
-        b = bufs[r]
-        for k in range(1, 5):
-            ci = L.rdb_conv(r, k)
-            ops.conv2d_f32(View(b, _rdb_cin(nf, k), 0), pk(ci), Bs(ci), View(b, GC, nf + (k - 1) * GC), 3, 1, 1,
-                           act=ACT_LRELU, slope=0.2)
-        ci = L.rdb_conv(r, 5)
-        dst = View(bufs[r + 1], nf, 0)
-        if r % 3 == 2:   # last RDB of an RRDB: (x5*0.2 + x)*0.2 + x_rrdb   block.py:286,309
-            ops.conv2d_f32(View(b, CS, 0), pk(ci), Bs(ci), dst, 3, 1, 1, alpha=0.04,
-                           res1=View(b, nf, 0), beta1=0.2, res2=View(bufs[r - 2], nf, 0), beta2=1.0)
-        else:
-            ops.conv2d_f32(View(b, CS, 0), pk(ci), Bs(ci), dst, 3, 1, 1, alpha=0.2, res1=View(b, nf, 0), beta1=1.0)
-    trunk = View(bufs[n_rdb], nf, 0)
-    lr = _empty((N, H, W, nf), x)
-    ops.conv2d_f32(trunk, pk(L.i_lr), Bs(L.i_lr), lr, 3, 1, 1, res1=fea, beta1=1.0)   # fea + LR_conv(...)  block.py:103-105
-    ups = [lr]
-    cur, h, w = lr, H, W
-    for u in range(L.n_up):
-        h, w = 2 * h, 2 * w
-        nxt = _empty((N, h, w, nf), x)
-        ops.conv2d_f32(cur, pk(L.i_up0 + u), Bs(L.i_up0 + u), nxt, 3, 1, 1, ups=2, act=ACT_LRELU)
-        ups.append(nxt)
-        cur = nxt
-    h0 = _empty((N, h, w, nf), x)
-    ops.conv2d_f32(cur, pk(L.i_hr0), Bs(L.i_hr0), h0, 3, 1, 1, act=ACT_LRELU)
-    out_nc = Wt(L.i_hr1).shape[0]
-    o = _empty((N, h, w, out_nc), x)
-    ops.conv2d_f32(h0, pk(L.i_hr1), Bs(L.i_hr1), o, 3, 1, 1)
-    out = _empty((N, out_nc, h, w), x)
-    ops.nhwc_to_nchw(o, out)
+        _rdb_f32(bufs[r], View(bufs[r + 1], nf, 0), r, L, pk, Bs, _rrdb_tail(bufs, r, nf))
+    out, ups, h0 = _trunk_tail_f32(View(bufs[n_rdb], nf, 0), fea, L, params, pk, Bs)
     ctx = None
     if save:
         ctx = dict(L=L, xin=xin, fea=fea, bufs=bufs, ups=ups, h0=h0, shape=(N, in_nc, H, W))
@@ -494,6 +510,100 @@ def _last_layer(h0, out, w, i, cache, wk, bk, hk, dtype):
         ops.conv_tc(h0, wk(i, cout_to=16), bk(i, 16), None, nchw_out=out, cout=16)
 
 
+def _tc_packers(params, cache, hk, bf):
+    """(wk, bk): cached kernel-layout filter / bias of conv i of the flat [w0, b0, w1, b1, ...] list (wgmma path)."""
+    Wt = lambda i: params[2 * i]
+
+    def wk(i, kind=TC_FPROP, cout_to=None, cin_to=None):
+        return cache.get(('w' + hk, i, kind), Wt(i), lambda: ops.pack_filter_tc(_pad_filter(Wt(i), cout_to, cin_to).float(), kind, bf))
+
+    def bk(i, n=None):
+        p = params[2 * i + 1]
+        return cache.get(('b', i, n), p, lambda: _pad_vec(p.float(), n or p.shape[0]).contiguous())
+    return wk, bk
+
+
+def _rdb_bf16(b, dst, r, tail, params, L, cache, sched_id, fused, half, wk, bk):
+    """The five wgmma launches of dense block r on its concat buffer b; conv5 writes dst with the epilogue `tail`
+    (alpha / res1 / res2 / weight map, forwarded to ops.conv_tc).  sched_id: dense-block schedule (None: the fused=True /
+    fused=False forms below)."""
+    nf = L.nf
+    hk = 'h' if half else ''
+    bf = torch.float16 if half else torch.bfloat16
+    CS = nf + 4 * GC
+    BW = CS + (nf if fused else 0)
+    if sched_id is not None:
+        if sched_id == '4' and r % 3 == 2:
+            # the third block of an RRDB carries two residual tiles per epilogue slot: with the K = 192 filter set of
+            # schedule 4's last launch they do not fit shared memory -> schedule 3 for these blocks
+            sched, stag = SCHED3, 's3' + hk
+        else:
+            sched, stag = SCHEDULES[sched_id], 's' + sched_id + hk
+        fw = _sched_rdb_filters(cache, params, L, r, nf, sched, stag, bf)
+        # consecutive launches walk the tile grid in opposite directions: each one starts with the tiles the previous
+        # one wrote last, which are still in L2 (DASR_B200_TILE_REV=0: always forwards)
+        rev = lambda j: TILE_REV and PAIR_MODE and ((5 * r + j) & 1) == 1
+        w1 = sum(nf if k == 5 else GC for k in sched[0][1])            # launch 1: x1 | partial sums of the convs it starts
+        _rdb_stage1(b, fw[0][0], fw[0][1], View(b, w1, nf), nf, tile_rev=rev(1))
+        for j in (2, 3, 4, 5):
+            ks = sched[j - 1][1]
+            width = sum(nf if k == 5 else GC for k in ks)
+            pair = PAIR_MODE                              # every dense-block launch runs on a CTA pair
+            if j < 5:
+                o = View(b, width, nf + (j - 1) * GC)                  # slots of conv j .. conv ks[-1], partial sums in place
+                ops.conv_tc(b, fw[j - 1][0], fw[j - 1][1], o, act=ACT_LRELU, slope=0.2, act_cols=GC, pre=o,
+                            chunks=fw[j - 1][2], pair=pair, tile_rev=rev(j))
+            else:
+                pre5 = View(b, nf, CS) if any(5 in kk for _, kk in sched[:4]) else None     # conv5 started earlier?
+                ops.conv_tc(b, fw[4][0], fw[4][1], dst, pre=pre5, chunks=fw[4][2], pair=pair, tile_rev=rev(5), **tail)
+    elif fused:
+        if half:
+            raise ops._lib.DasrError('half precision needs dense-block schedule 2 or 3 (DASR_B200_SCHED) or fused=False')
+        fw = _fused_rdb_filters(cache, params, L, r, nf)
+        # launch 1: x -> x1 (complete) | partial conv2..5
+        _rdb_stage1(b, fw[0][0], fw[0][1], View(b, BW - nf, nf), nf)
+        for j in (2, 3, 4):   # x_{j-1} -> x_j (complete) | partial conv_{j+1..5}, accumulated in place
+            o = View(b, BW - nf - (j - 1) * GC, nf + (j - 1) * GC)
+            ops.conv_tc(View(b, GC, nf + (j - 2) * GC), fw[j - 1][0], fw[j - 1][1], o, act=ACT_LRELU, slope=0.2,
+                        act_cols=GC, pre=o, pair=PAIR_MODE)
+        ops.conv_tc(View(b, GC, nf + 3 * GC), fw[4][0], fw[4][1], dst, pre=View(b, nf, CS), pair=PAIR_MODE and nf % 64 == 0, **tail)
+    else:
+        for k in range(1, 5):
+            ci = L.rdb_conv(r, k)
+            ops.conv_tc(View(b, _rdb_cin(nf, k), 0), wk(ci), bk(ci), View(b, GC, nf + (k - 1) * GC), act=ACT_LRELU, slope=0.2)
+        ci = L.rdb_conv(r, 5)
+        ops.conv_tc(View(b, CS, 0), wk(ci), bk(ci), dst, nt=_pick_nt(nf, CS), **tail)
+
+
+def _trunk_tail_bf16(bufs, fea, L, params, cache, wk, bk, hk, bf):
+    """fea + LR_conv(trunk) -> nearest-x2 upconvs -> HR_conv0 -> HR_conv1 on the wgmma kernels; the trunk is the x slot of
+    bufs[-1].  `bufs` (the dense-block buffers) is emptied once LR_conv has read them, so their memory returns to the pool
+    before the 4x-resolution layers allocate theirs.  Returns NCHW fp32."""
+    nf = L.nf
+    x = fea
+    N, H, W, _ = fea.shape
+    lr = _empty((N, H, W, nf), x, bf)
+    ops.conv_tc(View(bufs[-1], nf, 0), wk(L.i_lr), bk(L.i_lr), lr, nt=_pick_nt(nf, nf), res1=fea, beta1=1.0,
+                pair=PAIR_MODE and nf % 64 == 0)
+    bufs.clear()
+    cur, h, w = lr, H, W
+    for u in range(L.n_up):
+        h, w = 2 * h, 2 * w
+        nxt = _empty((N, h, w, nf), x, bf)
+        # nearest-x2 + 3x3 conv as four 2x2 sub-pixel convs with pre-summed filters (never materialise the 4x tensor)
+        ops.conv_tc(cur, wk(L.i_up0 + u, TC_UPCONV), bk(L.i_up0 + u), nxt, kind=TC_UPCONV, nt=_pick_nt(nf, nf, 4),
+                    act=ACT_LRELU, slope=0.2)
+        cur = nxt
+    h0 = _empty((N, h, w, nf), x, bf)
+    ops.conv_tc(cur, wk(L.i_hr0), bk(L.i_hr0), h0, nt=_pick_nt(nf, nf), act=ACT_LRELU, slope=0.2, pair=PAIR_MODE and nf % 64 == 0)
+    del cur
+    out_nc = params[2 * L.i_hr1].shape[0]
+    out = _empty((N, out_nc, h, w), x)
+    # last layer: Cout 3 -> one 16-wide wgmma N tile, epilogue writes the 3 real channels straight to NCHW fp32
+    _last_layer(h0, out, params[2 * L.i_hr1], L.i_hr1, cache, wk, bk, hk, bf)
+    return out
+
+
 def rrdb_forward_bf16(x, params, nb, upscale=4, cache=None, fused=True, half=False):
     """wgmma bf16 forward (inference).  NCHW fp32 in -> NCHW fp32 out; bf16 NHWC in between.
 
@@ -520,25 +630,17 @@ def rrdb_forward_bf16(x, params, nb, upscale=4, cache=None, fused=True, half=Fal
     BW = CS + (nf if fused else 0)        # fused: extra slot for conv5's partial sums
     sched_id = os.environ.get('DASR_B200_SCHED', '3')
     sched = SCHEDULES.get(sched_id) if (fused and nf == 64 and GC == 32) else None
-    Wt = lambda i: params[2 * i]
-
-    def wk(i, kind=TC_FPROP, cout_to=None, cin_to=None):
-        return cache.get(('w' + hk, i, kind), Wt(i), lambda: ops.pack_filter_tc(_pad_filter(Wt(i), cout_to, cin_to).float(), kind, bf))
-
-    def bk(i, n=None):
-        p = params[2 * i + 1]
-        return cache.get(('b', i, n), p, lambda: _pad_vec(p.float(), n or p.shape[0]).contiguous())
+    wk, bk = _tc_packers(params, cache, hk, bf)
 
     xin = torch.zeros((N, H, W, 32), dtype=bf, device=x.device)       # Cin 3 -> one zero-padded 32-channel chunk
     ops.nchw_to_nhwc(x.contiguous().float(), View(xin, in_nc, 0))
     n_rdb = L.n_rdb
-    rot = [_empty((N, H, W, BW), x, bf) for _ in range(3)]
-    bufs = [rot[i % 3] for i in range(n_rdb + 1)]
+    bufs = [_empty((N, H, W, BW), x, bf) for _ in range(3)]
+    bufs = [bufs[i % 3] for i in range(n_rdb + 1)]
     fea = _empty((N, H, W, nf), x, bf)
     _mark('tc_begin')
     ops.conv_tc(xin, wk(L.i_fea, cin_to=32), bk(L.i_fea), fea)
     ops.axpby(fea, 1.0, None, 0.0, View(bufs[0], nf, 0))
-    lr = _empty((N, H, W, nf), x, bf)
     # DASR_B200_BATCH_SPLIT=s (experiment): every dense block runs its five launches on one s-th of the batch at a time, so a
     # launch finds a larger share of what its predecessor wrote in L2 — at the price of s times the launches
     nsplit = max(1, min(N, int(os.environ.get('DASR_B200_BATCH_SPLIT', '1'))))
@@ -550,66 +652,156 @@ def rrdb_forward_bf16(x, params, nb, upscale=4, cache=None, fused=True, half=Fal
             tail = dict(alpha=0.04, res1=View(b, nf, 0), beta1=0.2, res2=View(bufs[r - 2][n0:n1], nf, 0), beta2=1.0)
         else:
             tail = dict(alpha=0.2, res1=View(b, nf, 0), beta1=1.0)
-        if sched is not None:
-            if sched_id == '4' and r % 3 == 2:
-                # the third block of an RRDB carries two residual tiles per epilogue slot: with the K = 192 filter set of
-                # schedule 4's last launch they do not fit shared memory -> schedule 3 for these blocks
-                sched, stag = SCHED3, 's3' + hk
-            else:
-                sched, stag = SCHEDULES[sched_id], 's' + sched_id + hk
-            fw = _sched_rdb_filters(cache, params, L, r, nf, sched, stag, bf)
-            # consecutive launches walk the tile grid in opposite directions: each one starts with the tiles the previous
-            # one wrote last, which are still in L2 (DASR_B200_TILE_REV=0: always forwards)
-            rev = lambda j: TILE_REV and PAIR_MODE and ((5 * r + j) & 1) == 1
-            w1 = sum(nf if k == 5 else GC for k in sched[0][1])            # launch 1: x1 | partial sums of the convs it starts
-            _rdb_stage1(b, fw[0][0], fw[0][1], View(b, w1, nf), nf, tile_rev=rev(1))
-            for j in (2, 3, 4, 5):
-                ks = sched[j - 1][1]
-                width = sum(nf if k == 5 else GC for k in ks)
-                pair = PAIR_MODE                              # every dense-block launch runs on a CTA pair
-                if j < 5:
-                    o = View(b, width, nf + (j - 1) * GC)                  # slots of conv j .. conv ks[-1], partial sums in place
-                    ops.conv_tc(b, fw[j - 1][0], fw[j - 1][1], o, act=ACT_LRELU, slope=0.2, act_cols=GC, pre=o,
-                                chunks=fw[j - 1][2], pair=pair, tile_rev=rev(j))
-                else:
-                    pre5 = View(b, nf, CS) if any(5 in kk for _, kk in sched[:4]) else None     # conv5 started earlier?
-                    ops.conv_tc(b, fw[4][0], fw[4][1], dst, pre=pre5, chunks=fw[4][2], pair=pair, tile_rev=rev(5), **tail)
-        elif fused:
-            if half:
-                raise ops._lib.DasrError('half precision needs dense-block schedule 2 or 3 (DASR_B200_SCHED) or fused=False')
-            fw = _fused_rdb_filters(cache, params, L, r, nf)
-            # launch 1: x -> x1 (complete) | partial conv2..5
-            _rdb_stage1(b, fw[0][0], fw[0][1], View(b, BW - nf, nf), nf)
-            for j in (2, 3, 4):   # x_{j-1} -> x_j (complete) | partial conv_{j+1..5}, accumulated in place
-                o = View(b, BW - nf - (j - 1) * GC, nf + (j - 1) * GC)
-                ops.conv_tc(View(b, GC, nf + (j - 2) * GC), fw[j - 1][0], fw[j - 1][1], o, act=ACT_LRELU, slope=0.2,
-                            act_cols=GC, pre=o, pair=PAIR_MODE)
-            ops.conv_tc(View(b, GC, nf + 3 * GC), fw[4][0], fw[4][1], dst, pre=View(b, nf, CS), pair=PAIR_MODE and nf % 64 == 0, **tail)
-        else:
-            for k in range(1, 5):
-                ci = L.rdb_conv(r, k)
-                ops.conv_tc(View(b, _rdb_cin(nf, k), 0), wk(ci), bk(ci), View(b, GC, nf + (k - 1) * GC), act=ACT_LRELU, slope=0.2)
-            ci = L.rdb_conv(r, 5)
-            ops.conv_tc(View(b, CS, 0), wk(ci), bk(ci), dst, nt=_pick_nt(nf, CS), **tail)
-    ops.conv_tc(View(bufs[n_rdb], nf, 0), wk(L.i_lr), bk(L.i_lr), lr, nt=_pick_nt(nf, nf), res1=fea, beta1=1.0,
-                pair=PAIR_MODE and nf % 64 == 0)
-    del rot, bufs
-    cur, h, w = lr, H, W
-    for u in range(L.n_up):
-        h, w = 2 * h, 2 * w
-        nxt = _empty((N, h, w, nf), x, bf)
-        # nearest-x2 + 3x3 conv as four 2x2 sub-pixel convs with pre-summed filters (never materialise the 4x tensor)
-        ops.conv_tc(cur, wk(L.i_up0 + u, TC_UPCONV), bk(L.i_up0 + u), nxt, kind=TC_UPCONV, nt=_pick_nt(nf, nf, 4),
-                    act=ACT_LRELU, slope=0.2)
-        cur = nxt
-    h0 = _empty((N, h, w, nf), x, bf)
-    ops.conv_tc(cur, wk(L.i_hr0), bk(L.i_hr0), h0, nt=_pick_nt(nf, nf), act=ACT_LRELU, slope=0.2, pair=PAIR_MODE and nf % 64 == 0)
-    del cur
-    out_nc = Wt(L.i_hr1).shape[0]
-    out = _empty((N, out_nc, h, w), x)
-    # last layer: Cout 3 -> one 16-wide wgmma N tile, epilogue writes the 3 real channels straight to NCHW fp32
-    _last_layer(h0, out, Wt(L.i_hr1), L.i_hr1, cache, wk, bk, hk, bf)
+        _rdb_bf16(b, dst, r, tail, params, L, cache, sched_id if sched is not None else None, fused, half, wk, bk)
+    out = _trunk_tail_bf16(bufs, fea, L, params, cache, wk, bk, hk, bf)
     _mark('tc_end')
+    return out
+    _mark('tc_end')
+    return out
+
+
+# ==================================================================================================
+# Adaptive-weight RRDB generators (inference): RRDBNet_Residual_conv_concat / RRDBNet_Residual_conv
+# (architecture.py:208-297, block.py:462-528)
+# ==================================================================================================
+# Flat parameter list: the RRDBNet layout of nb_ada + nb RRDBs (fea, the dense blocks of the adaptive blocks then of the
+# plain ones, LR_conv, upconvs, HR convs) followed by the extra convs of every adaptive block:
+#   concat: adaptive_conv.0 (65 -> 64), adaptive_conv.2, res_conv.0 (65 -> 64), res_conv.2        plain: res_conv.0, res_conv.2
+# The map is the sigmoid output of the patch discriminator, [N, 1, H, W] at the input resolution.
+
+def _ada_ext(L, concat):
+    n_ext = 4 if concat else 2
+    return lambda blk, i: L.n_conv + n_ext * blk + i
+
+
+def _check_map(x, amap, nb, nb_ada):
+    _need_cuda(x, 'adaptive RRDB generator')
+    N, _, H, W = x.shape
+    if tuple(amap.shape) != (N, 1, H, W):
+        raise ops._lib.DasrError('adaptive RRDB generator: the weight map must be [N, 1, H, W] = %s (got %s)'
+                                 % ((N, 1, H, W), tuple(amap.shape)))
+    if nb_ada < 1 or nb < 1:
+        raise ops._lib.DasrError('adaptive RRDB generator: needs nb >= 1 and nb_ada >= 1')
+    return amap.detach().float().contiguous()
+
+
+def adaptive_rrdb_forward_bf16(x, amap, params, nb, nb_ada, concat, upscale=4, cache=None, half=False):
+    """wgmma forward of the adaptive generators.  concat: an adaptive block is
+    t_k = RDB_k(A(t_{k-1} (+) 0.2a)), out = 0.2 t_3 + R(u (+) a); the 65-channel convs of A and R take the map as an extra
+    input channel in their epilogue (MAP_CHANNEL), A's second conv writes straight into the x slot of the dense block's
+    concat buffer, R is computed once at block entry.  plain: out = RRDB3chain(u) * a + 0.1 R(u); RDB3's conv5 applies the
+    map in its epilogue (MAP_SCALE)."""
+    a = _check_map(x, amap, nb, nb_ada)
+    L = RRDBLayout(nb + nb_ada, params[0].shape[0], upscale)
+    nf = L.nf
+    if nf != 64:
+        raise ops._lib.DasrError('adaptive RRDB generator: the wgmma path needs nf = 64 (got %d)' % nf)
+    cache = cache if cache is not None else _PackCache()
+    N, in_nc, H, W = x.shape
+    bf = torch.float16 if half else torch.bfloat16
+    hk = 'h' if half else ''
+    BW = nf + 4 * GC + nf
+    sched_id = os.environ.get('DASR_B200_SCHED', '3')
+    if sched_id not in SCHEDULES:
+        raise ops._lib.DasrError('adaptive RRDB generator: DASR_B200_SCHED must be one of %s' % sorted(SCHEDULES))
+    wk, bk = _tc_packers(params, cache, hk, bf)
+    ext = _ada_ext(L, concat)
+
+    def conv64(src, i, dst):        # 64 -> 64 conv + LeakyReLU of A / R: launched like LR_conv and HR_conv0
+        ops.conv_tc(src, wk(i), bk(i), dst, nt=_pick_nt(nf, nf), act=ACT_LRELU, slope=0.2, pair=PAIR_MODE)
+
+    def conv_map(src, i, dst, s):   # 65 -> 64 conv + LeakyReLU: 64 channels on the MMAs, s * map in the epilogue
+        w = params[2 * i]
+        wm = cache.get(('wm' + hk, i), w, lambda: ops.pack_filter_tc(w.detach()[:, :nf].float().contiguous(), TC_FPROP, bf))
+        taps = cache.get(('wmt', i), w, lambda: ops.map_channel_taps(w, nf))
+        ops.conv_tc(src, wm, bk(i), dst, act=ACT_LRELU, slope=0.2, amap=a, map_mode=ops.MAP_CHANNEL, map_scale=s, map_w=taps)
+
+    xin = torch.zeros((N, H, W, 32), dtype=bf, device=x.device)
+    ops.nchw_to_nhwc(x.contiguous().float(), View(xin, in_nc, 0))
+    n_rdb = L.n_rdb
+    bufs = [_empty((N, H, W, BW), x, bf) for _ in range(3)]
+    bufs = [bufs[i % 3] for i in range(n_rdb + 1)]
+    fea = _empty((N, H, W, nf), x, bf)
+    tmp = _empty((N, H, W, nf), x, bf)       # first conv of A / R
+    res = _empty((N, H, W, nf), x, bf)       # R of the current adaptive block
+    ops.conv_tc(xin, wk(L.i_fea, cin_to=32), bk(L.i_fea), fea)
+    ops.axpby(fea, 1.0, None, 0.0, View(bufs[0], nf, 0))
+    for r in range(n_rdb):
+        b, blk = bufs[r], r // 3
+        u = View(b, nf, 0)
+        tail = _rrdb_tail(bufs, r, nf)
+        if blk < nb_ada:
+            if concat:
+                if r % 3 == 0:
+                    conv_map(u, ext(blk, 2), tmp, 1.0)
+                    conv64(tmp, ext(blk, 3), res)
+                conv_map(u, ext(blk, 0), tmp, 0.2)
+                conv64(tmp, ext(blk, 1), u)
+                if r % 3 == 2:
+                    tail = dict(alpha=0.04, res1=u, beta1=0.2, res2=res, beta2=1.0)
+            else:
+                if r % 3 == 0:
+                    conv64(u, ext(blk, 0), tmp)
+                    conv64(tmp, ext(blk, 1), res)
+                if r % 3 == 2:
+                    tail = dict(alpha=0.2, res1=u, beta1=1.0, res2=res, beta2=0.1, amap=a, map_mode=ops.MAP_SCALE)
+        _rdb_bf16(b, View(bufs[r + 1], nf, 0), r, tail, params, L, cache, sched_id, True, half, wk, bk)
+    del tmp, res
+    return _trunk_tail_bf16(bufs, fea, L, params, cache, wk, bk, hk, bf)
+
+
+def adaptive_rrdb_forward_f32(x, amap, params, nb, nb_ada, concat, upscale=4):
+    """fp32 twin of adaptive_rrdb_forward_bf16 (the parity path): the 65-channel convs run on a materialised
+    [u | s * map] concat, the plain variant's map product is one elementwise kernel."""
+    a = _check_map(x, amap, nb, nb_ada)
+    L = RRDBLayout(nb + nb_ada, params[0].shape[0], upscale)
+    nf = L.nf
+    N, in_nc, H, W = x.shape
+    Bs = lambda i: params[2 * i + 1]
+    pk = lambda i: ops.pack_filter_f32(params[2 * i])
+    ext = _ada_ext(L, concat)
+
+    def conv64(src, i, dst):
+        ops.conv2d_f32(src, pk(i), Bs(i), dst, 3, 1, 1, act=ACT_LRELU, slope=0.2)
+
+    cat = _empty((N, H, W, nf + 1), x) if concat else None
+
+    def conv_cat(src, s, i, dst):   # conv(cat(src, s * map)) + LeakyReLU  (block.py:524-527)
+        ops.axpby(src, 1.0, None, 0.0, View(cat, nf, 0))
+        ops.map_axpby(None, a, s, None, 0.0, View(cat, 1, nf))
+        conv64(cat, i, dst)
+
+    xin = _empty((N, H, W, in_nc), x)
+    ops.nchw_to_nhwc(x.contiguous().float(), xin)
+    fea = _empty((N, H, W, nf), x)
+    ops.conv2d_f32(xin, pk(L.i_fea), Bs(L.i_fea), fea, 3, 1, 1)
+    n_rdb = L.n_rdb
+    rot = [_empty((N, H, W, nf + 4 * GC), x) for _ in range(3)]
+    bufs = [rot[i % 3] for i in range(n_rdb + 1)]
+    tmp, res = _empty((N, H, W, nf), x), _empty((N, H, W, nf), x)
+    ops.axpby(fea, 1.0, None, 0.0, View(bufs[0], nf, 0))
+    for r in range(n_rdb):
+        b, blk = bufs[r], r // 3
+        u, dst = View(b, nf, 0), View(bufs[r + 1], nf, 0)
+        tail = _rrdb_tail(bufs, r, nf)
+        if blk < nb_ada and concat:
+            if r % 3 == 0:
+                conv_cat(u, 1.0, ext(blk, 2), tmp)
+                conv64(tmp, ext(blk, 3), res)
+            conv_cat(u, 0.2, ext(blk, 0), tmp)
+            conv64(tmp, ext(blk, 1), u)
+            if r % 3 == 2:
+                tail = dict(alpha=0.04, res1=u, beta1=0.2, res2=res, beta2=1.0)
+        elif blk < nb_ada:
+            if r % 3 == 0:
+                conv64(u, ext(blk, 0), tmp)
+                conv64(tmp, ext(blk, 1), res)
+            if r % 3 == 2:      # RRDB3chain(u) * a + 0.1 * R(u)
+                _rdb_f32(b, tmp, r, L, pk, Bs, dict(alpha=0.2, res1=u, beta1=1.0))
+                ops.map_axpby(tmp, a, 1.0, res, 0.1, dst)
+                continue
+        _rdb_f32(b, dst, r, L, pk, Bs, tail)
+    out, _, _ = _trunk_tail_f32(View(bufs[n_rdb], nf, 0), fea, L, params, pk, Bs)
     return out
 
 

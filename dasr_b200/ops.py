@@ -260,12 +260,16 @@ def pack_filter_tc(w, kind, dtype=torch.bfloat16):
 
 def conv_tc(inp, w_packed, bias, out, kind=TC_FPROP, nt=None, act=ACT_NONE, slope=0.2, alpha=1.0, act_cols=None,
             pre=None, res1=None, beta1=0.0, res2=None, beta2=0.0, mask=None, mask_c0=0, mask_c1=0, mask_slope=0.2,
-            a_mode=0, nchw_out=None, cout=None, tile_rev=False, chunks=None, pair=None, tapn=False):
+            a_mode=0, nchw_out=None, cout=None, tile_rev=False, chunks=None, pair=None, tapn=False, amap=None, map_mode=0,
+            map_scale=1.0, map_w=None):
     """wgmma 3x3 conv on NHWC bf16 channel slices; chunks = optional list of 32-channel chunk offsets of `inp`'s buffer; `inp`/`out`/`pre`/`res*`/`mask` are Views (or tensors).
     v = alpha*act(acc + bias + pre) + beta1*res1 + beta2*res2, activation on the first `act_cols` channels only.
     nchw_out: fp32 NCHW tensor — the launch writes its first nchw_out.shape[1] channels there (last layer).
     pair: True = run on the CTA-pair kernel (dasr_conv_tc2: 2-CTA cluster, filters split over two SMs, activation tiles multicast;
-          plain 3x3 geometry, cout % 64 == 0, no mask; `nt` is ignored)."""
+          plain 3x3 geometry, cout % 64 == 0, no mask; `nt` is ignored).
+    amap: fp32 weight map [N, 1, H, W] (or [N, H, W]) at the output resolution, used as map_mode says (dasr_conv_tc_map):
+          MAP_CHANNEL = one more input channel map_scale * amap whose 3x3 taps are map_w ([9][cout] fp32, map_channel_taps);
+          MAP_SCALE   = v = amap * (alpha*act(acc + bias + pre) + beta1*res1) + beta2*res2."""
     inp = as_view(inp)
     N, H, W, _ = inp.t.shape
     if nchw_out is not None:
@@ -307,6 +311,10 @@ def conv_tc(inp, w_packed, bias, out, kind=TC_FPROP, nt=None, act=ACT_NONE, slop
         p.mask_cs, p.mask_coff, p.mask_c0, p.mask_c1, p.mask_slope = mask.cs, mask.coff, mask_c0, mask_c1, mask_slope
     p.a_mode = a_mode
     p.tile_rev = int(bool(tile_rev))
+    if amap is not None:
+        if amap.dtype != torch.float32 or amap.shape[0] != N or amap.shape[-2:] != (H, W) or amap.numel() != N * H * W:
+            raise _lib.DasrError('conv_tc: the weight map must be fp32 [N, 1, H, W] at the output resolution')
+        p.map_mode, p.map_scale, p.map_stride = map_mode, map_scale, H * W
     if pair is None:
         pair = False
     if pair:
@@ -319,11 +327,30 @@ def conv_tc(inp, w_packed, bias, out, kind=TC_FPROP, nt=None, act=ACT_NONE, slop
             p.res1_cs, p.res1_coff, p.beta1 = mask.cs, mask.coff, 0.0
         p.nt = nt if nt else p.cout              # Cout tile per CTA pair (grid.y = cout / nt); default: one tile
         p.epi_mode = 0
+        if amap is not None:
+            check(lib.dasr_conv_tc2_map(inp.ptr, _p(w_packed), _p(bias), pre.ptr if pre else None, res1.ptr if res1 else None,
+                                        res2.ptr if res2 else None, _p(amap), _p(map_w), out.ptr, C.byref(p), _stream()),
+                  'conv_tc2_map')
+            return
         check(lib.dasr_conv_tc2(inp.ptr, _p(w_packed), _p(bias), pre.ptr if pre else None, res1.ptr if res1 else None,
                                 res2.ptr if res2 else None, out.ptr, C.byref(p), _stream()), 'conv_tc2')
         return
+    if amap is not None:
+        if mask is not None:
+            raise _lib.DasrError('conv_tc: no dgrad mask together with the weight map')
+        check(lib.dasr_conv_tc_map(inp.ptr, _p(w_packed), _p(bias), pre.ptr if pre else None, res1.ptr if res1 else None,
+                                   res2.ptr if res2 else None, _p(amap), _p(map_w), out.ptr, C.byref(p), _stream()), 'conv_tc_map')
+        return
     check(lib.dasr_conv_tc(inp.ptr, _p(w_packed), _p(bias), pre.ptr if pre else None, res1.ptr if res1 else None,
                            res2.ptr if res2 else None, mask.ptr if mask else None, out.ptr, C.byref(p), _stream()), 'conv_tc')
+
+
+MAP_CHANNEL, MAP_SCALE = 1, 2      # DASR_MAP_CHANNEL / DASR_MAP_SCALE
+
+
+def map_channel_taps(w, c):
+    """Input channel c of an OIHW fp32 3x3 filter as the [9][cout] fp32 taps of the MAP_CHANNEL epilogue."""
+    return w.detach()[:, c].reshape(w.shape[0], 9).t().float().contiguous()
 
 
 def pick_nt_pair(cin, cout):
@@ -415,6 +442,19 @@ def axpby(x, a, y, b, dst):
     check(_lib.load().dasr_axpby(x.ptr, y.ptr if y else None, dst.ptr, npix, dst.c, x.cs, x.coff,
                                  y.cs if y else 0, y.coff if y else 0, dst.cs, dst.coff, a, b,
                                  _dt16(dst.t), _stream()), 'axpby')
+
+
+def map_axpby(x, amap, a, y, b, dst):
+    """dst = amap * (a * x) + b * y on fp32 NHWC channel slices (x None: dst = a * amap); amap: fp32, one value per pixel."""
+    dst = as_view(dst)
+    x = as_view(x) if x is not None else None
+    y = as_view(y) if y is not None else None
+    npix = dst.t.numel() // dst.cs
+    if amap.numel() != npix or amap.dtype != torch.float32:
+        raise _lib.DasrError('map_axpby: the map must hold one fp32 value per pixel')
+    check(_lib.load().dasr_map_axpby(x.ptr if x else None, _p(amap), y.ptr if y else None, dst.ptr, npix, dst.c,
+                                     x.cs if x else 0, x.coff if x else 0, y.cs if y else 0, y.coff if y else 0,
+                                     dst.cs, dst.coff, a, b, _stream()), 'map_axpby')
 
 
 def maxpool2_fwd(x, out):

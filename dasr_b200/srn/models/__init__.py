@@ -16,6 +16,8 @@ def create_model(opt):
         from .SRRaGAN_model import SRRaGANModel as M
     elif model in ('DASR', 'DASR_FS_ESRGAN_patchGAN'):
         from .DASR_model import DASR_Model as M
+    elif model == 'DASR_Adaptive_Model':
+        from .DASR_Adaptive_model import DASR_Adaptive_Model as M
     else:
         raise NotImplementedError('Model [{:s}] not recognized.'.format(str(model)))
     m = M(opt)

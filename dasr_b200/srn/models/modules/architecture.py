@@ -2,6 +2,7 @@
 state_dict keys (codes/SRN/models/modules/architecture.py), running on dasr_b200 kernels.
 
   RRDBNet               architecture.py:174-205   -> engine.RRDBNetFunction (fp32 train) / rrdb_forward_bf16 (wgmma)
+  RRDBNet_Residual_conv(_concat)  architecture.py:208-297 -> engine.adaptive_rrdb_forward_bf16 / _f32 (inference only)
   NLayerDiscriminator   architecture.py:983-1024  -> engine.NLayerDFunction
   VGGFeatureExtractor   architecture.py:1060-1088 -> engine.VGGFunction
   GaussianFilter / FilterLow / FilterHigh  :1177-1243 -> dwfilter kernel
@@ -131,6 +132,109 @@ class RRDBNet(nn.Module):
             return g(x)
         out, _ = engine.rrdb_forward_f32(x, [p.detach() for p in params], self.nb, self.upscale, save=False)
         return out
+
+
+class _GraphedForwardMap(_GraphedForward):
+    """_GraphedForward of a generator with a second input, the weight map: both live in static buffers."""
+
+    def __init__(self, fn, x, amap):
+        self.amap = amap.detach().clone()
+        super().__init__(lambda t: fn(t, self.amap), x)
+
+    def __call__(self, x, amap):
+        self.amap.copy_(amap)
+        return super().__call__(x)
+
+
+class _AdaptiveRRDBNet(nn.Module):
+    """RRDBNet_Residual_conv / RRDBNet_Residual_conv_concat (architecture.py:208-297): fea_conv -> nb_ada adaptive blocks
+    (weighted by the per-pixel map of the patch discriminator) -> nb RRDBs -> LR_conv + fea -> upconvs -> HR convs.
+    Same constructor, state_dict keys and forward(x, adaptive_weights) as the reference; inference only."""
+    concat = None
+
+    def __init__(self, in_nc, out_nc, nf, nb, gc=32, upscale=4, norm_type=None, act_type='leakyrelu', mode='CNA',
+                 upsample_mode='upconv', nb_ada=1):
+        super().__init__()
+        if norm_type is not None:
+            raise NotImplementedError('%s with norm layers is not on the H100 path' % type(self).__name__)
+        if upsample_mode != 'upconv':
+            raise NotImplementedError('upsample mode [{:s}] is not found'.format(upsample_mode))
+        if act_type != 'leakyrelu':
+            raise NotImplementedError('%s act_type must be leakyrelu (define_G passes it unconditionally)' % type(self).__name__)
+        if upscale == 3:
+            raise NotImplementedError('%s upscale=3 (nearest x3 upconv) is not supported by the H100 path' % type(self).__name__)
+        n_upscale = int(math.log(upscale, 2))
+        fea_conv = B.conv_block(in_nc, nf, kernel_size=3, norm_type=None, act_type=None)
+        rb_blocks = [B.RRDB(nf, kernel_size=3, gc=32, stride=1, bias=True, pad_type='zero', norm_type=norm_type,
+                            act_type=act_type, mode='CNA') for _ in range(nb)]
+        ada = B.RRDB_Residual_conv_concat if self.concat else B.RRDB_Residual_conv
+        rb_blocks_adaptive = [ada(nf, kernel_size=3, gc=32, stride=1, bias=True, pad_type='zero', norm_type=norm_type,
+                                  act_type=act_type, mode='CNA') for _ in range(nb_ada)]
+        LR_conv = B.conv_block(nf, nf, kernel_size=3, norm_type=norm_type, act_type=None, mode=mode)
+        upsampler = [B.upconv_blcok(nf, nf, act_type=act_type) for _ in range(n_upscale)]
+        HR_conv0 = B.conv_block(nf, nf, kernel_size=3, norm_type=None, act_type=act_type)
+        HR_conv1 = B.conv_block(nf, out_nc, kernel_size=3, norm_type=None, act_type=None)
+        self.fea_conv = fea_conv
+        self.rb_blocks = B.sequential(*rb_blocks)
+        self.rb_blocks_ada = B.sequential(*rb_blocks_adaptive)
+        self.LR_conv = LR_conv
+        self.up_conv = B.sequential(*upsampler, HR_conv0, HR_conv1)
+        self.nb, self.nb_ada, self.nf, self.upscale = nb, nb_ada, nf, upscale
+        self.precision = None          # None -> DASR_B200_PRECISION or 'bf16' ('bf16' | 'fp16' | 'fp32')
+        self._pack_cache = engine._PackCache()
+        self._graphs = {}
+        self._graph_seen = None
+
+    def _engine_params(self):
+        """Parameters in the flat order of engine.adaptive_rrdb_forward_*: the RRDBNet layout of all nb_ada + nb RRDBs, then the
+        extra convs of every adaptive block."""
+        ada = [self.rb_blocks_ada] if self.nb_ada == 1 else list(self.rb_blocks_ada)
+        trunk = [self.rb_blocks] if self.nb == 1 else list(self.rb_blocks)
+        convs = [self.fea_conv[0]]
+        for blk in ada + trunk:
+            for rdb in (blk.RDB1, blk.RDB2, blk.RDB3):
+                convs += [getattr(rdb, 'conv%d' % k)[0] for k in range(1, 6)]
+        convs.append(self.LR_conv[0])
+        convs += [m for m in self.up_conv if isinstance(m, nn.Conv2d)]
+        for blk in ada:
+            if self.concat:
+                convs += [blk.adaptive_conv[0], blk.adaptive_conv[2]]
+            convs += [blk.res_conv[0], blk.res_conv[2]]
+        return [t for c in convs for t in (c.weight, c.bias)]
+
+    def forward(self, x, adaptive_weights):
+        params = self._engine_params()
+        if torch.is_grad_enabled() and (x.requires_grad or adaptive_weights.requires_grad or any(p.requires_grad for p in params)):
+            raise NotImplementedError('training of the adaptive generators is not built (run the forward under torch.no_grad())')
+        prec = self.precision or _precision('bf16')
+        if prec == 'fp32':
+            return engine.adaptive_rrdb_forward_f32(x, adaptive_weights, params, self.nb, self.nb_ada, self.concat, self.upscale)
+        if prec not in ('bf16', 'fp16'):
+            raise NotImplementedError('%s: precision [%s] is not supported (bf16 | fp16 | fp32)' % (type(self).__name__, prec))
+        fn = lambda t, a: engine.adaptive_rrdb_forward_bf16(t, a, params, self.nb, self.nb_ada, self.concat, self.upscale,
+                                                            self._pack_cache, half=prec == 'fp16')
+        if os.environ.get('DASR_B200_GRAPH', '1') == '0' or not x.is_cuda or engine.PROFILE is not None:
+            return fn(x, adaptive_weights)
+        key = (tuple(x.shape), tuple(adaptive_weights.shape), x.device.index, prec, tuple(p._version for p in params),
+               params[0].data_ptr(), params[len(params) // 2].data_ptr(), params[-1].data_ptr())
+        g = self._graphs.get(key)
+        if g is None:
+            # capture on the second sighting of a (shape, parameter version), like RRDBNet
+            if self._graph_seen != key:
+                self._graph_seen = key
+                return fn(x, adaptive_weights)
+            if len(self._graphs) >= 2:
+                self._graphs.clear()
+            g = self._graphs[key] = _GraphedForwardMap(fn, x.contiguous().float(), adaptive_weights.contiguous().float())
+        return g(x, adaptive_weights)
+
+
+class RRDBNet_Residual_conv(_AdaptiveRRDBNet):
+    concat = False
+
+
+class RRDBNet_Residual_conv_concat(_AdaptiveRRDBNet):
+    concat = True
 
 
 class NLayerDiscriminator(nn.Module):

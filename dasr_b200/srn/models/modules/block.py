@@ -184,6 +184,51 @@ class RRDB(nn.Module):
         return self.RDB3(self.RDB2(self.RDB1(x))).mul(0.2) + x
 
 
+class RRDB_Residual_conv(nn.Module):
+    """Adaptive block of RRDBNet_Residual_conv (block.py:462-488): RRDB3chain(u) * a + 0.1 * res_conv(u), no identity skip.
+    x = [u, a]; returns [out, a].  A parameter container: the generator runs it through dasr_b200.engine."""
+
+    def __init__(self, nc, kernel_size=3, gc=32, stride=1, bias=True, pad_type='zero',
+                 norm_type=None, act_type='leakyrelu', mode='CNA', n_resconv=2, resconv_scale=[0.1, 1]):
+        super().__init__()
+        args = (nc, kernel_size, gc, stride, bias, pad_type, norm_type, act_type, mode)
+        self.RDB1 = ResidualDenseBlock_5C(*args)
+        self.RDB2 = ResidualDenseBlock_5C(*args)
+        self.RDB3 = ResidualDenseBlock_5C(*args)
+        self.resconv_scale = resconv_scale
+        self.res_conv = sequential(*[conv_block(nc, nc, kernel_size=3, stride=1, bias=True, pad_type='zero',
+                                                norm_type=norm_type, act_type=act_type, mode='CNA') for _ in range(n_resconv)])
+
+    def forward(self, x):
+        out = self.RDB3(self.RDB2(self.RDB1(x[0])))
+        return out.mul(x[1] * self.resconv_scale[1]) + self.res_conv(x[0]) * self.resconv_scale[0], x[1]
+
+
+class RRDB_Residual_conv_concat(nn.Module):
+    """Adaptive block of RRDBNet_Residual_conv_concat (block.py:490-528): t_k = RDB_k(A(t_{k-1} (+) 0.2a)) with one shared A,
+    out = 0.2 t_3 + res_conv(u (+) a); A and res_conv start with a 65 -> 64 conv.  x = [u, a]; returns [out, a]."""
+
+    def __init__(self, nc, kernel_size=3, gc=32, stride=1, bias=True, pad_type='zero',
+                 norm_type=None, act_type='leakyrelu', mode='CNA', n_resconv=2, n_ada_conv=2, adaptive_scale=[0.2, 1]):
+        super().__init__()
+        args = (nc, kernel_size, gc, stride, bias, pad_type, norm_type, act_type, mode)
+        self.RDB1 = ResidualDenseBlock_5C(*args)
+        self.RDB2 = ResidualDenseBlock_5C(*args)
+        self.RDB3 = ResidualDenseBlock_5C(*args)
+        self.adaptive_scale = adaptive_scale
+        cb = lambda cin: conv_block(cin, nc, kernel_size=3, stride=1, bias=True, pad_type='zero', norm_type=norm_type,
+                                    act_type=act_type, mode='CNA')
+        self.adaptive_conv = sequential(*([cb(nc + 1)] + [cb(nc) for _ in range(n_ada_conv - 1)]))
+        self.res_conv = sequential(*([cb(nc + 1)] + [cb(nc) for _ in range(n_resconv - 1)]))
+
+    def forward(self, x):
+        u, a = x[0], x[1]
+        out = u
+        for rdb in (self.RDB1, self.RDB2, self.RDB3):
+            out = rdb(self.adaptive_conv(torch.cat((out, a * self.adaptive_scale[0]), dim=1)))
+        return out.mul(0.2) + self.res_conv(torch.cat((u, a * self.adaptive_scale[1]), dim=1)), a
+
+
 def upconv_blcok(in_nc, out_nc, upscale_factor=2, kernel_size=3, stride=1, bias=True,
                  pad_type='zero', norm_type=None, act_type='relu', mode='nearest'):
     """nearest upsample + conv (+act).  (The reference spells it 'blcok'; the name is API.)"""

@@ -81,6 +81,13 @@ def define_G(opt):
         netG = arch.RRDBNet(in_nc=opt_net['in_nc'], out_nc=opt_net['out_nc'], nf=opt_net['nf'], nb=opt_net['nb'],
                             gc=opt_net['gc'], upscale=opt_net['scale'], norm_type=opt_net['norm_type'],
                             act_type='leakyrelu', mode=opt_net['mode'], upsample_mode='upconv')
+    elif which in ('RRDB_Residual_conv', 'RRDB_Residual_conv_concat'):
+        # networks.py:131-138: only the concat variant receives ada_nb; RRDB_Residual_conv always has ONE adaptive block
+        cls = arch.RRDBNet_Residual_conv_concat if which == 'RRDB_Residual_conv_concat' else arch.RRDBNet_Residual_conv
+        kw = {'nb_ada': opt_net['ada_nb']} if which == 'RRDB_Residual_conv_concat' else {}
+        netG = cls(in_nc=opt_net['in_nc'], out_nc=opt_net['out_nc'], nf=opt_net['nf'], nb=opt_net['nb'], gc=opt_net['gc'],
+                   upscale=opt_net['scale'], norm_type=opt_net['norm_type'], act_type='leakyrelu', mode=opt_net['mode'],
+                   upsample_mode='upconv', **kw)
     elif which == 'sr_resnet':      # networks.py:88-91
         netG = arch.SRResNet(in_nc=opt_net['in_nc'], out_nc=opt_net['out_nc'], nf=opt_net['nf'], nb=opt_net['nb'],
                              upscale=opt_net['scale'], norm_type=opt_net['norm_type'], act_type='relu', mode=opt_net['mode'],

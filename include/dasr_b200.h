@@ -168,7 +168,21 @@ typedef struct {
   int f16;                     /* 0: operands / activations / partial sums are bf16;  1: IEEE half (kind::f16 F16 operands, fp32
                                   accumulate; same rate, 3 more mantissa bits — the inference precision 'fp16').  Filters must be
                                   packed with DASR_TC_PACK_F16. */
+  /* Per-pixel weight map (dasr_conv_tc_map / dasr_conv_tc2_map only; dasr_conv_tc / dasr_conv_tc2 ignore these fields).
+   * The map is fp32 [N][H][W] at the output resolution (image stride map_stride >= H*W floats).  Plain 3x3 geometry
+   * (dasr_conv_tc_setup kind 0), staged epilogue (epi_mode 0), no dgrad mask.
+   *   DASR_MAP_CHANNEL: the map is one more input channel, scaled by map_scale:
+   *                     v = alpha*act(acc + bias + map_scale * sum_{3x3 taps} map_w[tap][co] * map[y+dy-1][x+dx-1]) ...
+   *                     (zero outside the image); map_w = the 9 x cout fp32 taps of that channel; no pre / residuals.
+   *   DASR_MAP_SCALE:   v = map[y][x] * (alpha*act(acc + bias + pre) + beta1*res1) + beta2*res2   (res1 and res2 required)
+   * Replaces the torch.cat((x, ada_weights * s), 1) conv of RRDB_Residual_conv_concat and the out.mul(ada_weights) of
+   * RRDB_Residual_conv (block.py:462-528). */
+  int map_mode;                /* 0 = off, DASR_MAP_CHANNEL, DASR_MAP_SCALE */
+  float map_scale;
+  int map_stride;
 } DasrConvTcParams;
+#define DASR_MAP_CHANNEL 1
+#define DASR_MAP_SCALE 2
 
 int dasr_conv_tc(const void* in_bf16, const void* w_packed_bf16, const float* bias, const void* pre_bf16,
                  const void* res1_bf16, const void* res2_bf16, const void* mask_src_bf16,
@@ -185,6 +199,14 @@ int dasr_conv_tc(const void* in_bf16, const void* w_packed_bf16, const float* bi
 int dasr_conv_tc2_supported(const DasrConvTcParams* p);
 int dasr_conv_tc2(const void* in_bf16, const void* w_packed_bf16, const float* bias, const void* pre_bf16,
                   const void* res1_bf16, const void* res2_bf16, void* out_bf16, const DasrConvTcParams* p, void* stream);
+
+/* The same two convolutions with the weight-map operand of p->map_mode (see DasrConvTcParams). */
+int dasr_conv_tc_map(const void* in_bf16, const void* w_packed_bf16, const float* bias, const void* pre_bf16,
+                     const void* res1_bf16, const void* res2_bf16, const float* map, const float* map_w, void* out_bf16,
+                     const DasrConvTcParams* p, void* stream);
+int dasr_conv_tc2_map(const void* in_bf16, const void* w_packed_bf16, const float* bias, const void* pre_bf16,
+                      const void* res1_bf16, const void* res2_bf16, const float* map, const float* map_w, void* out_bf16,
+                      const DasrConvTcParams* p, void* stream);
 
 /* OIHW fp32 3x3 filter -> tc packing.  kind: 0 = plain 3x3 fprop (1 variant, 9 taps)
  *                                            1 = dgrad of a 3x3 s1 p1 conv (flipped, in/out swapped)
@@ -239,6 +261,11 @@ int dasr_upsample2x_bwd(const void* src, void* dst, int N, int H, int W, int C, 
  * upconv layers in mixed-precision training; the forward never materialises it) */
 int dasr_upsample2x_fwd(const void* src, void* dst, int N, int H, int W, int C, int src_cs, int src_coff, int dst_cs,
                         int dst_coff, int is_bf16, void* stream);
+/* dst[p][c] = map[p] * (a * x[p][c]) + b * y[p][c] on fp32 NHWC channel slices; map: fp32 [npix] (the pixel order of the
+ * NHWC tensors).  x NULL: x = 1 (dst = a * map, e.g. the scaled map channel of a concat buffer); y NULL: b is ignored.
+ * The fp32 form of the weight-map operations of RRDB_Residual_conv(_concat) (block.py:462-528). */
+int dasr_map_axpby(const float* x, const float* map, const float* y, float* dst, long npix, int C, int x_cs, int x_coff,
+                   int y_cs, int y_coff, int d_cs, int d_coff, float a, float b, void* stream);
 /* dst = a*x + b*y on channel slices (gradient accumulation across concat consumers) */
 int dasr_axpby(const void* x, const void* y, void* dst, long npix, int C, int x_cs, int x_coff,
                int y_cs, int y_coff, int d_cs, int d_coff, float a, float b, int is_bf16, void* stream);
