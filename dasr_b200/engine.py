@@ -269,12 +269,15 @@ class _PackCache:
     def __init__(self):
         self.d = {}
 
-    def get(self, key, param, make):
-        """`param`: the tensor — or the list of ALL tensors — the cached value is derived from."""
+    @staticmethod
+    def version(param):
+        """`param`: the tensor — or the list of ALL tensors — a cached value is derived from."""
         if isinstance(param, (list, tuple)):
-            ver = tuple((q.data_ptr(), q._version) for q in param)
-        else:
-            ver = (param.data_ptr(), param._version)
+            return tuple((q.data_ptr(), q._version) for q in param)
+        return (param.data_ptr(), param._version)
+
+    def get(self, key, param, make):
+        ver = self.version(param)
         e = self.d.get(key)
         if e is None or e[0] != ver:
             e = (ver, make())
@@ -300,49 +303,17 @@ def _pad_vec(b, n):
     return o
 
 
-def _fused_rdb_filters(cache, params, L, r, nf):
-    """Dense-block N-fusion: launch j multiplies ONE input chunk (x for j=1, x_{j-1} otherwise) against the
-    filters of ALL convs k >= j that consume it, stacked along Cout.  Returns [(w_packed, bias)] for j=1..5."""
-    out = []
-    for j in range(1, 6):
-        lo, hi = (0, nf) if j == 1 else (nf + (j - 2) * GC, nf + (j - 1) * GC)
-        ks = list(range(j, 6))
-        wj = params[2 * L.rdb_conv(r, j)]
-
-        def stacked(lo=lo, hi=hi, ks=ks):
-            return torch.cat([params[2 * L.rdb_conv(r, k)].detach()[:, lo:hi] for k in ks], 0).float().contiguous()
-
-        def make_w(stacked=stacked):
-            return ops.pack_filter_tc(stacked(), TC_FPROP)
-
-        def make_b(j=j, ks=ks):
-            bj = params[2 * L.rdb_conv(r, j) + 1].detach().float()
-            n = sum(params[2 * L.rdb_conv(r, k)].shape[0] for k in ks)
-            b = torch.zeros(n, dtype=torch.float32, device=bj.device)
-            b[:bj.shape[0]] = bj          # the bias of conv j is added when conv j completes (this launch)
-            return b
-
-        wsrc = [params[2 * L.rdb_conv(r, k)] for k in ks]            # every filter the stack is built from
-        bj_p = params[2 * L.rdb_conv(r, j) + 1]
-        ent = [cache.get(('fw', r, j), wsrc, make_w), cache.get(('fb', r, j), bj_p, make_b)]
-        out.append(tuple(ent))
-    return out
-
-
-# Dense-block schedules (inference): which (conv k, input chunk) products each of the five launches computes.  Launch j
-# always completes conv j (bias + LeakyReLU on its GC columns); the other columns of a launch extend partial sums of later
-# convs IN PLACE in the channel slots their activations will occupy (conv5: the extra 64-channel slot).  Launch 1 touches
-# every conv, so all later launches read their partial sums through the `pre` addend.
-#   SCHED2 (round 1):  1: x -> x1 | p2 p3 p4 p5   2: x1 -> x2 | p3   3: x2 -> x3 | p4   4: x1,x3 -> x4 | p5   5: x2,x4 -> out
-#                      34 x 64 B per pixel of DRAM traffic, 9 chunk-passes of MMAs
-#   SCHED3 (round 2):  1: x -> x1 | p2 p3 p4 p5   2: x1 -> x2        3: x1,x2 -> x3 | p4   4: x3 -> x4      5: x1..x4 -> out
-#                      30 x 64 B per pixel, 11 chunk-passes: every partial sum is written once and read once.
-SCHED2 = ((('x',), (1, 2, 3, 4, 5)), ((1,), (2, 3)), ((2,), (3, 4)), ((1, 3), (4, 5)), ((2, 4), (5,)))
+# Dense-block schedules: which (conv k, input chunk) products each of the five launches computes.  Launch j always
+# completes conv j (bias + LeakyReLU on its GC columns); the other columns of a launch extend partial sums of later convs
+# IN PLACE in the channel slots their activations will occupy (conv5: the extra nf-channel slot).  Launch 1 touches every
+# conv, so all later launches read their partial sums through the `pre` addend.
+#   SCHED1:  launch j reads one chunk (x, then x_{j-1}) and carries the partial sums of every conv k >= j.
+#            Training, and inference with nf != 64.
+#   SCHED3:  1: x -> x1 | p2 p3 p4 p5   2: x1 -> x2   3: x1,x2 -> x3 | p4   4: x3 -> x4   5: x1..x4 -> out
+#            30 x 64 B per pixel of DRAM traffic, 11 chunk-passes: every partial sum is written once and read once.
+#            Inference with nf == 64.
+SCHED1 = ((('x',), (1, 2, 3, 4, 5)), ((1,), (2, 3, 4, 5)), ((2,), (3, 4, 5)), ((3,), (4, 5)), ((4,), (5,)))
 SCHED3 = ((('x',), (1, 2, 3, 4, 5)), ((1,), (2,)), ((1, 2), (3, 4)), ((3,), (4,)), ((1, 2, 3, 4), (5,)))
-# 4: like 3, but conv5's product with x moves from launch 1 (as a 64-channel partial sum: one slab written, one read back) to
-#    launch 5, which reads x as two more input chunks: 28 instead of 30 slabs of DRAM traffic for 12 instead of 11 chunk passes
-SCHED4 = ((('x',), (1, 2, 3, 4)), ((1,), (2,)), ((1, 2), (3, 4)), ((3,), (4,)), (('x', 1, 2, 3, 4), (5,)))
-SCHEDULES = {'2': SCHED2, '3': SCHED3, '4': SCHED4}
 
 
 def check_schedule(sched):
@@ -362,15 +333,18 @@ def check_schedule(sched):
     return True
 
 
-def _sched2_chunk_offsets(nf, chunk):
-    return [0, 32] if chunk == 'x' else [nf + (chunk - 1) * GC]
+def _chunk_offsets(nf, chunk):
+    """Channel offsets of the 32-channel chunks of input `chunk` ('x' or activation k) in the [x | x1..x4 | p5] buffer."""
+    return list(range(0, nf, 32)) if chunk == 'x' else [nf + (chunk - 1) * GC]
 
 
 def _sched_rdb_filters(cache, params, L, r, nf, sched, tag, dtype=torch.bfloat16):
-    """[(packed filters, bias, chunk channel offsets)] of the five launches of schedule `sched` for dense block r."""
+    """[(packed filters, bias, chunk channel offsets)] of the five launches of schedule `sched` for dense block r: launch j
+    multiplies its input chunks against the filters of every conv it touches, stacked along Cout.  Cache keys
+    (tag + 'w' | tag + 'b', r, j)."""
     out = []
     for j, (chunks, ks) in enumerate(sched, start=1):
-        offs = [o for c in chunks for o in _sched2_chunk_offsets(nf, c)]
+        offs = [o for c in chunks for o in _chunk_offsets(nf, c)]
         wj = params[2 * L.rdb_conv(r, j)]
 
         def make_w(offs=offs, ks=ks):
@@ -382,15 +356,11 @@ def _sched_rdb_filters(cache, params, L, r, nf, sched, tag, dtype=torch.bfloat16
             bj = params[2 * L.rdb_conv(r, j) + 1].detach().float()
             n = sum(params[2 * L.rdb_conv(r, k)].shape[0] for k in ks)
             b = torch.zeros(n, dtype=torch.float32, device=bj.device)
-            b[:bj.shape[0]] = bj
+            b[:bj.shape[0]] = bj          # the bias of conv j is added when conv j completes (this launch)
             return b
-        wsrc = [params[2 * L.rdb_conv(r, k)] for k in ks]
+        wsrc = [params[2 * L.rdb_conv(r, k)] for k in ks]            # every filter the stack is built from
         out.append((cache.get((tag + 'w', r, j), wsrc, make_w), cache.get((tag + 'b', r, j), params[2 * L.rdb_conv(r, j) + 1], make_b), offs))
     return out
-
-
-def _sched2_rdb_filters(cache, params, L, r, nf):
-    return _sched_rdb_filters(cache, params, L, r, nf, SCHED2, 's2')
 
 
 class _BatchPacker:
@@ -401,18 +371,13 @@ class _BatchPacker:
     ones seen at construction — i.e. for graph capture right after; replays call launch() from inside the graph)."""
 
     def __init__(self, params, L, nf):
-        import ctypes as C
         from ._lib import PackJob
         dev = params[0].device
         self.cache = _PackCache()
         jobs, keep = [], []
         W = lambda i: params[2 * i]
         Bv = lambda i: params[2 * i + 1]
-
-        def ver(p):
-            if isinstance(p, (list, tuple)):
-                return tuple((q.data_ptr(), q._version) for q in p)
-            return (p.data_ptr(), p._version)
+        ver = _PackCache.version
 
         def add(key, param, kind, rows_total, k_ch, parts, nvar_taps):
             # parts: [(src param, ci_lo, ci_n, cout_rows, k_pad, row_off)]
@@ -460,15 +425,17 @@ class _BatchPacker:
             fprop(L.i_hr1, cout_to=16); bias_copy(('b', L.i_hr1, 16), Bv(L.i_hr1), Bv(L.i_hr1), 16)
         dgrad(L.i_hr1, cout_to=32)
         for r in range(L.n_rdb):
-            for j in range(1, 6):
-                lo, hi = (0, nf) if j == 1 else (nf + (j - 2) * GC, nf + (j - 1) * GC)
-                ks = list(range(j, 6))
-                couts = [W(L.rdb_conv(r, k)).shape[0] for k in ks]
+            # the filter stacks of the training schedule, under the keys _sched_rdb_filters(..., SCHED1, 'f') uses
+            for j, (chunks, ks) in enumerate(SCHED1, start=1):
+                offs = [o for c in chunks for o in _chunk_offsets(nf, c)]
+                lo, n = offs[0], 32 * len(offs)
+                assert offs == list(range(lo, lo + n, 32)), 'a PackJob packs one contiguous input channel range'
                 parts, off = [], 0
-                for k, co in zip(ks, couts):
-                    parts.append((W(L.rdb_conv(r, k)), lo, hi - lo, co, 0, off))
+                for k in ks:
+                    co = W(L.rdb_conv(r, k)).shape[0]
+                    parts.append((W(L.rdb_conv(r, k)), lo, n, co, 0, off))
                     off += co
-                add(('fw', r, j), [W(L.rdb_conv(r, k)) for k in ks], TC_FPROP, off, hi - lo, parts, 9)
+                add(('fw', r, j), [W(L.rdb_conv(r, k)) for k in ks], TC_FPROP, off, n, parts, 9)
                 bias_copy(('fb', r, j), Bv(L.rdb_conv(r, j)), Bv(L.rdb_conv(r, j)), off)
                 dgrad(L.rdb_conv(r, j))
         arr = (PackJob * len(jobs))(*jobs)
@@ -483,7 +450,6 @@ class _BatchPacker:
 
 
 PAIR_MODE = os.environ.get('DASR_B200_PAIR', '1') != '0'      # run eligible launches on the CTA-pair kernel (conv_tc2)
-PAIR_STAGE1 = PAIR_MODE
 TILE_REV = os.environ.get('DASR_B200_TILE_REV', '1') != '0'
 
 
@@ -492,7 +458,7 @@ def _rdb_stage1(b, w, bias, out, nf, tile_rev=False):
     first GC columns (= x1).  One CTA cannot keep the 192-wide filter set resident, so the single-CTA kernel runs it as
     two Cout tiles of 96 that each load the activation tile; the cluster pair splits the filters over two SMs and
     multicasts one load of the activation tile into both."""
-    if PAIR_STAGE1 and nf == 64 and GC == 32:
+    if PAIR_MODE and nf == 64:
         ops.conv_tc(View(b, nf, 0), w, bias, out, act=ACT_LRELU, slope=0.2, act_cols=GC, pair=True, tile_rev=tile_rev)
     else:
         ops.conv_tc(View(b, nf, 0), w, bias, out, nt=out.c // 2, act=ACT_LRELU, slope=0.2, act_cols=GC)
@@ -523,69 +489,62 @@ def _tc_packers(params, cache, hk, bf):
     return wk, bk
 
 
-def _rdb_bf16(b, dst, r, tail, params, L, cache, sched_id, fused, half, wk, bk):
-    """The five wgmma launches of dense block r on its concat buffer b; conv5 writes dst with the epilogue `tail`
-    (alpha / res1 / res2 / weight map, forwarded to ops.conv_tc).  sched_id: dense-block schedule (None: the fused=True /
-    fused=False forms below)."""
+def _rdb_bf16(b, dst, r, tail, params, L, cache, half, wk, bk, sched=None, tile_rev=False, chunk_list=False):
+    """The five wgmma launches of dense block r on its concat buffer b = [x | x1..x4 | conv5 partial sums]; conv5 writes dst
+    with the epilogue `tail` (alpha / res1 / res2 / weight map, forwarded to ops.conv_tc).
+    sched     : dense-block schedule (SCHED1 / SCHED3): launch j completes conv j and carries partial sums of later convs.
+                None: one launch per conv over the growing concat (the per-layer form, the reference of the tests).
+    tile_rev  : consecutive launches walk the tile grid in opposite directions, so each one starts with the tiles the
+                previous one wrote last, which are still in L2 (DASR_B200_TILE_REV=0: always forwards).
+    chunk_list: launches 2..5 name their input chunks in a chunk list (ops.conv_tc chunks=); otherwise a launch reads its
+                one chunk as a 32-channel slice of b.  The kernel treats a one-chunk list and such a slice alike."""
     nf = L.nf
-    hk = 'h' if half else ''
-    bf = torch.float16 if half else torch.bfloat16
     CS = nf + 4 * GC
-    BW = CS + (nf if fused else 0)
-    if sched_id is not None:
-        if sched_id == '4' and r % 3 == 2:
-            # the third block of an RRDB carries two residual tiles per epilogue slot: with the K = 192 filter set of
-            # schedule 4's last launch they do not fit shared memory -> schedule 3 for these blocks
-            sched, stag = SCHED3, 's3' + hk
-        else:
-            sched, stag = SCHEDULES[sched_id], 's' + sched_id + hk
-        fw = _sched_rdb_filters(cache, params, L, r, nf, sched, stag, bf)
-        # consecutive launches walk the tile grid in opposite directions: each one starts with the tiles the previous
-        # one wrote last, which are still in L2 (DASR_B200_TILE_REV=0: always forwards)
-        rev = lambda j: TILE_REV and PAIR_MODE and ((5 * r + j) & 1) == 1
-        w1 = sum(nf if k == 5 else GC for k in sched[0][1])            # launch 1: x1 | partial sums of the convs it starts
-        _rdb_stage1(b, fw[0][0], fw[0][1], View(b, w1, nf), nf, tile_rev=rev(1))
-        for j in (2, 3, 4, 5):
-            ks = sched[j - 1][1]
-            width = sum(nf if k == 5 else GC for k in ks)
-            pair = PAIR_MODE                              # every dense-block launch runs on a CTA pair
-            if j < 5:
-                o = View(b, width, nf + (j - 1) * GC)                  # slots of conv j .. conv ks[-1], partial sums in place
-                ops.conv_tc(b, fw[j - 1][0], fw[j - 1][1], o, act=ACT_LRELU, slope=0.2, act_cols=GC, pre=o,
-                            chunks=fw[j - 1][2], pair=pair, tile_rev=rev(j))
-            else:
-                pre5 = View(b, nf, CS) if any(5 in kk for _, kk in sched[:4]) else None     # conv5 started earlier?
-                ops.conv_tc(b, fw[4][0], fw[4][1], dst, pre=pre5, chunks=fw[4][2], pair=pair, tile_rev=rev(5), **tail)
-    elif fused:
-        if half:
-            raise ops._lib.DasrError('half precision needs dense-block schedule 2 or 3 (DASR_B200_SCHED) or fused=False')
-        fw = _fused_rdb_filters(cache, params, L, r, nf)
-        # launch 1: x -> x1 (complete) | partial conv2..5
-        _rdb_stage1(b, fw[0][0], fw[0][1], View(b, BW - nf, nf), nf)
-        for j in (2, 3, 4):   # x_{j-1} -> x_j (complete) | partial conv_{j+1..5}, accumulated in place
-            o = View(b, BW - nf - (j - 1) * GC, nf + (j - 1) * GC)
-            ops.conv_tc(View(b, GC, nf + (j - 2) * GC), fw[j - 1][0], fw[j - 1][1], o, act=ACT_LRELU, slope=0.2,
-                        act_cols=GC, pre=o, pair=PAIR_MODE)
-        ops.conv_tc(View(b, GC, nf + 3 * GC), fw[4][0], fw[4][1], dst, pre=View(b, nf, CS), pair=PAIR_MODE and nf % 64 == 0, **tail)
-    else:
+    if sched is None:
         for k in range(1, 5):
             ci = L.rdb_conv(r, k)
             ops.conv_tc(View(b, _rdb_cin(nf, k), 0), wk(ci), bk(ci), View(b, GC, nf + (k - 1) * GC), act=ACT_LRELU, slope=0.2)
         ci = L.rdb_conv(r, 5)
         ops.conv_tc(View(b, CS, 0), wk(ci), bk(ci), dst, nt=_pick_nt(nf, CS), **tail)
+        return
+    tag = ('f' if sched is SCHED1 else 's3') + ('h' if half else '')
+    fw = _sched_rdb_filters(cache, params, L, r, nf, sched, tag, torch.float16 if half else torch.bfloat16)
+    rev = lambda j: tile_rev and TILE_REV and PAIR_MODE and ((5 * r + j) & 1) == 1
+    w1 = sum(nf if k == 5 else GC for k in sched[0][1])            # launch 1: x1 | partial sums of the convs it starts
+    _rdb_stage1(b, fw[0][0], fw[0][1], View(b, w1, nf), nf, tile_rev=rev(1))
+    for j in (2, 3, 4, 5):
+        w, bias, offs = fw[j - 1]
+        if chunk_list:
+            inp, chunks = b, offs
+        else:
+            assert len(offs) == 1, 'a launch that reads several chunks needs chunk_list'
+            inp, chunks = View(b, 32, offs[0]), None
+        if j < 5:
+            ks = sched[j - 1][1]
+            o = View(b, sum(nf if k == 5 else GC for k in ks), nf + (j - 1) * GC)     # slots of conv j .. ks[-1], in place
+            ops.conv_tc(inp, w, bias, o, act=ACT_LRELU, slope=0.2, act_cols=GC, pre=o, chunks=chunks, pair=PAIR_MODE,
+                        tile_rev=rev(j))
+        else:
+            pre5 = View(b, nf, CS) if any(5 in kk for _, kk in sched[:4]) else None     # conv5 started earlier?
+            ops.conv_tc(inp, w, bias, dst, pre=pre5, chunks=chunks, pair=PAIR_MODE and nf % 64 == 0, tile_rev=rev(5), **tail)
 
 
-def _trunk_tail_bf16(bufs, fea, L, params, cache, wk, bk, hk, bf):
+def _trunk_tail_bf16(bufs, fea, L, params, cache, wk, bk, hk, bf, pair=True, save=False):
     """fea + LR_conv(trunk) -> nearest-x2 upconvs -> HR_conv0 -> HR_conv1 on the wgmma kernels; the trunk is the x slot of
-    bufs[-1].  `bufs` (the dense-block buffers) is emptied once LR_conv has read them, so their memory returns to the pool
-    before the 4x-resolution layers allocate theirs.  Returns NCHW fp32."""
+    bufs[-1].  Returns (out NCHW fp32, ups, h0).
+    pair: LR_conv and HR_conv0 run on the cluster pair (when PAIR_MODE and nf % 64 == 0).
+    save: keep what the backward reads: `bufs`, ups = [LR_conv + fea, upconv outputs...] and h0 = HR_conv0's output.
+          Without it ups and h0 are None, and `bufs` (the dense-block buffers) is emptied once LR_conv has read them, so
+          their memory returns to the pool before the 4x-resolution layers allocate theirs."""
     nf = L.nf
     x = fea
     N, H, W, _ = fea.shape
+    pair = pair and PAIR_MODE and nf % 64 == 0
     lr = _empty((N, H, W, nf), x, bf)
-    ops.conv_tc(View(bufs[-1], nf, 0), wk(L.i_lr), bk(L.i_lr), lr, nt=_pick_nt(nf, nf), res1=fea, beta1=1.0,
-                pair=PAIR_MODE and nf % 64 == 0)
-    bufs.clear()
+    ops.conv_tc(View(bufs[-1], nf, 0), wk(L.i_lr), bk(L.i_lr), lr, nt=_pick_nt(nf, nf), res1=fea, beta1=1.0, pair=pair)
+    ups = [lr] if save else None
+    if not save:
+        bufs.clear()
     cur, h, w = lr, H, W
     for u in range(L.n_up):
         h, w = 2 * h, 2 * w
@@ -593,45 +552,51 @@ def _trunk_tail_bf16(bufs, fea, L, params, cache, wk, bk, hk, bf):
         # nearest-x2 + 3x3 conv as four 2x2 sub-pixel convs with pre-summed filters (never materialise the 4x tensor)
         ops.conv_tc(cur, wk(L.i_up0 + u, TC_UPCONV), bk(L.i_up0 + u), nxt, kind=TC_UPCONV, nt=_pick_nt(nf, nf, 4),
                     act=ACT_LRELU, slope=0.2)
+        if save:
+            ups.append(nxt)
         cur = nxt
     h0 = _empty((N, h, w, nf), x, bf)
-    ops.conv_tc(cur, wk(L.i_hr0), bk(L.i_hr0), h0, nt=_pick_nt(nf, nf), act=ACT_LRELU, slope=0.2, pair=PAIR_MODE and nf % 64 == 0)
+    ops.conv_tc(cur, wk(L.i_hr0), bk(L.i_hr0), h0, nt=_pick_nt(nf, nf), act=ACT_LRELU, slope=0.2, pair=pair)
     del cur
     out_nc = params[2 * L.i_hr1].shape[0]
     out = _empty((N, out_nc, h, w), x)
     # last layer: Cout 3 -> one 16-wide wgmma N tile, epilogue writes the 3 real channels straight to NCHW fp32
     _last_layer(h0, out, params[2 * L.i_hr1], L.i_hr1, cache, wk, bk, hk, bf)
-    return out
+    return out, ups, (h0 if save else None)
 
 
-def rrdb_forward_bf16(x, params, nb, upscale=4, cache=None, fused=True, half=False):
+def rrdb_forward_bf16(x, params, nb, upscale=4, cache=None, per_layer=False, half=False):
     """wgmma bf16 forward (inference).  NCHW fp32 in -> NCHW fp32 out; bf16 NHWC in between.
 
-    fused=True : dense-block N-fusion.  Each RDB runs 5 launches; launch j reads one or two 32-channel chunks ONCE
-                 and produces conv j's output plus partial sums of later convs of the block (one wide-N wgmma
-                 instead of several N = 32 ones on the same A tile).  Partial sums live IN PLACE in the channel slots the
-                 finished activations will occupy (bf16), so the only extra state is a 64-channel slot for conv5.
-                 DASR_B200_SCHED=3 (default) / 2: engine.SCHED3 / SCHED2; =1: every launch carries all later partial sums.
-    fused=False: one launch per conv over the growing concat (the straightforward restatement).
-    half=True  : IEEE half instead of bf16 for filters, activations and partial sums (wgmma with F16 operands:
-                 same rate, 11 instead of 8 significand bits).  RRDBNet activations stay far inside half's range
-                 (|x| < 6.5e4); meant for inference, where it brings PSNR / SSIM within 3 decimals of the fp32 path.
+    per_layer=False: dense-block N-fusion.  Each RDB runs 5 launches; launch j reads one or more 32-channel chunks ONCE
+                     and produces conv j's output plus partial sums of later convs of the block (one wide-N wgmma
+                     instead of several N = 32 ones on the same A tile).  Partial sums live IN PLACE in the channel slots
+                     the finished activations will occupy, so the only extra state is an nf-channel slot for conv5.
+                     Schedule SCHED3 when nf == 64, SCHED1 otherwise (bf16 only).
+    per_layer=True : one launch per conv over the growing concat (the straightforward restatement).
+    half=True      : IEEE half instead of bf16 for filters, activations and partial sums (wgmma with F16 operands:
+                     same rate, 11 instead of 8 significand bits).  RRDBNet activations stay far inside half's range
+                     (|x| < 6.5e4); meant for inference, where it brings PSNR / SSIM within 3 decimals of the fp32 path.
     """
     _need_cuda(x, 'RRDBNet')
     L = RRDBLayout(nb, params[0].shape[0], upscale)
     nf = L.nf
-    if nf % 32 or GC % 32:
+    if nf % 32:
         raise ops._lib.DasrError('bf16 path needs nf %% 32 == 0 (got %d)' % nf)
+    if per_layer:
+        sched = None
+    elif nf == 64:
+        sched = SCHED3
+    elif half:
+        raise ops._lib.DasrError('half precision with nf != 64 needs precision fp16_layer (got nf = %d)' % nf)
+    else:
+        sched = SCHED1
     cache = cache if cache is not None else _PackCache()
     N, in_nc, H, W = x.shape
     bf = torch.float16 if half else torch.bfloat16
     hk = 'h' if half else ''
-    CS = nf + 4 * GC
-    BW = CS + (nf if fused else 0)        # fused: extra slot for conv5's partial sums
-    sched_id = os.environ.get('DASR_B200_SCHED', '3')
-    sched = SCHEDULES.get(sched_id) if (fused and nf == 64 and GC == 32) else None
+    BW = nf + 4 * GC + (0 if per_layer else nf)        # N-fusion: extra slot for conv5's partial sums
     wk, bk = _tc_packers(params, cache, hk, bf)
-
     xin = torch.zeros((N, H, W, 32), dtype=bf, device=x.device)       # Cin 3 -> one zero-padded 32-channel chunk
     ops.nchw_to_nhwc(x.contiguous().float(), View(xin, in_nc, 0))
     n_rdb = L.n_rdb
@@ -641,21 +606,10 @@ def rrdb_forward_bf16(x, params, nb, upscale=4, cache=None, fused=True, half=Fal
     _mark('tc_begin')
     ops.conv_tc(xin, wk(L.i_fea, cin_to=32), bk(L.i_fea), fea)
     ops.axpby(fea, 1.0, None, 0.0, View(bufs[0], nf, 0))
-    # DASR_B200_BATCH_SPLIT=s (experiment): every dense block runs its five launches on one s-th of the batch at a time, so a
-    # launch finds a larger share of what its predecessor wrote in L2 — at the price of s times the launches
-    nsplit = max(1, min(N, int(os.environ.get('DASR_B200_BATCH_SPLIT', '1'))))
-    bounds = [(N * i // nsplit, N * (i + 1) // nsplit) for i in range(nsplit)]
-    for r, (n0, n1) in ((r, sl) for r in range(n_rdb) for sl in bounds):
-        b = bufs[r][n0:n1]
-        dst = View(bufs[r + 1][n0:n1], nf, 0)
-        if r % 3 == 2:      # (x5*0.2 + x)*0.2 + x_rrdb
-            tail = dict(alpha=0.04, res1=View(b, nf, 0), beta1=0.2, res2=View(bufs[r - 2][n0:n1], nf, 0), beta2=1.0)
-        else:
-            tail = dict(alpha=0.2, res1=View(b, nf, 0), beta1=1.0)
-        _rdb_bf16(b, dst, r, tail, params, L, cache, sched_id if sched is not None else None, fused, half, wk, bk)
-    out = _trunk_tail_bf16(bufs, fea, L, params, cache, wk, bk, hk, bf)
-    _mark('tc_end')
-    return out
+    for r in range(n_rdb):
+        _rdb_bf16(bufs[r], View(bufs[r + 1], nf, 0), r, _rrdb_tail(bufs, r, nf), params, L, cache, half, wk, bk, sched,
+                  tile_rev=sched is SCHED3, chunk_list=sched is SCHED3)
+    out, _, _ = _trunk_tail_bf16(bufs, fea, L, params, cache, wk, bk, hk, bf)
     _mark('tc_end')
     return out
 
@@ -701,9 +655,6 @@ def adaptive_rrdb_forward_bf16(x, amap, params, nb, nb_ada, concat, upscale=4, c
     bf = torch.float16 if half else torch.bfloat16
     hk = 'h' if half else ''
     BW = nf + 4 * GC + nf
-    sched_id = os.environ.get('DASR_B200_SCHED', '3')
-    if sched_id not in SCHEDULES:
-        raise ops._lib.DasrError('adaptive RRDB generator: DASR_B200_SCHED must be one of %s' % sorted(SCHEDULES))
     wk, bk = _tc_packers(params, cache, hk, bf)
     ext = _ada_ext(L, concat)
 
@@ -745,9 +696,9 @@ def adaptive_rrdb_forward_bf16(x, amap, params, nb, nb_ada, concat, upscale=4, c
                     conv64(tmp, ext(blk, 1), res)
                 if r % 3 == 2:
                     tail = dict(alpha=0.2, res1=u, beta1=1.0, res2=res, beta2=0.1, amap=a, map_mode=ops.MAP_SCALE)
-        _rdb_bf16(b, View(bufs[r + 1], nf, 0), r, tail, params, L, cache, sched_id, True, half, wk, bk)
+        _rdb_bf16(b, View(bufs[r + 1], nf, 0), r, tail, params, L, cache, half, wk, bk, SCHED3, tile_rev=True, chunk_list=True)
     del tmp, res
-    return _trunk_tail_bf16(bufs, fea, L, params, cache, wk, bk, hk, bf)
+    return _trunk_tail_bf16(bufs, fea, L, params, cache, wk, bk, hk, bf)[0]
 
 
 def adaptive_rrdb_forward_f32(x, amap, params, nb, nb_ada, concat, upscale=4):
@@ -808,62 +759,25 @@ def adaptive_rrdb_forward_f32(x, amap, params, nb, nb_ada, concat, upscale=4):
 # ---- bf16 wgmma training (mixed precision: bf16 activations/gradients, fp32 accumulation, fp32 filter grads) ----
 
 def rrdb_forward_bf16_train(x, params, nb, upscale=4, cache=None):
-    """Forward of the mixed-precision training mode: the dense-block N-fused wgmma schedule of the inference path,
-    but every RDB keeps its own buffer (the backward needs x, x1..x4)."""
+    """Forward of the mixed-precision training mode: the dense blocks run schedule SCHED1 on the wgmma kernels, and every
+    RDB keeps its own buffer (the backward needs x, x1..x4)."""
     _need_cuda(x, 'RRDBNet')
     L = RRDBLayout(nb, params[0].shape[0], upscale)
     nf = L.nf
     cache = cache if cache is not None else _PackCache()
     N, in_nc, H, W = x.shape
     bf = torch.bfloat16
-    CS = nf + 4 * GC
-    BW = CS + nf
-    Wt = lambda i: params[2 * i]
-
-    def wk(i, kind=TC_FPROP, cout_to=None, cin_to=None):
-        return cache.get(('w', i, kind), Wt(i), lambda: ops.pack_filter_tc(_pad_filter(Wt(i), cout_to, cin_to).float(), kind))
-
-    def bk(i, n=None):
-        p = params[2 * i + 1]
-        return cache.get(('b', i, n), p, lambda: _pad_vec(p.float(), n or p.shape[0]).contiguous())
-
+    wk, bk = _tc_packers(params, cache, '', bf)
     xin = torch.zeros((N, H, W, 32), dtype=bf, device=x.device)
     ops.nchw_to_nhwc(x.contiguous().float(), View(xin, in_nc, 0))
     fea = _empty((N, H, W, nf), x, bf)
     ops.conv_tc(xin, wk(L.i_fea, cin_to=32), bk(L.i_fea), fea)
     n_rdb = L.n_rdb
-    bufs = [_empty((N, H, W, BW), x, bf) for _ in range(n_rdb)] + [_empty((N, H, W, nf), x, bf)]
+    bufs = [_empty((N, H, W, nf + 4 * GC + nf), x, bf) for _ in range(n_rdb)] + [_empty((N, H, W, nf), x, bf)]
     ops.axpby(fea, 1.0, None, 0.0, View(bufs[0], nf, 0))
     for r in range(n_rdb):
-        b = bufs[r]
-        dst = View(bufs[r + 1], nf, 0)
-        if r % 3 == 2:
-            tail = dict(alpha=0.04, res1=View(b, nf, 0), beta1=0.2, res2=View(bufs[r - 2], nf, 0), beta2=1.0)
-        else:
-            tail = dict(alpha=0.2, res1=View(b, nf, 0), beta1=1.0)
-        fw = _fused_rdb_filters(cache, params, L, r, nf)
-        _rdb_stage1(b, fw[0][0], fw[0][1], View(b, BW - nf, nf), nf)
-        for j in (2, 3, 4):
-            o = View(b, BW - nf - (j - 1) * GC, nf + (j - 1) * GC)
-            ops.conv_tc(View(b, GC, nf + (j - 2) * GC), fw[j - 1][0], fw[j - 1][1], o, act=ACT_LRELU, slope=0.2, act_cols=GC, pre=o,
-                        pair=PAIR_MODE)
-        ops.conv_tc(View(b, GC, nf + 3 * GC), fw[4][0], fw[4][1], dst, pre=View(b, nf, CS), pair=PAIR_MODE and nf % 64 == 0, **tail)
-    lr = _empty((N, H, W, nf), x, bf)
-    ops.conv_tc(View(bufs[n_rdb], nf, 0), wk(L.i_lr), bk(L.i_lr), lr, nt=_pick_nt(nf, nf), res1=fea, beta1=1.0)
-    ups = [lr]
-    cur, h, w = lr, H, W
-    for u in range(L.n_up):
-        h, w = 2 * h, 2 * w
-        nxt = _empty((N, h, w, nf), x, bf)
-        ops.conv_tc(cur, wk(L.i_up0 + u, TC_UPCONV), bk(L.i_up0 + u), nxt, kind=TC_UPCONV, nt=_pick_nt(nf, nf, 4),
-                    act=ACT_LRELU, slope=0.2)
-        ups.append(nxt)
-        cur = nxt
-    h0 = _empty((N, h, w, nf), x, bf)
-    ops.conv_tc(cur, wk(L.i_hr0), bk(L.i_hr0), h0, nt=_pick_nt(nf, nf), act=ACT_LRELU, slope=0.2)
-    out_nc = Wt(L.i_hr1).shape[0]
-    out = _empty((N, out_nc, h, w), x)
-    _last_layer(h0, out, Wt(L.i_hr1), L.i_hr1, cache, wk, bk, '', bf)
+        _rdb_bf16(bufs[r], View(bufs[r + 1], nf, 0), r, _rrdb_tail(bufs, r, nf), params, L, cache, False, wk, bk, SCHED1)
+    out, ups, h0 = _trunk_tail_bf16(bufs, fea, L, params, cache, wk, bk, '', bf, pair=False, save=True)
     ctx = dict(L=L, xin=xin, fea=fea, bufs=bufs, ups=ups, h0=h0, shape=(N, in_nc, H, W))
     return out, ctx
 
@@ -882,7 +796,6 @@ def rrdb_backward_bf16(ctx, params, dout, cache=None, flat=None):
     """Backward of the mixed-precision mode: input gradients (dgrad) on the wgmma kernel (3x3 conv with flipped,
     transposed filters; gradient contributions of a dense block accumulate in place in one bf16 buffer), filter
     gradients on the wgmma wgrad kernel (MN-major operands straight from the NHWC tiles, fp32 register accumulation).  Returns fp32 grads."""
-    from .ops import TC_DGRAD
     L = ctx['L']
     nf = L.nf
     N, in_nc, H, W = ctx['shape']
@@ -962,17 +875,16 @@ def rrdb_backward_bf16(ctx, params, dout, cache=None, flat=None):
     g_y = _empty((N, H, W, nf), dev, bf)
     ops.conv_tc(g_lr, wd(L.i_lr), None, g_y, kind=TC_DGRAD, nt=_pick_nt(nf, nf))
 
-    fused_wgrad = nf == 64 and GC == 32 and os.environ.get('DASR_B200_RDB_WGRAD', '1') == '1'
+    fused_wgrad = nf == 64
     # The filter / bias gradients of a block depend on its finished gradient buffer but nothing downstream depends on
     # them: they run on a SIDE stream (fork / join inside the captured graph) and fill the SMs the latency-bound dgrad
     # chain of the next block leaves idle.  Two gradient buffers alternate; the main stream waits for the side stream's
     # readers of a buffer before the block after next overwrites it.
     overlap = fused_wgrad and os.environ.get('DASR_B200_BWD_OVERLAP', '1') == '1'
-    pair_dgrad = PAIR_MODE and nf == 64 and GC == 32 and os.environ.get('DASR_B200_PAIR_DGRAD', '0') == '1'
     # DASR_B200_FUSE_MASK=1: LeakyReLU backward of x1..x4 inside the epilogue of the dgrad launch that completes each slot (pair
     # kernel, activation in the res1 slot): 276 launches less per step, gradients within 4e-3
     # rel-L2 of the unfused ones (one rounding instead of two) -> off by default
-    fuse_mask = PAIR_STAGE1 and nf == 64 and GC == 32 and os.environ.get('DASR_B200_FUSE_MASK', '0') == '1'
+    fuse_mask = PAIR_MODE and nf == 64 and os.environ.get('DASR_B200_FUSE_MASK', '0') == '1'
     nset = 2 if overlap else 1
     GBs = [_empty((N, H, W, CS), dev, bf) for _ in range(nset)]
     gx5s = [_empty((N, H, W, nf), dev, bf) for _ in range(nset)]
@@ -996,7 +908,7 @@ def rrdb_backward_bf16(ctx, params, dout, cache=None, flat=None):
             wgrad(View(b, CS, 0), g_x5, ci)
         elif not overlap:
             ops.bias_grad(g_x5, gB(ci))
-        if PAIR_STAGE1 and nf == 64 and GC == 32:                                          # K=64 -> N=192 on a CTA pair
+        if PAIR_MODE and nf == 64:                                                         # K=64 -> N=192 on a CTA pair
             if fuse_mask:      # ... which also completes the gradient of x4: its LeakyReLU mask is applied in the epilogue
                 ops.conv_tc(g_x5, wd(ci), None, View(GB, CS, 0), kind=TC_DGRAD, pair=True, mask=View(b, CS, 0),
                             mask_c0=nf + 3 * GC, mask_c1=nf + 4 * GC, mask_slope=0.2)
@@ -1020,15 +932,14 @@ def rrdb_backward_bf16(ctx, params, dout, cache=None, flat=None):
                 ops.conv_tc(gk, wd(ci), None, o, kind=TC_DGRAD, pre=o, pair=True, mask=View(b, cin, 0),
                             mask_c0=cin - GC, mask_c1=cin, mask_slope=0.2)
             elif k > 1:
-                ops.conv_tc(gk, wd(ci), None, o, kind=TC_DGRAD, pre=o, pair=pair_dgrad)     # accumulate in place
+                ops.conv_tc(gk, wd(ci), None, o, kind=TC_DGRAD, pre=o)     # accumulate in place
             elif r % 3 == 0 and g_rrdb is not None:
                 # conv1's dgrad completes the block's input gradient: + what conv2..5 left in the x slot + the block skip
                 # (b1 * g_y) + the RRDB skip, written straight to the next gradient buffer (no separate add kernels)
-                ops.conv_tc(gk, wd(ci), None, g_new, kind=TC_DGRAD, pre=o, res1=g_y, beta1=b1, res2=g_rrdb, beta2=1.0,
-                            pair=pair_dgrad)
+                ops.conv_tc(gk, wd(ci), None, g_new, kind=TC_DGRAD, pre=o, res1=g_y, beta1=b1, res2=g_rrdb, beta2=1.0)
                 g_rrdb = None
             else:
-                ops.conv_tc(gk, wd(ci), None, g_new, kind=TC_DGRAD, pre=o, res1=g_y, beta1=b1, pair=pair_dgrad)
+                ops.conv_tc(gk, wd(ci), None, g_new, kind=TC_DGRAD, pre=o, res1=g_y, beta1=b1)
         c1, c5 = L.rdb_conv(r, 1), L.rdb_conv(r, 5)
 
         def reductions(b=b, GB=GB, g_x5=g_x5, c1=c1, c5=c5, r=r):

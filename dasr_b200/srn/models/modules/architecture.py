@@ -114,7 +114,7 @@ class RRDBNet(nn.Module):
             # 'bf16' / 'fp16' = dense-block N-fused launches (bf16 is the default); '*_layer' = one launch per conv;
             # fp16 = IEEE half operands on the same wgmma kernels (3 more significand bits, same speed)
             fn = lambda t: engine.rrdb_forward_bf16(t, params, self.nb, self.upscale, self._pack_cache,
-                                                    fused=not prec.endswith('_layer'), half=prec.startswith('fp16'))
+                                                    per_layer=prec.endswith('_layer'), half=prec.startswith('fp16'))
             if os.environ.get('DASR_B200_GRAPH', '1') == '0' or not x.is_cuda or engine.PROFILE is not None:
                 return fn(x)
             key = (tuple(x.shape), x.dtype, x.device.index, prec, tuple(p._version for p in params),

@@ -318,18 +318,19 @@ def test_bench_cpu_leg_and_generators_run():
 
 
 def test_dense_block_schedules_cover_every_product_once():
-    """engine.SCHED2 / SCHED3: every (conv k, input chunk c < k) product of the dense block is computed by exactly one
+    """engine.SCHED1 / SCHED3: every (conv k, input chunk c < k) product of the dense block is computed by exactly one
     launch, launch j completes conv j (first of its contiguous column set), only reads activations that already exist and
     launch 1 initialises every partial sum."""
     from dasr_b200 import engine
-    for sched in engine.SCHEDULES.values():
+    for sched in (engine.SCHED1, engine.SCHED3):
         assert engine.check_schedule(sched)
     bad = ((('x',), (1, 2, 3, 4, 5)), ((1,), (2,)), ((2,), (3, 4)), ((3,), (4,)), ((1, 2, 3, 4), (5,)))     # (3, x1) missing
     import pytest
     with pytest.raises(AssertionError):
         engine.check_schedule(bad)
     # channel offsets of the chunks inside the [x | x1..x4 | p5] buffer
-    assert engine._sched2_chunk_offsets(64, 'x') == [0, 32] and engine._sched2_chunk_offsets(64, 3) == [128]
+    assert engine._chunk_offsets(64, 'x') == [0, 32] and engine._chunk_offsets(64, 3) == [128]
+    assert engine._chunk_offsets(96, 'x') == [0, 32, 64] and engine._chunk_offsets(96, 1) == [96]
 
 
 def test_ddm_window_ranges_reproduce_the_reference_scatter(golden):
