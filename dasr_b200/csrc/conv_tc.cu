@@ -24,6 +24,7 @@
 // keeps only its half of the filters resident, and the leader's TMA multicasts every A halo tile into both CTAs, so an
 // activation tile crosses L2 -> SMEM once for the pair.  That is what lets a 192-wide filter set (221 KB) run as one tile.
 #include <stdlib.h>
+#include <type_traits>
 #include "tc_common.cuh"
 
 namespace dasr {
@@ -113,6 +114,26 @@ __device__ __forceinline__ void issue_tap(float* acc, uint32_t a_addr, uint64_t 
   }
 }
 
+// Ping-pong path: all taps of one A load for a warpgroup that owns a whole 128-pixel tile.  The tile is two m64 row
+// blocks (blk_off = 8 image rows down the halo tile); both take the same B descriptor per K step, so each thread holds N
+// accumulators, block 0 in acc[0, N/2) and block 1 in acc[N/2, N).  Products per output element run in the order of the
+// cooperative path (tap, then K step).
+template <int N, int NTAPS, int KS, int F16>
+__device__ __forceinline__ void issue_load_pp(float* acc, uint32_t a_base, uint32_t blk_off, uint64_t a_hi, const uint32_t* sTap,
+                                              uint32_t b_base, uint32_t b_tap, uint32_t b_slot, uint64_t b_hi, bool first) {
+#pragma unroll
+  for (int tap = 0; tap < NTAPS; tap++) {
+    const uint32_t at = a_base + sTap[tap], bt = b_base + (uint32_t)tap * b_tap;
+#pragma unroll
+    for (int ks = 0; ks < KS; ks++) {
+      const uint64_t db = make_desc(bt + (uint32_t)(ks >> 1) * b_slot + 32u * (ks & 1), b_hi);
+      const int sc = (first && tap == 0 && ks == 0) ? 0 : 1;
+      wgmma<N, F16, 0>(acc, make_desc(at + 32u * ks, a_hi), db, sc);
+      wgmma<N, F16, 0>(acc + N / 2, make_desc(at + blk_off + 32u * ks, a_hi), db, sc);
+    }
+  }
+}
+
 template <int F16>
 __device__ __forceinline__ void issue_tap_rt(int nt, float* acc, uint32_t a_addr, uint64_t a_hi, uint32_t b_addr, uint32_t b_slot,
                                              uint64_t b_hi, int ksteps, int first) {
@@ -126,10 +147,76 @@ __device__ __forceinline__ void issue_tap_rt(int nt, float* acc, uint32_t a_addr
   }
 }
 
+// Staged epilogue of one accumulator pair (channels co, co + 1 of tile pixel m; o = their byte offset in the staged tile):
+// pre addend, weight-map channel, activation, scale, res1 (or the dgrad mask carried in its slot), weight-map scale, res2,
+// then the bf16 / half pair goes back into the staged tile.  v0, v1 already carry the bias.
+template <bool HAS_PRE, int NRES, int MAP>
+__device__ __forceinline__ void staged_epi_pair(float v0, float v1, int co, uint32_t o, uint32_t bS, uint32_t bR1, uint32_t bR2,
+                                                const float* mv, const DasrConvTcParams& p, const float* map_w, bool mask_mode,
+                                                int f16) {
+  if constexpr (HAS_PRE) {
+    const float2 q = h16x2_to_f2(lds32(bS + o), f16);
+    v0 += q.x; v1 += q.y;
+  }
+  if constexpr (MAP == DASR_MAP_CHANNEL) {
+    const float* wa = map_w + co;
+#pragma unroll
+    for (int t = 0; t < 9; t++) {
+      v0 = fmaf(mv[t], __ldg(wa + t * p.cout), v0);
+      v1 = fmaf(mv[t], __ldg(wa + t * p.cout + 1), v1);
+    }
+  }
+  if (p.act != DASR_ACT_NONE && co < p.act_cols) {
+    if (p.act == DASR_ACT_LRELU) { v0 = fmaxf(v0, v0 * p.slope); v1 = fmaxf(v1, v1 * p.slope); }   // 0 < slope < 1
+    else { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+  }
+  v0 *= p.alpha; v1 *= p.alpha;
+  if constexpr (NRES >= 1) {
+    const uint32_t r = lds32(bR1 + o);
+    if (mask_mode) {
+      if (co >= p.mask_c0 && co < p.mask_c1) {    // a positive finite bf16 / half is a positive 16-bit integer
+        if (!((short)(r & 0xFFFF) > 0)) v0 *= p.mask_slope;
+        if (!((short)(r >> 16) > 0)) v1 *= p.mask_slope;
+      }
+    } else {
+      const float2 q = h16x2_to_f2(r, f16);
+      v0 = fmaf(p.beta1, q.x, v0); v1 = fmaf(p.beta1, q.y, v1);
+    }
+  }
+  if constexpr (MAP == DASR_MAP_SCALE) { v0 *= mv[0]; v1 *= mv[0]; }
+  if constexpr (NRES >= 2) {
+    const float2 q = h16x2_to_f2(lds32(bR2 + o), f16);
+    v0 = fmaf(p.beta2, q.x, v0); v1 = fmaf(p.beta2, q.y, v1);
+  }
+  sts32(bS + o, f2_to_h16x2(v0, v1, f16));
+}
+
+// Tile-phase trace (only in the selftest_trace build, compiled with -DDASR_TC_TRACE; the library never records):
+// clock64 stamps of the first TRACE_CTAS CTAs (grid row 0, i.e. the leader of a pair) for their first TRACE_TILES local tiles.
+#ifdef DASR_TC_TRACE
+constexpr int TRACE_CTAS = 8, TRACE_TILES = 48, TRACE_EV = 16;
+__device__ long long* g_tc_trace;
+#define TC_STAMP(lt, ev)                                                                                           \
+  do {                                                                                                             \
+    const uint32_t lt_ = (uint32_t)(lt);                                                                           \
+    if (g_tc_trace && blockIdx.x < TRACE_CTAS && blockIdx.y == 0 && lt_ < TRACE_TILES)                             \
+      g_tc_trace[((size_t)blockIdx.x * TRACE_TILES + lt_) * TRACE_EV + (ev)] = clock64();                          \
+  } while (0)
+#else
+#define TC_STAMP(lt, ev) do { } while (0)
+#endif
+// event slots of one tile: consumer warpgroup g (warp 4g, lane 0) at 5g + {0: first A wait begins, 1: last A wait ends,
+// 2: MMAs retired, 3: pre / sfree wait ends, 4: epilogue done}; producer: 15 empty wait of the first load begins,
+// 10: it ends, 11: last A load issued; epilogue TMA warp: 12 sfull wait ends, 13 stores issued, 14 stores have read the tile.
+enum { TEV_P_EMPTY = 10, TEV_P_ISSUED = 11, TEV_E_SFULL = 12, TEV_E_STORED = 13, TEV_E_READ = 14, TEV_P_EMPTY0 = 15 };
+
 // EPI_MODE / HAS_PRE / NRES are compile-time so that each instantiation carries only its own epilogue code.
 // MAP (staged epilogue only): 0 = no weight map; DASR_MAP_CHANNEL = one more input channel map_scale * map convolved with
 // the 3x3 taps map_w, added before the activation; DASR_MAP_SCALE = v = map * (alpha * act(...) + beta1 * res1) + beta2 * res2.
-template <int EPI_MODE, bool HAS_PRE, int NRES, int MAP = 0>
+// NT: 0 = cooperative consumers (both warpgroups on every tile, one 64-pixel half each; Cout tile p.nt at run time);
+// NT > 0 = ping-pong consumers for the staged epilogue without a map: warpgroup (it & 1) owns local tile it whole, the Cout
+// tile is NT and the tap loop (NTAPS taps) is unrolled, so one warpgroup's epilogue overlaps the other's MMAs.
+template <int EPI_MODE, bool HAS_PRE, int NRES, int MAP = 0, int NT = 0, int NTAPS = 9>
 __global__ void __launch_bounds__(TCK_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ CUtensorMap tmap_w,
                const __grid_constant__ EpiMaps em, const TcKernelArgs a) {
@@ -165,18 +252,20 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
   const bool pair = a.pair != 0;
   const uint32_t rank = pair ? cluster_ctarank() : 0u;
   const uint32_t a_row = a.chunk64 ? 2u * ROW_B : (uint32_t)ROW_B;    // bytes per pixel row of an A tile
+  static_assert(NT == 0 || (EPI_MODE == 0 && MAP == 0 && NT % 16 == 0 && NT <= 96), "ping-pong: staged epilogue, N <= 96");
+  constexpr int TILE_WARPS = NT ? 4 : CONS_WARPS;      // consumer warps that read one A stage / write one staged tile
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_in);
     tma_prefetch_desc(&tmap_w);
     for (int s = 0; s < a.stages; s++) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], CONS_WARPS * ((pair && rank == 0) ? 2 : 1));   // one arrive per consumer warp (of both CTAs)
+      mbar_init(&empty_bar[s], TILE_WARPS * ((pair && rank == 0) ? 2 : 1));   // one arrive per consumer warp (of both CTAs)
     }
     mbar_init(w_bar, 1);
     for (int b = 0; b < 4; b++) {
       mbar_init(&pre_bar[b], 1);
-      mbar_init(&sfull_bar[b], CONS_WARPS);
+      mbar_init(&sfull_bar[b], TILE_WARPS);
       mbar_init(&sfree_bar[b], 1);
     }
     fence_barrier_init();
@@ -214,11 +303,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
       pdl_wait();                        // activations come from the previous launch (filters / bias above do not)
       int stage = 0;
       uint32_t phase = 0;
-      for (long tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x) {
+      uint32_t it = 0;
+      for (long tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x, it++) {
         int x0, y0, n;
         tile_xyz(tile, x0, y0, n);
         for (int c = 0; c < a.nloads; c++) {
+          if (c == 0) TC_STAMP(it, TEV_P_EMPTY0);
           mbar_wait(&empty_bar[stage], phase ^ 1);
+          if (c == 0) TC_STAMP(it, TEV_P_EMPTY);
           uint8_t* dst = sA + (size_t)stage * a.a_stage_bytes;
           if (p.a_mode == 0) {
             // 64 channels per load when the slice allows it: half the TMA requests per byte
@@ -234,6 +326,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
           }
           if (++stage == a.stages) { stage = 0; phase ^= 1; }
         }
+        TC_STAMP(it, TEV_P_ISSUED);
       }
     }
     __syncwarp();
@@ -285,13 +378,18 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
           int x0, y0, n;
           tile_xyz(tile, x0, y0, n);
           mbar_wait(&sfull_bar[b], (it / (uint32_t)nbuf) & 1);
+          TC_STAMP(it, TEV_E_SFULL);
           for (int i = 0; i < nblocks; i++) {
             int col, off, k;
             staged_block(i, nb64, tail32, col, off, k);
             tma_store_4d(&em.m[k + omap], sS + b * a.epi_bytes + off, co_base + col, x0, y0, n);
           }
           bulk_commit();
-          if (prev_tile >= 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");   // the previous tile's stores have read their buffer
+          TC_STAMP(it, TEV_E_STORED);
+          if (prev_tile >= 0) {
+            asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");   // the previous tile's stores have read their buffer
+            TC_STAMP(it - 1, TEV_E_READ);
+          }
         }
         __syncwarp();
         if (prev_tile >= 0) retire(prev_tile, prev_b);
@@ -299,7 +397,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
         prev_b = b;
       }
       if (prev_tile >= 0) {
-        if (lane == 0) bulk_wait_read0();
+        if (lane == 0) {
+          bulk_wait_read0();
+          TC_STAMP(it - 1, TEV_E_READ);
+        }
         __syncwarp();
         retire(prev_tile, prev_b);
       }
@@ -328,6 +429,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
     const bool has_bias = a.bias != nullptr;
     const int r0 = 16 * wi + (lane >> 2);       // this thread's accumulator rows: r0 and r0 + 8 of the warpgroup's 64
     const int cq = 2 * (lane & 3);              // and columns 8j + cq, 8j + cq + 1
+    const bool rec = wi == 0 && lane == 0;      // records this warpgroup's tile-phase stamps (traced build only)
 
     auto release = [&](int s) {                 // this warp's wgmmas reading stage s have completed
       __syncwarp();
@@ -418,10 +520,86 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
         }
         asm volatile("bar.sync 1, %0;" ::"n"(CONS_WARPS * 32) : "memory");   // S may be overwritten by the next tile
       }
+    } else if constexpr (NT > 0) {
+      // Ping-pong: warpgroup wg takes local tiles wg, wg + 2, ...; the A ring and the staging buffers are indexed by the
+      // tile, as in the cooperative path.  Warpgroup (it & 1) starts waiting for the A loads of tile it only after the
+      // other warpgroup has seen every load of tile it - 1 land (named barrier 2 + ((it - 1) & 1)): every earlier phase
+      // of each A stage has then completed, so a parity wait can never be satisfied by a phase two rounds old.
+      constexpr int NB64 = NT / 64;
+      constexpr bool T32 = (NT & 32) != 0;
+      const uint32_t G = gridDim.x, ntiles = (uint32_t)a.ntiles;   // 32-bit tile arithmetic (checked on the host)
+      const uint32_t nl = (uint32_t)a.nloads, ns = (uint32_t)a.stages;
+      const uint32_t blk_off = 8u * HALO_W * a_row;
+      const uint32_t b_tap = (uint32_t)a.nchunks * b_slot;
+      // KS (K = 16 steps per A load: 4 with 64-channel loads) and the operand type are launch constants: one copy of the
+      // loop per combination, so no branch sits between the wgmmas that share the accumulators
+      auto run = [&](auto ks_c, auto f16_c) {
+        constexpr int KS = decltype(ks_c)::value, F16 = decltype(f16_c)::value;
+        float acc[NT];
+        for (; blockIdx.x + it * G < ntiles; it += 2) {     // local tile it is tile blockIdx.x + it * G
+          if (it > 0) asm volatile("bar.sync %0, 256;" ::"r"(2 + ((it - 1) & 1)) : "memory");
+          const uint32_t g0 = it * nl;
+          stage = (int)(g0 % ns);
+          phase = (g0 / ns) & 1;
+          int prev = -1;
+          if (rec) TC_STAMP(it, 5 * wg + 0);
+          for (int c = 0; c < a.nloads; c++) {
+            mbar_wait(&full_bar[stage], phase);
+            wgmma_fence();
+            issue_load_pp<NT, NTAPS, KS, F16>(acc, sA_u + (uint32_t)stage * a.a_stage_bytes, blk_off, a_hi, sTap,
+                                              sW_u + (uint32_t)(KS / 2) * (uint32_t)c * b_slot, b_tap, b_slot, b_hi, c == 0);
+            wgmma_commit();
+            if (prev >= 0) { wgmma_wait<1>(); release(prev); }
+            prev = stage;
+            if (++stage == a.stages) { stage = 0; phase ^= 1; }
+          }
+          if (rec) TC_STAMP(it, 5 * wg + 1);
+          if (blockIdx.x + (it + 1) * G < ntiles) asm volatile("bar.arrive %0, 256;" ::"r"(2 + (it & 1)) : "memory");   // tile it landed
+          wgmma_wait<0>();
+          fence_regs<NT>(acc);
+          release(prev);
+          if (rec) TC_STAMP(it, 5 * wg + 2);
+
+          const int sb = (int)(it % (uint32_t)nbuf);
+          const uint32_t sphase = (it / (uint32_t)nbuf) & 1;
+          const uint32_t bS = sS_u + sb * a.epi_bytes, bR1 = sR1_u + sb * a.epi_bytes, bR2 = sR2_u + sb * a.epi_bytes;
+          if (has_loads) mbar_wait(&pre_bar[sb], sphase);
+          else if (it >= (uint32_t)nbuf) mbar_wait(&sfree_bar[sb], sphase ^ 1);
+          if (rec) TC_STAMP(it, 5 * wg + 3);
+#pragma unroll
+          for (int blk = 0; blk < 2; blk++) {
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+              const int m = 64 * blk + r0 + 8 * h;
+#pragma unroll
+              for (int j = 0; j < NT / 8; j++) {
+                const int cl = 8 * j + cq;
+                float v0 = acc[blk * (NT / 2) + 4 * j + 2 * h], v1 = acc[blk * (NT / 2) + 4 * j + 2 * h + 1];
+                if (has_bias) { v0 += sBias[cl]; v1 += sBias[cl + 1]; }
+                staged_epi_pair<HAS_PRE, NRES, 0>(v0, v1, co_base + cl, staged_off(m, cl, NB64, T32), bS, bR1, bR2, nullptr, p,
+                                                  nullptr, mask_mode, F16);
+              }
+            }
+          }
+          fence_proxy_async();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&sfull_bar[sb]);
+          if (rec) TC_STAMP(it, 5 * wg + 4);
+        }
+      };
+      it = (uint32_t)wg;
+      if (a.chunk64) {
+        if (f16) run(std::integral_constant<int, 4>(), std::integral_constant<int, 1>());
+        else run(std::integral_constant<int, 4>(), std::integral_constant<int, 0>());
+      } else {
+        if (f16) run(std::integral_constant<int, 2>(), std::integral_constant<int, 1>());
+        else run(std::integral_constant<int, 2>(), std::integral_constant<int, 0>());
+      }
     } else {
       float acc[ACC_REGS];
       for (long tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x, it++) {
         int prev = -1;
+        if (rec) TC_STAMP(it, 5 * wg + 0);
         for (int c = 0; c < a.nloads; c++) {
           mbar_wait(&full_bar[stage], phase);
           const uint32_t a_base = sA_u + (uint32_t)stage * a.a_stage_bytes + wg_off;
@@ -441,9 +619,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
           prev = stage;
           if (++stage == a.stages) { stage = 0; phase ^= 1; }
         }
+        if (rec) TC_STAMP(it, 5 * wg + 1);
         wgmma_wait<0>();
         fence_regs<ACC_REGS>(acc);
         release(prev);
+        if (rec) TC_STAMP(it, 5 * wg + 2);
 
         int x0, y0, n;
         tile_xyz(tile, x0, y0, n);
@@ -453,6 +633,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
         if constexpr (EPI_MODE == 0) {
           if (has_loads) mbar_wait(&pre_bar[sb], sphase);                      // pre / residual tiles of this tile landed
           else if (it >= (uint32_t)nbuf) mbar_wait(&sfree_bar[sb], sphase ^ 1); // stores of tile it-nbuf have read the buffer
+          if (rec) TC_STAMP(it, 5 * wg + 3);
         }
 #pragma unroll
         for (int h = 0; h < 2; h++) {
@@ -483,42 +664,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
               if (has_bias) { v0 += sBias[cl]; v1 += sBias[cl + 1]; }
               const bool do_act = (act != DASR_ACT_NONE) && (co < p.act_cols);
               if constexpr (EPI_MODE == 0) {
-                const uint32_t o = staged_off(m, cl, nb64, tail32);
-                if constexpr (HAS_PRE) {
-                  const float2 q = h16x2_to_f2(lds32(bS + o), f16);
-                  v0 += q.x; v1 += q.y;
-                }
-                if constexpr (MAP == DASR_MAP_CHANNEL) {
-                  const float* wa = a.map_w + co;
-#pragma unroll
-                  for (int t = 0; t < 9; t++) {
-                    v0 = fmaf(mv[t], __ldg(wa + t * p.cout), v0);
-                    v1 = fmaf(mv[t], __ldg(wa + t * p.cout + 1), v1);
-                  }
-                }
-                if (do_act) {
-                  if (act == DASR_ACT_LRELU) { v0 = fmaxf(v0, v0 * slope); v1 = fmaxf(v1, v1 * slope); }   // 0 < slope < 1
-                  else { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-                }
-                v0 *= alpha; v1 *= alpha;
-                if constexpr (NRES >= 1) {
-                  const uint32_t r = lds32(bR1 + o);
-                  if (mask_mode) {
-                    if (co >= p.mask_c0 && co < p.mask_c1) {    // a positive finite bf16 / half is a positive 16-bit integer
-                      if (!((short)(r & 0xFFFF) > 0)) v0 *= p.mask_slope;
-                      if (!((short)(r >> 16) > 0)) v1 *= p.mask_slope;
-                    }
-                  } else {
-                    const float2 q = h16x2_to_f2(r, f16);
-                    v0 = fmaf(p.beta1, q.x, v0); v1 = fmaf(p.beta1, q.y, v1);
-                  }
-                }
-                if constexpr (MAP == DASR_MAP_SCALE) { v0 *= mv[0]; v1 *= mv[0]; }
-                if constexpr (NRES >= 2) {
-                  const float2 q = h16x2_to_f2(lds32(bR2 + o), f16);
-                  v0 = fmaf(p.beta2, q.x, v0); v1 = fmaf(p.beta2, q.y, v1);
-                }
-                sts32(bS + o, f2_to_h16x2(v0, v1, f16));
+                staged_epi_pair<HAS_PRE, NRES, MAP>(v0, v1, co, staged_off(m, cl, nb64, tail32), bS, bR1, bR2, mv, p, a.map_w,
+                                                    mask_mode, f16);
               } else if (valid) {
                 if (do_act) {
                   v0 = (act == DASR_ACT_LRELU) ? fmaxf(v0, v0 * slope) : fmaxf(v0, 0.f);
@@ -556,6 +703,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
           fence_proxy_async();          // generic-proxy writes of the staged tile -> visible to the TMA engine
           __syncwarp();
           if (lane == 0) mbar_arrive(&sfull_bar[sb]);
+          if (rec) TC_STAMP(it, 5 * wg + 4);
         }
       }
     }
@@ -834,6 +982,10 @@ static int tc_plan(int w_bytes, int a_stage, int epi_bytes, int nres_loaded, int
   return stages > MAX_STAGES ? MAX_STAGES : stages;
 }
 
+#ifdef DASR_TC_TRACE
+static int g_trace_coop = 0;   // traced build: 1 = every launch on the cooperative consumers (the before / after comparison)
+#endif
+
 static int chunk64_allowed() {
   static int ok = -1;
   if (ok < 0) {
@@ -957,14 +1109,36 @@ static int conv_tc_launch(const void* in, const void* w, const float* bias, cons
   if (p->map_mode == DASR_MAP_CHANNEL) ki = 9;
   else if (p->map_mode == DASR_MAP_SCALE) ki = 10 + a.has_pre;
   if (p->epi_mode == 0) DASR_REQUIRE(!(a.has_res2 && !a.has_res1), "conv_tc: res2 without res1");
+  // ping-pong consumers (compile-time Cout tile) for the staged epilogue without a weight map, instantiated for the launches
+  // of the inference forward: Cout tile 16 / 32 / 64 with 9 taps (dense-block launches 2-5, LR_conv, HR_conv0, the first
+  // conv), 96 with 9 taps and no pre / residual tiles (dense-block launch 1), 64 with 4 taps (the upconv sub-pixel
+  // variants).  Two tiles are in flight per CTA, so the staging ring needs nbuf >= 2.
+#define DASR_PP_ROW(n)                                                                                                 \
+  {conv_tc_kernel<0, false, 0, 0, n>, conv_tc_kernel<0, false, 1, 0, n>, conv_tc_kernel<0, false, 2, 0, n>,            \
+   conv_tc_kernel<0, true, 0, 0, n>,  conv_tc_kernel<0, true, 1, 0, n>,  conv_tc_kernel<0, true, 2, 0, n>}
+  static const KernelFn pp_kernels[5][6] = {DASR_PP_ROW(16), DASR_PP_ROW(32), DASR_PP_ROW(64),
+                                            {conv_tc_kernel<0, false, 0, 0, 96>}, {conv_tc_kernel<0, false, 0, 0, 64, 4>}};
+#undef DASR_PP_ROW
+  int pp = -1;
+  if (p->epi_mode == 0 && p->map_mode == 0 && p->a_mode == 0 && nbuf >= 2) {
+    if (p->ntaps == 9) pp = p->nt == 16 ? 0 : p->nt == 32 ? 1 : p->nt == 64 ? 2 : p->nt == 96 ? 3 : -1;
+    else if (p->ntaps == 4 && p->nt == 64) pp = 4;
+  }
+  if (pp >= 0 && !pp_kernels[pp][ki]) pp = -1;
+#ifdef DASR_TC_TRACE
+  if (g_trace_coop) pp = -1;
+#endif
+  const KernelFn fn = pp >= 0 ? pp_kernels[pp][ki] : kernels[ki];
   static bool attr_set[12] = {false, false, false, false, false, false, false, false, false, false, false, false};
-  if (!attr_set[ki]) {
-    cudaError_t e = cudaFuncSetAttribute(kernels[ki], cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
+  static bool attr_set_pp[5][6] = {};
+  bool& attr = pp >= 0 ? attr_set_pp[pp][ki] : attr_set[ki];
+  if (!attr) {
+    cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
     if (e != cudaSuccess) {
       set_error("conv_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
       return DASR_E_LAUNCH;
     }
-    attr_set[ki] = true;
+    attr = true;
   }
   int gy = p->nvar * a.n_ntiles;
   int gx = num_sms() / gy;
@@ -986,7 +1160,7 @@ static int conv_tc_launch(const void* in, const void* w, const float* bias, cons
   attrs[1].val.clusterDim.z = 1;
   cfg.attrs = attrs;
   cfg.numAttrs = pair ? 2 : 1;
-  cudaError_t le = cudaLaunchKernelEx(&cfg, kernels[ki], tm_in, tm_w, em, a);
+  cudaError_t le = cudaLaunchKernelEx(&cfg, fn, tm_in, tm_w, em, a);
   if (le != cudaSuccess) {
     cudaGetLastError();                 // reported here, not by the next launch's check
     set_error("conv_tc: launch failed: %s", cudaGetErrorString(le));
@@ -1147,6 +1321,17 @@ int dasr_conv_tc2_map(const void* in, const void* w, const float* bias, const vo
   if (rc) return rc;
   return conv_tc2_run(in, w, bias, pre, res1, res2, out, p, stream, map, map_w);
 }
+
+#ifdef DASR_TC_TRACE
+// traced selftest build only: where the tile-phase stamps go (nullptr: none) and which consumer schedule to launch
+int dasr_tc_trace_attach(long long* buf, int coop, int* ctas, int* tiles, int* events) {
+  g_trace_coop = coop;
+  *ctas = TRACE_CTAS;
+  *tiles = TRACE_TILES;
+  *events = TRACE_EV;
+  return cudaMemcpyToSymbol(g_tc_trace, &buf, sizeof(buf)) == cudaSuccess ? DASR_OK : DASR_E_LAUNCH;
+}
+#endif
 
 // selftest-only probe (declared in selftest.cu, not in the public header)
 int dasr_probe_tma_rate(int row_elems, int rows_per_box, int cs, int store, double* cycles_per_box) {

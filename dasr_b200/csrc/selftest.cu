@@ -1,7 +1,8 @@
 // Standalone GPU self-test / micro-benchmark of the C-ABI library (no Python, no torch).
-// Usage: selftest [check] [bench]      (default: both)
+// Usage: selftest [check] [bench]      (default: both)  |  selftest fused | tmarate | prof  |  selftest_trace trace
 // `check` compares every conv kernel with a CPU double-precision loop nest on small shapes;
-// `bench` times the RRDB-shaped tensor-core convs at BASELINE config 2 size (16 x 256 x 256).
+// `bench` times the RRDB-shaped tensor-core convs at BASELINE config 2 size (16 x 256 x 256);
+// `trace` (the -DDASR_TC_TRACE build only) prints the per-tile phases of the five dense-block launches.
 // Test infrastructure only — nothing here is on the product path.
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -10,6 +11,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <algorithm>
 #include <vector>
 #include "../../include/dasr_b200.h"
 
@@ -492,8 +494,13 @@ static void bench_tc_fused(int N, int H, int W, int cin, int cout, int nt, int w
   CK(cudaEventSynchronize(e1));
   float ms; cudaEventElapsedTime(&ms, e0, e1);
   ms /= iters;
-  double tiles_per_sm = (double)N * (H / 16) * (W / 8) / 148.0 * (cout / nt);
-  if (pair) tiles_per_sm = (double)N * (H / 16) * (W / 8) / 148.0;
+  // tiles one CTA (one SM) works through: the grid is (SMs / grid.y) x grid.y CTAs, grid.y = the Cout tiles of a launch
+  // (two CTAs per Cout tile in a cluster pair), and every grid column walks the pixel tiles of its Cout tile
+  int sms = 0;
+  CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0));
+  const int gy = (pair ? 2 : 1) * (cout / nt);
+  const int gx = sms / gy > 0 ? sms / gy : 1;
+  const double tiles_per_sm = (double)N * ((H + 15) / 16) * ((W + 7) / 8) / gx;
   printf("bench fused  %dx%dx%d K%-3d N%-3d nt%-3d pre%d %s%s: %8.3f ms  %7.1f TFLOP/s  %6.2f us/tile\n", N, H, W, cin, cout, nt,
          with_pre, planar ? "planar " : "", pair ? "pair " : "", ms, 2.0 * N * H * W * cin * cout * 9 / ms * 1e-9, ms * 1e3 / tiles_per_sm);
   if (planar) cudaFree(obuf);
@@ -522,6 +529,116 @@ static void bench_f32(int N, int H, int W, int cin, int cout, int iters) {
   cudaFree(din); cudaFree(dout); cudaFree(dw); cudaFree(db);
 }
 
+#ifdef DASR_TC_TRACE
+extern "C" int dasr_tc_trace_attach(long long* buf, int coop, int* ctas, int* tiles, int* events);
+
+static double median(std::vector<double> v) {
+  if (v.empty()) return NAN;
+  std::sort(v.begin(), v.end());
+  return v[v.size() / 2];
+}
+
+// The five dense-block launches of schedule 3 (engine.SCHED3 / engine._rdb_bf16, nf = 64) at 16 x 256 x 256 on one
+// 256-channel bf16 buffer [x | x1..x4 | conv5 partial sums], cluster pair, chunk lists, partial sums in place, tile walk
+// reversed on launches 1, 3, 5, launch 5 with the RRDB tail (res1 = x, res2 = the RRDB input).  For each launch: event time
+// and the median per-tile phases of the first CTAs (clock64 stamps, converted with the SM clock).
+static void trace_rdb(int coop) {
+  const int N = 16, H = 256, W = 256, CS = 256;
+  const size_t n = (size_t)N * H * W * CS;
+  __nv_bfloat16 *b = dalloc<__nv_bfloat16>(n), *dst = dalloc<__nv_bfloat16>(n), *rin = dalloc<__nv_bfloat16>(n);
+  int ctas, tiles, nev;
+  long long* dtr;
+  if (dasr_tc_trace_attach(nullptr, coop, &ctas, &tiles, &nev)) { printf("trace attach failed\n"); exit(2); }
+  CK(cudaMalloc(&dtr, (size_t)ctas * tiles * nev * 8));
+  int clk_khz = 0;
+  CK(cudaDeviceGetAttribute(&clk_khz, cudaDevAttrClockRate, 0));
+  const double cyc_per_us = clk_khz / 1e3;
+  struct Launch { int cin, cout, out_coff; std::vector<int> chunks; int pre_coff; int rev; int tail; };
+  const Launch ls[5] = {{64, 192, 64, {}, -1, 1, 0},       {32, 32, 96, {64}, 96, 0, 0},
+                        {64, 64, 128, {64, 96}, 128, 1, 0}, {32, 32, 160, {128}, 160, 0, 0},
+                        {128, 64, 0, {64, 96, 128, 160}, 192, 1, 1}};
+  printf("trace (%s consumers): median per tile, us; first %d CTAs (leader of each pair), tiles 2..%d\n",
+         coop ? "cooperative" : "ping-pong", ctas, tiles - 1);
+  printf("launch  K   N  us/launch us/tile | A-wait  MMA  epi-in-wait epilogue busy  period | prod: empty-wait issue-gap | "
+         "epi-TMA: sfull-lag store-issue read\n");
+  for (int li = 0; li < 5; li++) {
+    const Launch& L = ls[li];
+    std::vector<float> w((size_t)L.cout * L.cin * 9);
+    for (auto& v : w) v = rnd_q(4, 64.f);
+    float* dw = dalloc<float>(w.size());
+    h2d(dw, w);
+    void* dwp;
+    CK(cudaMalloc(&dwp, dasr_pack_filter_tc_bytes(L.cout, L.cin, 0)));
+    dasr_pack_filter_tc(dw, dwp, L.cout, L.cin, 0, 0);
+    float* bias = dalloc<float>(L.cout);
+    DasrConvTcParams p;
+    memset(&p, 0, sizeof(p));
+    dasr_conv_tc_setup(&p, 0);
+    p.N = N; p.H = H; p.W = W; p.cin = L.cin; p.in_cs = CS; p.in_coff = 0;
+    p.nchunk_list = (int)L.chunks.size();
+    for (size_t i = 0; i < L.chunks.size(); i++) p.chunk_off[i] = L.chunks[i];
+    p.cout = L.cout; p.out_cs = CS; p.out_coff = L.out_coff; p.nt = L.cout;
+    p.tile_rev = L.rev;
+    __nv_bfloat16* out = L.tail ? dst : b;
+    const void* pre = L.pre_coff >= 0 ? b : nullptr;
+    p.pre_cs = CS; p.pre_coff = L.pre_coff >= 0 ? L.pre_coff : 0;
+    if (L.tail) {
+      p.act = DASR_ACT_NONE; p.alpha = 0.04f; p.act_cols = 0;
+      p.res1_cs = CS; p.res1_coff = 0; p.beta1 = 0.2f; p.res2_cs = CS; p.res2_coff = 0; p.beta2 = 1.f;
+    } else {
+      p.act = DASR_ACT_LRELU; p.slope = 0.2f; p.alpha = 1.f; p.act_cols = 32;
+    }
+    auto run = [&]() {
+      return dasr_conv_tc2(b, dwp, bias, pre, L.tail ? b : nullptr, L.tail ? rin : nullptr, out, &p, 0);
+    };
+    int rc = 0;
+    for (int i = 0; i < 3; i++) rc |= run();
+    CK(cudaDeviceSynchronize());
+    if (rc) { printf("trace launch %d: rc=%d %s\n", li + 1, rc, dasr_last_error()); exit(3); }
+    cudaEvent_t e0, e1;
+    cudaEventCreate(&e0); cudaEventCreate(&e1);
+    const int iters = 20;
+    cudaEventRecord(e0);
+    for (int i = 0; i < iters; i++) run();
+    cudaEventRecord(e1);
+    CK(cudaEventSynchronize(e1));
+    float ms; cudaEventElapsedTime(&ms, e0, e1);
+    ms /= iters;
+    CK(cudaMemset(dtr, 0, (size_t)ctas * tiles * nev * 8));
+    dasr_tc_trace_attach(dtr, coop, &ctas, &tiles, &nev);
+    run();
+    CK(cudaDeviceSynchronize());
+    dasr_tc_trace_attach(nullptr, coop, &ctas, &tiles, &nev);
+    std::vector<long long> tr((size_t)ctas * tiles * nev);
+    CK(cudaMemcpy(tr.data(), dtr, tr.size() * 8, cudaMemcpyDeviceToHost));
+    std::vector<double> ph[11];
+    for (int c = 0; c < ctas; c++) {
+      auto ev = [&](int t, int e) { return tr[((size_t)c * tiles + t) * nev + e]; };
+      auto cons = [&](int t, int e) { return ev(t, 4) ? ev(t, e) : ev(t, 5 + e); };   // whichever warpgroup ran tile t
+      for (int t = 2; t < tiles; t++) {
+        if (!cons(t, 4) || !cons(t - 1, 4) || !ev(t, 11)) continue;
+        const double v[11] = {(double)(cons(t, 1) - cons(t, 0)), (double)(cons(t, 2) - cons(t, 1)),
+                              (double)(cons(t, 3) - cons(t, 2)), (double)(cons(t, 4) - cons(t, 3)),
+                              (double)(cons(t, 4) - cons(t, 0)), (double)(cons(t, 4) - cons(t - 1, 4)),
+                              (double)(ev(t, 10) - ev(t, 15)),   (double)(ev(t, 11) - ev(t - 1, 11)),
+                              (double)(ev(t, 12) - cons(t, 4)),  (double)(ev(t, 13) - ev(t, 12)),
+                              (double)(ev(t, 14) - ev(t, 13))};
+        for (int k = 0; k < 11; k++) ph[k].push_back(v[k] / cyc_per_us);
+      }
+    }
+    int sms = 0;
+    CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0));
+    const double tiles_per_cta = (double)N * (H / 16) * (W / 8) / (sms / 2);
+    printf("  %d   %3d %3d  %8.1f %6.2f  | %6.2f %5.2f %6.2f %9.2f %6.2f %6.2f | %6.2f %9.2f          | %6.2f %9.2f %6.2f\n",
+           li + 1, L.cin, L.cout, ms * 1e3, ms * 1e3 / tiles_per_cta, median(ph[0]), median(ph[1]), median(ph[2]),
+           median(ph[3]), median(ph[4]), median(ph[5]), median(ph[6]), median(ph[7]), median(ph[8]), median(ph[9]),
+           median(ph[10]));
+    cudaFree(dw); cudaFree(dwp); cudaFree(bias);
+  }
+  cudaFree(dtr); cudaFree(b); cudaFree(dst); cudaFree(rin);
+}
+#endif
+
 int main(int argc, char** argv) {
   bool do_check = argc == 1, do_bench = argc == 1;
   for (int i = 1; i < argc; i++) {
@@ -540,6 +657,16 @@ int main(int argc, char** argv) {
                    store ? "store" : "load ", re * 2, rows, pitch * 2, c, c / rows, re * 2.0 * rows / c, rc);
           }
       return 0;
+    }
+    if (!strcmp(argv[i], "trace")) {
+#ifdef DASR_TC_TRACE
+      trace_rdb(1);
+      trace_rdb(0);
+      return 0;
+#else
+      printf("trace: build the traced self-test (make ../lib/selftest_trace)\n");
+      return 2;
+#endif
     }
     if (!strcmp(argv[i], "fused")) {
       bench_tc_fused(16, 256, 256, 64, 192, 96, 0, 10);
@@ -667,6 +794,25 @@ int main(int argc, char** argv) {
         test_tc(1, 20, 13, 96, 32, 32, 0, 0, 2);       // single-CTA kernel, staged epilogue
         test_tc(1, 16, 16, 64, 64, 64, 2, 0, 0);       // upsample-fused (direct-store epilogue)
         test_tc(1, 21, 10, 64, 16, 16, 0, 0, 3);       // NCHW fp32 tail
+        g_f16 = 0;
+        // ping-pong consumers at every compile-time Cout tile (16 / 32 / 64 / 96 with 9 taps, 64 with 4): ragged images (the
+        // last tile row holds 2 of 16 rows, the last tile column 5 of 8) and tile counts that leave some CTAs an odd and
+        // some an even number of tiles (220 tiles over 66 columns of the grid: 3 or 4 each)
+        test_tc(5, 50, 85, 32, 32, 32, 0, 0, 5);       // N = 16 per CTA (pair), pre + res1 + res2
+        test_tc(5, 50, 85, 64, 64, 32, 0, 0, 2);       // N = 32, single CTA, two Cout tiles, 64-channel A loads
+        test_tc(5, 50, 85, 64, 64, 64, 0, 0, 5);       // N = 32 per CTA (pair)
+        test_tc(10, 50, 85, 64, 64, 64, 0, 0, 2);      // N = 64: 440 tiles over 132 CTAs
+        test_tc(4, 50, 85, 64, 192, 192, 0, 0, 4);     // N = 96 per CTA (pair), no loads: 176 tiles, 2 or 3 per cluster
+        g_tile_rev = 1;
+        test_tc(5, 50, 85, 32, 32, 32, 0, 0, 5);
+        test_tc(4, 50, 85, 64, 192, 192, 0, 0, 4);
+        g_tile_rev = 0;
+        g_up_staged = 1;
+        test_tc(2, 50, 45, 64, 64, 64, 2, 0, 0);       // 4 taps, N = 64: 48 tiles over 33 CTAs per variant
+        g_up_staged = 0;
+        g_f16 = 1;
+        test_tc(5, 50, 85, 64, 64, 64, 0, 0, 5);
+        test_tc(5, 50, 85, 32, 32, 32, 0, 0, 5);
         g_f16 = 0;
       }
       test_tc(1, 16, 16, 64, 64, 64, 2, am, 1);        // upsample-fused
