@@ -395,6 +395,17 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
         if (prev_tile >= 0) retire(prev_tile, prev_b);
         prev_tile = tile;
         prev_b = b;
+        if (nbuf == 1) {
+          // one staging buffer: the next tile's epilogue needs this buffer back (its pre / residual loads or sfree), so
+          // the retire cannot wait for the next tile's stores — that wait would never end
+          if (lane == 0) {
+            bulk_wait_read0();
+            TC_STAMP(it, TEV_E_READ);
+          }
+          __syncwarp();
+          retire(tile, b);
+          prev_tile = -1;
+        }
       }
       if (prev_tile >= 0) {
         if (lane == 0) {
@@ -1207,9 +1218,23 @@ static int conv_tc_run(const void* in, const void* w, const float* bias, const v
   } else {
     DASR_REQUIRE(!pre, "conv_tc: the pre-activation addend is only supported by the staged epilogue (epi_mode 0)");
   }
-  if (res1) DASR_REQUIRE(p->res1_cs % 8 == 0 && p->res1_coff % 8 == 0, "conv_tc: res1 alignment");
-  if (res2) DASR_REQUIRE(p->res2_cs % 8 == 0 && p->res2_coff % 8 == 0, "conv_tc: res2 alignment");
-  if (pre) DASR_REQUIRE(p->pre_cs % 8 == 0 && p->pre_coff % 8 == 0, "conv_tc: pre alignment");
+  // pre / residual channels [coff, coff + cout) of every output pixel: the direct epilogue reads them by pointer arithmetic
+  // (a wider slice would read the next pixel's channels), the staged one by TMA (which zero-fills beyond cs)
+  if (res1)
+    DASR_REQUIRE(p->res1_cs % 8 == 0 && p->res1_coff % 8 == 0 && p->res1_coff >= 0 && p->res1_coff + p->cout <= p->res1_cs,
+                 "conv_tc: res1 slice");
+  if (res2)
+    DASR_REQUIRE(p->res2_cs % 8 == 0 && p->res2_coff % 8 == 0 && p->res2_coff >= 0 && p->res2_coff + p->cout <= p->res2_cs,
+                 "conv_tc: res2 slice");
+  if (pre)
+    DASR_REQUIRE(p->pre_cs % 8 == 0 && p->pre_coff % 8 == 0 && p->pre_coff >= 0 && p->pre_coff + p->cout <= p->pre_cs,
+                 "conv_tc: pre slice");
+  // dgrad mask: output channel co in [mask_c0, mask_c1) is gated by mask channel mask_coff + co - mask_c0
+  if (mask_src)
+    DASR_REQUIRE(p->mask_c0 >= 0 && p->mask_c0 < p->mask_c1 && p->mask_c1 <= p->cout && p->mask_cs % 8 == 0 &&
+                     p->mask_coff % 8 == 0 && p->mask_coff >= 0 && p->mask_coff + (p->mask_c1 - p->mask_c0) <= p->mask_cs,
+                 "conv_tc: mask slice (mask_c0 %d, mask_c1 %d, cout %d, mask_coff %d, mask_cs %d)", p->mask_c0, p->mask_c1,
+                 p->cout, p->mask_coff, p->mask_cs);
   DASR_REQUIRE((reinterpret_cast<uintptr_t>(in) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0 &&
                    (reinterpret_cast<uintptr_t>(w) & 15) == 0,
                "conv_tc: pointers must be 16-byte aligned");

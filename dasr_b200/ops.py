@@ -258,12 +258,24 @@ def pack_filter_tc(w, kind, dtype=torch.bfloat16):
     return o
 
 
+def _check_operand(what, v, pix, width, dtype):
+    """An NHWC epilogue operand of conv_tc: [N, H, W] = pix, at least `width` channels, `dtype` (None: any)."""
+    if tuple(v.t.shape[:3]) != pix or v.t.dim() != 4:
+        raise _lib.DasrError('conv_tc: %s is %s, the launch needs [N, H, W] = %s' % (what, tuple(v.t.shape), pix))
+    if v.c < width:
+        raise _lib.DasrError('conv_tc: %s slice has %d channels, the launch needs %d' % (what, v.c, width))
+    if dtype is not None and v.t.dtype != dtype:
+        raise _lib.DasrError('conv_tc: %s is %s, the input is %s' % (what, v.t.dtype, dtype))
+
+
 def conv_tc(inp, w_packed, bias, out, kind=TC_FPROP, nt=None, act=ACT_NONE, slope=0.2, alpha=1.0, act_cols=None,
             pre=None, res1=None, beta1=0.0, res2=None, beta2=0.0, mask=None, mask_c0=0, mask_c1=0, mask_slope=0.2,
             a_mode=0, nchw_out=None, cout=None, tile_rev=False, chunks=None, pair=None, tapn=False, amap=None, map_mode=0,
             map_scale=1.0, map_w=None):
     """wgmma 3x3 conv on NHWC bf16 channel slices; chunks = optional list of 32-channel chunk offsets of `inp`'s buffer; `inp`/`out`/`pre`/`res*`/`mask` are Views (or tensors).
     v = alpha*act(acc + bias + pre) + beta1*res1 + beta2*res2, activation on the first `act_cols` channels only.
+    pre / res1 / res2 / mask have the output's [N, H, W] (the output resolution) and at least its channel count (mask: mask_c1);
+    output channels [mask_c0, mask_c1) are multiplied by mask_slope where channel mask.coff + co of the mask is not > 0.
     nchw_out: fp32 NCHW tensor — the launch writes its first nchw_out.shape[1] channels there (last layer).
     pair: True = run on the CTA-pair kernel (dasr_conv_tc2: 2-CTA cluster, filters split over two SMs, activation tiles multicast;
           plain 3x3 geometry, cout % 64 == 0, no mask; `nt` is ignored).
@@ -289,6 +301,18 @@ def conv_tc(inp, w_packed, bias, out, kind=TC_FPROP, nt=None, act=ACT_NONE, slop
         for i, c in enumerate(chunks):
             p.chunk_off[i] = c
     p.cout, p.out_cs, p.out_coff = out.c, out.cs, out.coff
+    # every NHWC operand of the epilogue is read at the output resolution, in channels [coff, coff + cout)
+    opix = (N, H * p.out_mul, W * p.out_mul)
+    _check_operand('output', out, opix, out.c, inp.t.dtype)
+    for what, v in (('pre', pre), ('res1', res1), ('res2', res2)):
+        if v is not None:
+            _check_operand(what, as_view(v), opix, out.c, inp.t.dtype)
+    if mask is not None:
+        if not 0 <= mask_c0 < mask_c1 <= out.c:
+            raise _lib.DasrError('conv_tc: mask range [%d, %d) outside the %d output channels' % (mask_c0, mask_c1, out.c))
+        _check_operand('mask', as_view(mask), opix, mask_c1, None)
+        if as_view(mask).t.dtype not in (torch.bfloat16, torch.float16):
+            raise _lib.DasrError('conv_tc: the mask must be a 16-bit tensor (got %s)' % as_view(mask).t.dtype)
     p.nt = nt if nt else out.c
     p.act, p.slope, p.alpha = act, slope, alpha
     p.act_cols = (out.c if act != ACT_NONE else 0) if act_cols is None else act_cols
@@ -307,8 +331,9 @@ def conv_tc(inp, w_packed, bias, out, kind=TC_FPROP, nt=None, act=ACT_NONE, slop
         res2 = as_view(res2)
         p.beta2, p.res2_cs, p.res2_coff = beta2, res2.cs, res2.coff
     if mask is not None:
+        # the mask is laid out like the output: channel mask.coff + co gates output channel co (both kernels)
         mask = as_view(mask)
-        p.mask_cs, p.mask_coff, p.mask_c0, p.mask_c1, p.mask_slope = mask.cs, mask.coff, mask_c0, mask_c1, mask_slope
+        p.mask_cs, p.mask_coff, p.mask_c0, p.mask_c1, p.mask_slope = mask.cs, mask.coff + mask_c0, mask_c0, mask_c1, mask_slope
     p.a_mode = a_mode
     p.tile_rev = int(bool(tile_rev))
     if amap is not None:

@@ -127,6 +127,9 @@ int dasr_pack_filter_f32(const float* w_oihw, float* w_packed, int cout, int cin
  * epilogue: v = alpha*act(acc + bias + pre) + beta1*res1 + beta2*res2 ;   (act on channels < act_cols only)
  *           channels [mask_c0,mask_c1) additionally multiplied by (mask_src>0 ? 1 : mask_slope)
  *           (LeakyReLU backward fused into the dgrad that completes a dense-block gradient slice).
+ *           pre / res1 / res2: channels [coff, coff + cout) of an NHWC tensor at the output resolution (coff + cout <= cs);
+ *           mask_src: output channel co reads mask channel mask_coff + co - mask_c0 (mask_coff + mask_c1 - mask_c0 <=
+ *           mask_cs, mask_c1 <= cout); dasr_conv_tc2 reads the mask in the res1 slot, channel res1_coff + co.
  * One variant with the 9 taps of a 3x3 = plain conv.  Four variants with 2x2 taps and pre-summed
  * filters = nearest-x2 upsample + 3x3 conv without materialising the upsampled tensor.
  * ---------------------------------------------------------------------------------------------- */
