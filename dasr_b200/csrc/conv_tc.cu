@@ -48,7 +48,9 @@ struct TcKernelArgs {
   const __nv_bfloat16* mask_src;
   void* out;
   int nchunks;       // cin / 32
-  int chunk64;       // 1: A tiles are loaded as 64-channel chunks (128 B rows, SWIZZLE_128B): half the TMA requests per byte
+  int chunk64;       // A tiles loaded as 64-channel chunks (128 B rows, SWIZZLE_128B): half the TMA requests per byte.
+                     // 1: K steps tap-major over the 64 channels; 2 (pair, ping-pong): channels 0-31 over all taps, then
+                     // 32-63, the products and order of two 32-channel loads
   int nloads;        // A loads per pixel tile: nchunks, or nchunks / 2 with chunk64
   int n_ntiles;      // cout / nt
   int tiles_x, tiles_y;
@@ -117,19 +119,25 @@ __device__ __forceinline__ void issue_tap(float* acc, uint32_t a_addr, uint64_t 
 // Ping-pong path: all taps of one A load for a warpgroup that owns a whole 128-pixel tile.  The tile is two m64 row
 // blocks (blk_off = 8 image rows down the halo tile); both take the same B descriptor per K step, so each thread holds N
 // accumulators, block 0 in acc[0, N/2) and block 1 in acc[N/2, N).  Products per output element run in the order of the
-// cooperative path (tap, then K step).
-template <int N, int NTAPS, int KS, int F16>
+// cooperative path (tap, then K step).  HALVES (a 64-channel load, KS = 4): channels 0-31 over all taps, then channels
+// 32-63 over all taps, the sequence two 32-channel loads issue, so every output element sums the same products in the same
+// order as with 32-channel loads.
+template <int N, int NTAPS, int KS, int F16, bool HALVES = false>
 __device__ __forceinline__ void issue_load_pp(float* acc, uint32_t a_base, uint32_t blk_off, uint64_t a_hi, const uint32_t* sTap,
                                               uint32_t b_base, uint32_t b_tap, uint32_t b_slot, uint64_t b_hi, bool first) {
+  constexpr int NH = HALVES ? 2 : 1, KH = KS / NH;
 #pragma unroll
-  for (int tap = 0; tap < NTAPS; tap++) {
-    const uint32_t at = a_base + sTap[tap], bt = b_base + (uint32_t)tap * b_tap;
+  for (int h = 0; h < NH; h++) {
 #pragma unroll
-    for (int ks = 0; ks < KS; ks++) {
-      const uint64_t db = make_desc(bt + (uint32_t)(ks >> 1) * b_slot + 32u * (ks & 1), b_hi);
-      const int sc = (first && tap == 0 && ks == 0) ? 0 : 1;
-      wgmma<N, F16, 0>(acc, make_desc(at + 32u * ks, a_hi), db, sc);
-      wgmma<N, F16, 0>(acc + N / 2, make_desc(at + blk_off + 32u * ks, a_hi), db, sc);
+    for (int tap = 0; tap < NTAPS; tap++) {
+      const uint32_t at = a_base + sTap[tap] + 64u * h, bt = b_base + (uint32_t)tap * b_tap + (uint32_t)h * b_slot;
+#pragma unroll
+      for (int ks = 0; ks < KH; ks++) {
+        const uint64_t db = make_desc(bt + (uint32_t)(ks >> 1) * b_slot + 32u * (ks & 1), b_hi);
+        const int sc = (first && h == 0 && tap == 0 && ks == 0) ? 0 : 1;
+        wgmma<N, F16, 0>(acc, make_desc(at + 32u * ks, a_hi), db, sc);
+        wgmma<N, F16, 0>(acc + N / 2, make_desc(at + blk_off + 32u * ks, a_hi), db, sc);
+      }
     }
   }
 }
@@ -313,8 +321,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
           if (c == 0) TC_STAMP(it, TEV_P_EMPTY);
           uint8_t* dst = sA + (size_t)stage * a.a_stage_bytes;
           if (p.a_mode == 0) {
-            // 64 channels per load when the slice allows it: half the TMA requests per byte
-            const int ch = a.chunk64 ? p.in_coff + c * 2 * CHUNK : (p.nchunk_list ? p.chunk_off[c] : p.in_coff + c * CHUNK);
+            // 64 channels per load when the slice or the chunk list allows it: half the TMA requests per byte
+            const int ch = p.nchunk_list ? p.chunk_off[a.chunk64 ? 2 * c : c] : p.in_coff + c * (a.chunk64 ? 2 : 1) * CHUNK;
             mbar_expect_tx(&full_bar[stage], (uint32_t)((a.chunk64 ? 2 : 1) * A_HALO_BYTES));
             if (!pair) tma_load_4d(dst, &tmap_in, &full_bar[stage], ch, x0 - 1, y0 - 1, n);
             else if (rank == 0) tma_load_4d_mc(dst, &tmap_in, &full_bar[stage], ch, x0 - 1, y0 - 1, n, (uint16_t)3);
@@ -544,8 +552,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
       const uint32_t b_tap = (uint32_t)a.nchunks * b_slot;
       // KS (K = 16 steps per A load: 4 with 64-channel loads) and the operand type are launch constants: one copy of the
       // loop per combination, so no branch sits between the wgmmas that share the accumulators
-      auto run = [&](auto ks_c, auto f16_c) {
+      auto run = [&](auto ks_c, auto f16_c, auto halves_c) {
         constexpr int KS = decltype(ks_c)::value, F16 = decltype(f16_c)::value;
+        constexpr bool HALVES = decltype(halves_c)::value;
         float acc[NT];
         for (; blockIdx.x + it * G < ntiles; it += 2) {     // local tile it is tile blockIdx.x + it * G
           if (it > 0) asm volatile("bar.sync %0, 256;" ::"r"(2 + ((it - 1) & 1)) : "memory");
@@ -557,8 +566,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
           for (int c = 0; c < a.nloads; c++) {
             mbar_wait(&full_bar[stage], phase);
             wgmma_fence();
-            issue_load_pp<NT, NTAPS, KS, F16>(acc, sA_u + (uint32_t)stage * a.a_stage_bytes, blk_off, a_hi, sTap,
-                                              sW_u + (uint32_t)(KS / 2) * (uint32_t)c * b_slot, b_tap, b_slot, b_hi, c == 0);
+            issue_load_pp<NT, NTAPS, KS, F16, HALVES>(acc, sA_u + (uint32_t)stage * a.a_stage_bytes, blk_off, a_hi, sTap,
+                                                      sW_u + (uint32_t)(KS / 2) * (uint32_t)c * b_slot, b_tap, b_slot, b_hi, c == 0);
             wgmma_commit();
             if (prev >= 0) { wgmma_wait<1>(); release(prev); }
             prev = stage;
@@ -599,12 +608,22 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
         }
       };
       it = (uint32_t)wg;
-      if (a.chunk64) {
-        if (f16) run(std::integral_constant<int, 4>(), std::integral_constant<int, 1>());
-        else run(std::integral_constant<int, 4>(), std::integral_constant<int, 0>());
+      using I1 = std::integral_constant<int, 1>;
+      using I0 = std::integral_constant<int, 0>;
+      using I2 = std::integral_constant<int, 2>;
+      using I4 = std::integral_constant<int, 4>;
+      using B0 = std::false_type;
+      if (a.chunk64 == 2) {
+        if constexpr (NTAPS == 9 && NT <= 64) {   // pair launches (plain 3x3 geometry) with Cout tiles up to 64 per CTA
+          if (f16) run(I4(), I1(), std::true_type());
+          else run(I4(), I0(), std::true_type());
+        }
+      } else if (a.chunk64) {
+        if (f16) run(I4(), I1(), B0());
+        else run(I4(), I0(), B0());
       } else {
-        if (f16) run(std::integral_constant<int, 2>(), std::integral_constant<int, 1>());
-        else run(std::integral_constant<int, 2>(), std::integral_constant<int, 0>());
+        if (f16) run(I2(), I1(), B0());
+        else run(I2(), I0(), B0());
       }
     } else {
       float acc[ACC_REGS];
@@ -997,13 +1016,26 @@ static int tc_plan(int w_bytes, int a_stage, int epi_bytes, int nres_loaded, int
 static int g_trace_coop = 0;   // traced build: 1 = every launch on the cooperative consumers (the before / after comparison)
 #endif
 
+static int env_switch(const char* name) {
+  const char* e = getenv(name);
+  return (e && e[0] == '0') ? 0 : 1;
+}
 static int chunk64_allowed() {
-  static int ok = -1;
-  if (ok < 0) {
-    const char* e = getenv("DASR_TC_CHUNK64");
-    ok = (e && e[0] == '0') ? 0 : 1;
-  }
+  static const int ok = env_switch("DASR_TC_CHUNK64");
   return ok;
+}
+// pair A feed: 64-channel loads where they pay (0: 32-channel loads on every pair launch, the A/B comparison)
+static int pair_feed_allowed() {
+  static const int ok = env_switch("DASR_TC_PAIR_FEED");
+  return ok;
+}
+
+// a chunk list of 64-channel runs: pairs (c, c + 32) with c % 64 == 0
+static bool chunk_list_pairs64(const DasrConvTcParams* p) {
+  if (p->nchunk_list == 0 || p->nchunk_list % 2) return false;
+  for (int i = 0; i < p->nchunk_list; i += 2)
+    if (p->chunk_off[i] % (2 * CHUNK) != 0 || p->chunk_off[i + 1] != p->chunk_off[i] + CHUNK) return false;
+  return true;
 }
 
 // pair = 1: (1, 2, 1) clusters, p->nt is the Cout tile of ONE CTA (half of the pair's tile)
@@ -1032,25 +1064,73 @@ static int conv_tc_launch(const void* in, const void* w, const float* bias, cons
   a.tiles_y = cdiv(p->H, TILE_H);
   a.ntiles = (long)p->N * a.tiles_x * a.tiles_y;
   a.w_bytes = p->ntaps * a.nchunks * p->nt * ROW_B;
-  // 64-channel A chunks: contiguous input slice whose channel count is a multiple of 64; a pair keeps 32-channel stages,
-  // whose smaller footprint leaves room for the larger filter sets it exists for
+  // single CTA: 64-channel A chunks for a contiguous input slice whose channel count is a multiple of 64 (a pair starts
+  // from 32-channel stages, whose smaller footprint leaves room for the larger filter sets it exists for; see below)
   a.chunk64 = (chunk64_allowed() && !pair && p->a_mode == 0 && p->nchunk_list == 0 && p->cin % (2 * CHUNK) == 0) ? 1 : 0;
-  a.nloads = a.chunk64 ? a.nchunks / 2 : a.nchunks;
-  a.a_stage_bytes = (int)a_stage_bytes_for(p, a.chunk64);
   a.has_pre = (p->epi_mode == 0 && pre) ? 1 : 0;
   a.has_res1 = (p->epi_mode == 0 && res1) ? 1 : 0;
   a.has_res2 = (p->epi_mode == 0 && res2) ? 1 : 0;
   a.epi_bytes = (p->epi_mode == 0) ? p->nt * 128 * 2 : (p->epi_mode == 3 ? 21504 : 0);   // mode 3: 180 halo pixels x 29 floats
   int nbuf = 2;
-  const int stages = tc_plan(a.w_bytes, a.a_stage_bytes, a.epi_bytes, a.has_res1 + a.has_res2, p->epi_mode, &nbuf);
-  a.nbuf = nbuf;
-  const int epi_total = nbuf * a.epi_bytes * (1 + a.has_res1 + a.has_res2);
+  int stages = tc_plan(a.w_bytes, (int)a_stage_bytes_for(p, a.chunk64), a.epi_bytes, a.has_res1 + a.has_res2, p->epi_mode, &nbuf);
   if (stages < 2) {
     set_error("conv_tc: resident filters (%d B) + epilogue tiles (%d B) + 2 A stages do not fit shared memory; use a smaller nt",
-              a.w_bytes, epi_total);
+              a.w_bytes, nbuf * a.epi_bytes * (1 + a.has_res1 + a.has_res2));
     return DASR_E_SMEM;
   }
+
+  typedef void (*KernelFn)(const CUtensorMap, const CUtensorMap, const EpiMaps, const TcKernelArgs);
+  static const KernelFn kernels[12] = {
+      conv_tc_kernel<0, false, 0>, conv_tc_kernel<0, false, 1>, conv_tc_kernel<0, false, 2>,
+      conv_tc_kernel<0, true, 0>,  conv_tc_kernel<0, true, 1>,  conv_tc_kernel<0, true, 2>,
+      conv_tc_kernel<1, false, 0>, conv_tc_kernel<2, false, 0>, conv_tc_kernel<3, false, 0>,
+      // weight-map variants (dasr_conv_tc_map / dasr_conv_tc2_map)
+      conv_tc_kernel<0, false, 0, DASR_MAP_CHANNEL>, conv_tc_kernel<0, false, 2, DASR_MAP_SCALE>,
+      conv_tc_kernel<0, true, 2, DASR_MAP_SCALE>};
+  int ki = (p->epi_mode == 0) ? (a.has_pre * 3 + a.has_res1 + a.has_res2) : (5 + p->epi_mode);
+  if (p->map_mode == DASR_MAP_CHANNEL) ki = 9;
+  else if (p->map_mode == DASR_MAP_SCALE) ki = 10 + a.has_pre;
+  if (p->epi_mode == 0) DASR_REQUIRE(!(a.has_res2 && !a.has_res1), "conv_tc: res2 without res1");
+  // ping-pong consumers (compile-time Cout tile) for the staged epilogue without a weight map, instantiated for the launches
+  // of the inference forward: Cout tile 16 / 32 / 64 with 9 taps (dense-block launches 2-5, LR_conv, HR_conv0, the first
+  // conv), 96 with 9 taps and no pre / residual tiles (dense-block launch 1), 64 with 4 taps (the upconv sub-pixel
+  // variants).  Two tiles are in flight per CTA, so the staging ring needs nbuf >= 2.
+#define DASR_PP_ROW(n)                                                                                                 \
+  {conv_tc_kernel<0, false, 0, 0, n>, conv_tc_kernel<0, false, 1, 0, n>, conv_tc_kernel<0, false, 2, 0, n>,            \
+   conv_tc_kernel<0, true, 0, 0, n>,  conv_tc_kernel<0, true, 1, 0, n>,  conv_tc_kernel<0, true, 2, 0, n>}
+  static const KernelFn pp_kernels[5][6] = {DASR_PP_ROW(16), DASR_PP_ROW(32), DASR_PP_ROW(64),
+                                            {conv_tc_kernel<0, false, 0, 0, 96>}, {conv_tc_kernel<0, false, 0, 0, 64, 4>}};
+#undef DASR_PP_ROW
+  int pp = -1;
+  if (p->epi_mode == 0 && p->map_mode == 0 && p->a_mode == 0 && nbuf >= 2) {
+    if (p->ntaps == 9) pp = p->nt == 16 ? 0 : p->nt == 32 ? 1 : p->nt == 64 ? 2 : p->nt == 96 ? 3 : -1;
+    else if (p->ntaps == 4 && p->nt == 64) pp = 4;
+  }
+  if (pp >= 0 && !pp_kernels[pp][ki]) pp = -1;
+#ifdef DASR_TC_TRACE
+  if (g_trace_coop) pp = -1;
+#endif
+
+  // Pair on the ping-pong consumers: 64-channel A loads (half the TMA requests per byte) for a contiguous slice of 64k
+  // channels or a chunk list of 64-channel runs, issued half-major (chunk64 = 2), so the products and their order stay
+  // those of 32-channel loads.  Only when the larger stages keep at least as many A bytes in flight and still leave two
+  // staging buffers; otherwise the launch keeps its 32-channel plan.  (Not instantiated for the Cout tile of 96: the extra
+  // copy of its MMA loop would cost that kernel spills, and dense-block launch 1 keeps more A bytes in 32-channel stages.)
+  if (pair && pair_feed_allowed() && pp >= 0 && p->ntaps == 9 && p->nt <= 64 &&
+      ((p->nchunk_list == 0 && p->cin % (2 * CHUNK) == 0) || chunk_list_pairs64(p))) {
+    int nbuf64 = 0;
+    const int stages64 = tc_plan(a.w_bytes, (int)a_stage_bytes_for(p, 1), a.epi_bytes, a.has_res1 + a.has_res2, 0, &nbuf64);
+    if (stages64 >= 2 && nbuf64 >= 2 && 2 * stages64 >= stages) {
+      a.chunk64 = 2;
+      stages = stages64;
+      nbuf = nbuf64;
+    }
+  }
+  a.nloads = a.chunk64 ? a.nchunks / 2 : a.nchunks;
+  a.a_stage_bytes = (int)a_stage_bytes_for(p, a.chunk64);
+  a.nbuf = nbuf;
   a.stages = stages;
+  const int epi_total = nbuf * a.epi_bytes * (1 + a.has_res1 + a.has_res2);
   const size_t smem = 1024 + (size_t)a.w_bytes + (size_t)stages * a.a_stage_bytes + epi_total + TC_BAR_BYTES;
 
   CUtensorMap tm_in, tm_w;
@@ -1108,37 +1188,6 @@ static int conv_tc_launch(const void* in, const void* w, const float* bias, cons
     }
   }
 
-  typedef void (*KernelFn)(const CUtensorMap, const CUtensorMap, const EpiMaps, const TcKernelArgs);
-  static const KernelFn kernels[12] = {
-      conv_tc_kernel<0, false, 0>, conv_tc_kernel<0, false, 1>, conv_tc_kernel<0, false, 2>,
-      conv_tc_kernel<0, true, 0>,  conv_tc_kernel<0, true, 1>,  conv_tc_kernel<0, true, 2>,
-      conv_tc_kernel<1, false, 0>, conv_tc_kernel<2, false, 0>, conv_tc_kernel<3, false, 0>,
-      // weight-map variants (dasr_conv_tc_map / dasr_conv_tc2_map)
-      conv_tc_kernel<0, false, 0, DASR_MAP_CHANNEL>, conv_tc_kernel<0, false, 2, DASR_MAP_SCALE>,
-      conv_tc_kernel<0, true, 2, DASR_MAP_SCALE>};
-  int ki = (p->epi_mode == 0) ? (a.has_pre * 3 + a.has_res1 + a.has_res2) : (5 + p->epi_mode);
-  if (p->map_mode == DASR_MAP_CHANNEL) ki = 9;
-  else if (p->map_mode == DASR_MAP_SCALE) ki = 10 + a.has_pre;
-  if (p->epi_mode == 0) DASR_REQUIRE(!(a.has_res2 && !a.has_res1), "conv_tc: res2 without res1");
-  // ping-pong consumers (compile-time Cout tile) for the staged epilogue without a weight map, instantiated for the launches
-  // of the inference forward: Cout tile 16 / 32 / 64 with 9 taps (dense-block launches 2-5, LR_conv, HR_conv0, the first
-  // conv), 96 with 9 taps and no pre / residual tiles (dense-block launch 1), 64 with 4 taps (the upconv sub-pixel
-  // variants).  Two tiles are in flight per CTA, so the staging ring needs nbuf >= 2.
-#define DASR_PP_ROW(n)                                                                                                 \
-  {conv_tc_kernel<0, false, 0, 0, n>, conv_tc_kernel<0, false, 1, 0, n>, conv_tc_kernel<0, false, 2, 0, n>,            \
-   conv_tc_kernel<0, true, 0, 0, n>,  conv_tc_kernel<0, true, 1, 0, n>,  conv_tc_kernel<0, true, 2, 0, n>}
-  static const KernelFn pp_kernels[5][6] = {DASR_PP_ROW(16), DASR_PP_ROW(32), DASR_PP_ROW(64),
-                                            {conv_tc_kernel<0, false, 0, 0, 96>}, {conv_tc_kernel<0, false, 0, 0, 64, 4>}};
-#undef DASR_PP_ROW
-  int pp = -1;
-  if (p->epi_mode == 0 && p->map_mode == 0 && p->a_mode == 0 && nbuf >= 2) {
-    if (p->ntaps == 9) pp = p->nt == 16 ? 0 : p->nt == 32 ? 1 : p->nt == 64 ? 2 : p->nt == 96 ? 3 : -1;
-    else if (p->ntaps == 4 && p->nt == 64) pp = 4;
-  }
-  if (pp >= 0 && !pp_kernels[pp][ki]) pp = -1;
-#ifdef DASR_TC_TRACE
-  if (g_trace_coop) pp = -1;
-#endif
   const KernelFn fn = pp >= 0 ? pp_kernels[pp][ki] : kernels[ki];
   static bool attr_set[12] = {false, false, false, false, false, false, false, false, false, false, false, false};
   static bool attr_set_pp[5][6] = {};

@@ -645,17 +645,18 @@ int main(int argc, char** argv) {
     if (!strcmp(argv[i], "check")) do_check = true;
     if (!strcmp(argv[i], "bench")) do_bench = true;
     if (!strcmp(argv[i], "tmarate")) {
+      // 180 rows: one conv halo tile (10 x 18 pixels) per box
       for (int store = 0; store <= 1; store++)
-        for (int re : {32, 64, 128, 256})
-          for (int cs : {256, 0}) {             // pitch 512 B (channel slice of a 256-channel buffer, 512 MB: HBM) | dense (L2)
-            const int rows = 128;
-            if ((long)re * 2 * rows > 49152) continue;
-            const int pitch = cs ? cs : re;
-            double c = 0;
-            int rc = dasr_probe_tma_rate(re, rows, pitch, store, &c);
-            printf("tma_%s row=%4d B rows/box=%3d pitch=%4d B : %8.1f cycles/box  %6.2f cycles/row  %6.2f B/clk/SM rc=%d\n",
-                   store ? "store" : "load ", re * 2, rows, pitch * 2, c, c / rows, re * 2.0 * rows / c, rc);
-          }
+        for (int rows : {128, 180})
+          for (int re : {32, 64, 128, 256})
+            for (int cs : {256, 0}) {           // pitch 512 B (channel slice of a 256-channel buffer, 512 MB: HBM) | dense (L2)
+              if ((long)re * 2 * rows > 49152) continue;
+              const int pitch = cs ? cs : re;
+              double c = 0;
+              int rc = dasr_probe_tma_rate(re, rows, pitch, store, &c);
+              printf("tma_%s row=%4d B rows/box=%3d pitch=%4d B : %8.1f cycles/box  %6.2f cycles/row  %6.2f B/clk/SM rc=%d\n",
+                     store ? "store" : "load ", re * 2, rows, pitch * 2, c, c / rows, re * 2.0 * rows / c, rc);
+            }
       return 0;
     }
     if (!strcmp(argv[i], "trace")) {
