@@ -35,6 +35,9 @@ constexpr int EPI_TMA_WARP = CONS_WARPS + 1;         // staged-epilogue TMA
 constexpr int TCK_THREADS = 32 * (CONS_WARPS + 2);
 constexpr int ACC_REGS = 128;                        // nt <= 256: a warpgroup's 64 x nt fp32 accumulators per thread
 constexpr int A_STAGE_ROWS = 192;                    // halo tile rows reserved per stage: the taps-in-N path reads 3 x 64
+constexpr int MAX_FRAMES = 4;                        // staged-epilogue tile frames
+constexpr int FRAME_BLKS = 2;                        // staged blocks with their own barriers per frame (ping-pong: NT <= 96)
+constexpr int EPI_BARS = MAX_FRAMES * FRAME_BLKS;    // barrier (frame f, block i) = f * FRAME_BLKS + i
 
 struct EpiMaps {          // TMA descriptors of the staged epilogue: [out, pre, res1, res2] x [64-, 32-, 16-channel box]
   CUtensorMap m[12];
@@ -60,7 +63,8 @@ struct TcKernelArgs {
   int a_stage_bytes; // bytes of one A stage
   int epi_bytes;     // bytes of ONE staged epilogue tile: 128 pixels x nt channels bf16
   int has_pre, has_res1, has_res2;
-  int nbuf;          // staged-epilogue tile buffers (2..4): pre / residual tiles are requested nbuf tiles ahead
+  int nbuf;          // staged-epilogue tile frames (1..4): pre / residual blocks are requested nbuf tiles ahead
+  int ring;          // ping-pong: each staged block is stored and its frame slots retired on their own (0: whole tiles)
   int pair;          // 1: launched as (1, 2, 1) clusters, A tiles multicast by the leader (rank 0)
   const float* map;  // weight map [N][H][W] fp32 (image stride p.map_stride), MAP != 0 only
   const float* map_w;// MAP 1: the map channel's filter taps [9][cout] fp32
@@ -241,11 +245,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
   uint64_t* full_bar = bars;                     // [stages]  A chunk landed
   uint64_t* empty_bar = bars + MAX_STAGES;       // [stages]  A chunk consumed (leader of a pair: by both CTAs)
   uint64_t* w_bar = bars + 2 * MAX_STAGES;       // [1]       resident filters landed
-  uint64_t* pre_bar = w_bar + 1;                 // [4]       pre / residual tiles landed in staging buffer b
-  uint64_t* sfull_bar = pre_bar + 4;             // [4]       staging buffer b holds a finished tile
-  uint64_t* sfree_bar = sfull_bar + 4;           // [4]       staging buffer b has been read by its TMA stores
-  uint32_t* sTap = reinterpret_cast<uint32_t*>(bars + 2 * MAX_STAGES + 16);   // [9] A byte offset of each tap
-  float* sBias = reinterpret_cast<float*>(bars + 2 * MAX_STAGES + 24);        // [nt] (16-byte aligned)
+  // staged-epilogue barriers, one per (frame, block) on the ping-pong consumers, one per frame (block 0) otherwise
+  uint64_t* pre_bar = w_bar + 1;                 // [EPI_BARS] pre / residual blocks landed
+  uint64_t* sfull_bar = pre_bar + EPI_BARS;      // [EPI_BARS] the block holds finished output
+  uint64_t* sfree_bar = sfull_bar + EPI_BARS;    // [EPI_BARS] the block has been read by its TMA store
+  uint32_t* sTap = reinterpret_cast<uint32_t*>(bars + 2 * MAX_STAGES + 2 + 3 * EPI_BARS);   // [9] A byte offset of each tap
+  float* sBias = reinterpret_cast<float*>(bars + 2 * MAX_STAGES + 8 + 3 * EPI_BARS);        // [nt] (16-byte aligned)
 
   const DasrConvTcParams& p = a.p;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -271,7 +276,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
       mbar_init(&empty_bar[s], TILE_WARPS * ((pair && rank == 0) ? 2 : 1));   // one arrive per consumer warp (of both CTAs)
     }
     mbar_init(w_bar, 1);
-    for (int b = 0; b < 4; b++) {
+    for (int b = 0; b < EPI_BARS; b++) {
       mbar_init(&pre_bar[b], 1);
       mbar_init(&sfull_bar[b], TILE_WARPS);
       mbar_init(&sfree_bar[b], 1);
@@ -340,24 +345,33 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
     __syncwarp();
   } else if (warp == EPI_TMA_WARP) {
     // =========================== epilogue TMA warp ===========================
-    // Feeds the staged epilogue: pre-activation / residual tiles in (nbuf tiles ahead), finished tiles out.
+    // Feeds the staged epilogue: pre-activation / residual blocks in (nbuf tiles ahead), finished blocks out.  A tile's
+    // frame is frame it % nbuf; its blocks go out in store units: each block on its own on the ping-pong consumers with
+    // the stage ring (a.ring), otherwise the whole tile.  Ping-pong frames have one barrier per block, so a block is
+    // stored as soon as its warpgroup has written it and its slots return (next pre / residual loads, or sfree) as soon as
+    // that store has read them; the other frames have one barrier per tile.
     if constexpr (EPI_MODE == 0) {
       const int co_base = p.out_coff + ntile * nt;
       const int omap = (p.out_mul == 2) ? 3 * var : 0;      // sub-pixel variants: one strided output map triple per parity
-      const uint32_t load_bytes = (uint32_t)(((HAS_PRE ? 1 : 0) + NRES) * a.epi_bytes);
+      const int nload = (HAS_PRE ? 1 : 0) + NRES;
+      const int unit = (NT > 0 && a.ring) ? 1 : nblocks;   // blocks per store unit
+      auto bar_of = [&](int f, int i) { return f * FRAME_BLKS + (NT > 0 ? i : 0); };
       pdl_wait();                      // pre / residual tiles and the output slots belong to earlier launches until now
-      auto issue_loads = [&](long tile, int b) {      // lane 0 issues
+      auto issue_loads = [&](long tile, int f, int i0, int i1) {      // blocks [i0, i1) of a tile into frame f; lane 0 issues
         int x0, y0, n;
         tile_xyz(tile, x0, y0, n);
         if (lane == 0) {
-          mbar_expect_tx(&pre_bar[b], load_bytes);
           const int cb = ntile * nt;
-          for (int i = 0; i < nblocks; i++) {
+          for (int i = i0; i < i1; i++) {
             int col, off, k;
             staged_block(i, nb64, tail32, col, off, k);
-            if constexpr (HAS_PRE) tma_load_4d(sS + b * a.epi_bytes + off, &em.m[3 + k], &pre_bar[b], p.pre_coff + cb + col, x0, y0, n);
-            if constexpr (NRES >= 1) tma_load_4d(sR1 + b * a.epi_bytes + off, &em.m[6 + k], &pre_bar[b], p.res1_coff + cb + col, x0, y0, n);
-            if constexpr (NRES >= 2) tma_load_4d(sR2 + b * a.epi_bytes + off, &em.m[9 + k], &pre_bar[b], p.res2_coff + cb + col, x0, y0, n);
+            uint64_t* bar = &pre_bar[bar_of(f, i)];
+            if (NT > 0) mbar_expect_tx(bar, (uint32_t)(nload * (EPI_BLK64_BYTES >> k)));
+            else if (i == 0) mbar_expect_tx(bar, (uint32_t)(nload * a.epi_bytes));
+            off += f * a.epi_bytes;
+            if constexpr (HAS_PRE) tma_load_4d(sS + off, &em.m[3 + k], bar, p.pre_coff + cb + col, x0, y0, n);
+            if constexpr (NRES >= 1) tma_load_4d(sR1 + off, &em.m[6 + k], bar, p.res1_coff + cb + col, x0, y0, n);
+            if constexpr (NRES >= 2) tma_load_4d(sR2 + off, &em.m[9 + k], bar, p.res2_coff + cb + col, x0, y0, n);
           }
         }
         __syncwarp();
@@ -365,54 +379,62 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
       const long G = gridDim.x;
       if (has_loads) {
         for (int k = 0; k < nbuf; k++)
-          if ((long)blockIdx.x + k * G < a.ntiles) issue_loads(blockIdx.x + k * G, k);
+          if ((long)blockIdx.x + k * G < a.ntiles) issue_loads(blockIdx.x + k * G, k, 0, nblocks);
       }
-      // The store of tile i is retired (its staging buffer handed back: next pre/residual loads, or sfree) only after
-      // the store of tile i+1 has been issued: `wait_group.read 1` then covers tile i while tile i+1 is still being read.
+      // The store of a unit is retired (its blocks handed back) only after the store of the next unit has been issued:
+      // `wait_group.read 1` then covers the earlier unit while the later one is still being read.
       uint32_t it = 0;
       long prev_tile = -1;
-      int prev_b = 0;
-      auto retire = [&](long t, int bb) {           // whole warp
+      int prev_f = 0, prev_i0 = 0, prev_i1 = 0;
+      auto retire = [&](long t, int f, int i0, int i1) {           // whole warp
         if (has_loads) {
-          if (t + (long)nbuf * G < a.ntiles) issue_loads(t + (long)nbuf * G, bb);
+          if (t + (long)nbuf * G < a.ntiles) issue_loads(t + (long)nbuf * G, f, i0, i1);
         } else if (lane == 0) {
-          mbar_arrive(&sfree_bar[bb]);
+          for (int i = i0; i < i1; i++)
+            if (NT > 0 || i == 0) mbar_arrive(&sfree_bar[bar_of(f, i)]);
         }
         __syncwarp();
       };
       for (long tile = blockIdx.x; tile < a.ntiles; tile += G, it++) {
-        const int b = (int)(it % (uint32_t)nbuf);
-        if (lane == 0) {
-          int x0, y0, n;
-          tile_xyz(tile, x0, y0, n);
-          mbar_wait(&sfull_bar[b], (it / (uint32_t)nbuf) & 1);
-          TC_STAMP(it, TEV_E_SFULL);
-          for (int i = 0; i < nblocks; i++) {
-            int col, off, k;
-            staged_block(i, nb64, tail32, col, off, k);
-            tma_store_4d(&em.m[k + omap], sS + b * a.epi_bytes + off, co_base + col, x0, y0, n);
-          }
-          bulk_commit();
-          TC_STAMP(it, TEV_E_STORED);
-          if (prev_tile >= 0) {
-            asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");   // the previous tile's stores have read their buffer
-            TC_STAMP(it - 1, TEV_E_READ);
-          }
-        }
-        __syncwarp();
-        if (prev_tile >= 0) retire(prev_tile, prev_b);
-        prev_tile = tile;
-        prev_b = b;
-        if (nbuf == 1) {
-          // one staging buffer: the next tile's epilogue needs this buffer back (its pre / residual loads or sfree), so
-          // the retire cannot wait for the next tile's stores — that wait would never end
+        const int f = (int)(it % (uint32_t)nbuf);
+        const uint32_t fphase = (it / (uint32_t)nbuf) & 1;
+        for (int i0 = 0; i0 < nblocks; i0 += unit) {
+          const int i1 = min(i0 + unit, nblocks);
           if (lane == 0) {
-            bulk_wait_read0();
-            TC_STAMP(it, TEV_E_READ);
+            int x0, y0, n;
+            tile_xyz(tile, x0, y0, n);
+            for (int i = i0; i < i1; i++)
+              if (NT > 0 || i == 0) mbar_wait(&sfull_bar[bar_of(f, i)], fphase);
+            if (i0 == 0) TC_STAMP(it, TEV_E_SFULL);
+            for (int i = i0; i < i1; i++) {
+              int col, off, k;
+              staged_block(i, nb64, tail32, col, off, k);
+              tma_store_4d(&em.m[k + omap], sS + f * a.epi_bytes + off, co_base + col, x0, y0, n);
+            }
+            bulk_commit();
+            if (i1 == nblocks) TC_STAMP(it, TEV_E_STORED);
+            if (prev_tile >= 0) {
+              asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");   // the previous unit's stores have read it
+              if (prev_i1 == nblocks) TC_STAMP(it - 1, TEV_E_READ);     // the previous tile's last unit
+            }
           }
           __syncwarp();
-          retire(tile, b);
-          prev_tile = -1;
+          if (prev_tile >= 0) retire(prev_tile, prev_f, prev_i0, prev_i1);
+          prev_tile = tile;
+          prev_f = f;
+          prev_i0 = i0;
+          prev_i1 = i1;
+          if (nbuf == 1) {
+            // one frame (cooperative consumers only): the next tile's epilogue needs this frame back (its pre / residual
+            // loads or sfree), so the retire cannot wait for the next tile's stores — that wait would never end
+            if (lane == 0) {
+              bulk_wait_read0();
+              TC_STAMP(it, TEV_E_READ);
+            }
+            __syncwarp();
+            retire(tile, f, i0, i1);
+            prev_tile = -1;
+          }
         }
       }
       if (prev_tile >= 0) {
@@ -421,7 +443,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
           TC_STAMP(it - 1, TEV_E_READ);
         }
         __syncwarp();
-        retire(prev_tile, prev_b);
+        retire(prev_tile, prev_f, prev_i0, prev_i1);
       }
       if (lane == 0) bulk_wait0();                 // all stores complete before the CTA (and its smem) goes away
     }
@@ -546,6 +568,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
       // of each A stage has then completed, so a parity wait can never be satisfied by a phase two rounds old.
       constexpr int NB64 = NT / 64;
       constexpr bool T32 = (NT & 32) != 0;
+      constexpr int NBLK = NB64 + (T32 ? 1 : 0) + ((NT & 16) ? 1 : 0);
+      static_assert(NBLK <= FRAME_BLKS, "ping-pong: one barrier per staged block");
       const uint32_t G = gridDim.x, ntiles = (uint32_t)a.ntiles;   // 32-bit tile arithmetic (checked on the host)
       const uint32_t nl = (uint32_t)a.nloads, ns = (uint32_t)a.stages;
       const uint32_t blk_off = 8u * HALO_W * a_row;
@@ -583,27 +607,37 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
           const int sb = (int)(it % (uint32_t)nbuf);
           const uint32_t sphase = (it / (uint32_t)nbuf) & 1;
           const uint32_t bS = sS_u + sb * a.epi_bytes, bR1 = sR1_u + sb * a.epi_bytes, bR2 = sR2_u + sb * a.epi_bytes;
-          if (has_loads) mbar_wait(&pre_bar[sb], sphase);
-          else if (it >= (uint32_t)nbuf) mbar_wait(&sfree_bar[sb], sphase ^ 1);
-          if (rec) TC_STAMP(it, 5 * wg + 3);
+          // one staged block at a time (64-channel blocks, then the 32- / 16-channel tail): wait for its slots, write it,
+          // hand it to the epilogue TMA warp, which can store it while the next block is written
+          auto epi_block = [&](auto i_c) {
+            constexpr int i = decltype(i_c)::value, TAIL0 = NB64 * 64;
+            constexpr int c0 = i < NB64 ? 64 * i : (T32 && i == NB64 ? TAIL0 : TAIL0 + (T32 ? 32 : 0));
+            constexpr int c1 = i < NB64 ? c0 + 64 : (T32 && i == NB64 ? c0 + 32 : c0 + 16);
+            const int bi = sb * FRAME_BLKS + i;
+            if (has_loads) mbar_wait(&pre_bar[bi], sphase);
+            else if (it >= (uint32_t)nbuf) mbar_wait(&sfree_bar[bi], sphase ^ 1);
+            if (rec && i == 0) TC_STAMP(it, 5 * wg + 3);
 #pragma unroll
-          for (int blk = 0; blk < 2; blk++) {
+            for (int blk = 0; blk < 2; blk++) {
 #pragma unroll
-            for (int h = 0; h < 2; h++) {
-              const int m = 64 * blk + r0 + 8 * h;
+              for (int h = 0; h < 2; h++) {
+                const int m = 64 * blk + r0 + 8 * h;
 #pragma unroll
-              for (int j = 0; j < NT / 8; j++) {
-                const int cl = 8 * j + cq;
-                float v0 = acc[blk * (NT / 2) + 4 * j + 2 * h], v1 = acc[blk * (NT / 2) + 4 * j + 2 * h + 1];
-                if (has_bias) { v0 += sBias[cl]; v1 += sBias[cl + 1]; }
-                staged_epi_pair<HAS_PRE, NRES, 0>(v0, v1, co_base + cl, staged_off(m, cl, NB64, T32), bS, bR1, bR2, nullptr, p,
-                                                  nullptr, mask_mode, F16);
+                for (int j = c0 / 8; j < c1 / 8; j++) {
+                  const int cl = 8 * j + cq;
+                  float v0 = acc[blk * (NT / 2) + 4 * j + 2 * h], v1 = acc[blk * (NT / 2) + 4 * j + 2 * h + 1];
+                  if (has_bias) { v0 += sBias[cl]; v1 += sBias[cl + 1]; }
+                  staged_epi_pair<HAS_PRE, NRES, 0>(v0, v1, co_base + cl, staged_off(m, cl, NB64, T32), bS, bR1, bR2, nullptr,
+                                                    p, nullptr, mask_mode, F16);
+                }
               }
             }
-          }
-          fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&sfull_bar[sb]);
+            fence_proxy_async();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&sfull_bar[bi]);
+          };
+          epi_block(std::integral_constant<int, 0>());
+          if constexpr (NBLK > 1) epi_block(std::integral_constant<int, 1>());
           if (rec) TC_STAMP(it, 5 * wg + 4);
         }
       };
@@ -614,7 +648,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
       using I4 = std::integral_constant<int, 4>;
       using B0 = std::false_type;
       if (a.chunk64 == 2) {
-        if constexpr (NTAPS == 9 && NT <= 64) {   // pair launches (plain 3x3 geometry) with Cout tiles up to 64 per CTA
+        if constexpr (NTAPS == 9) {               // pair launches (plain 3x3 geometry)
           if (f16) run(I4(), I1(), std::true_type());
           else run(I4(), I0(), std::true_type());
         }
@@ -661,8 +695,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
         const uint32_t sphase = (it / (uint32_t)nbuf) & 1;
         const uint32_t bS = sS_u + sb * a.epi_bytes, bR1 = sR1_u + sb * a.epi_bytes, bR2 = sR2_u + sb * a.epi_bytes;
         if constexpr (EPI_MODE == 0) {
-          if (has_loads) mbar_wait(&pre_bar[sb], sphase);                      // pre / residual tiles of this tile landed
-          else if (it >= (uint32_t)nbuf) mbar_wait(&sfree_bar[sb], sphase ^ 1); // stores of tile it-nbuf have read the buffer
+          const int bi = sb * FRAME_BLKS;                                       // the frame's one barrier
+          if (has_loads) mbar_wait(&pre_bar[bi], sphase);                       // pre / residual tiles of this tile landed
+          else if (it >= (uint32_t)nbuf) mbar_wait(&sfree_bar[bi], sphase ^ 1); // stores of tile it-nbuf have read the frame
           if (rec) TC_STAMP(it, 5 * wg + 3);
         }
 #pragma unroll
@@ -732,7 +767,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
         if constexpr (EPI_MODE == 0) {
           fence_proxy_async();          // generic-proxy writes of the staged tile -> visible to the TMA engine
           __syncwarp();
-          if (lane == 0) mbar_arrive(&sfull_bar[sb]);
+          if (lane == 0) mbar_arrive(&sfull_bar[sb * FRAME_BLKS]);
           if (rec) TC_STAMP(it, 5 * wg + 4);
         }
       }
@@ -993,7 +1028,7 @@ static int encode_staged_maps(PFN_encodeTiled enc, CUtensorMap* m, const void* b
 static size_t a_stage_bytes_for(const DasrConvTcParams* p, int chunk64) {
   return (p->a_mode == 0) ? (size_t)(chunk64 ? 2 : 1) * A_STAGE_ROWS * ROW_B : (size_t)p->ntaps * A_TAP_BYTES;
 }
-static const int TC_BAR_BYTES = (2 * MAX_STAGES + 24) * 8 + 256 * 4 + 16;
+static const int TC_BAR_BYTES = (2 * MAX_STAGES + 8 + 3 * EPI_BARS) * 8 + 256 * 4 + 16;
 
 // Shared-memory plan: staged-epilogue buffers as many (<= 4) as still leave 4 A stages — loads of pre / residual tiles
 // are issued nbuf tiles ahead, which hides their latency — then as many A stages as fit (<= MAX_STAGES).  One buffer
@@ -1027,6 +1062,11 @@ static int chunk64_allowed() {
 // pair A feed: 64-channel loads where they pay (0: 32-channel loads on every pair launch, the A/B comparison)
 static int pair_feed_allowed() {
   static const int ok = env_switch("DASR_TC_PAIR_FEED");
+  return ok;
+}
+// ping-pong staged epilogue stored and retired block by block (0: whole tiles and the whole-tile A plan, the A/B comparison)
+static int stage_ring_allowed() {
+  static const int ok = env_switch("DASR_TC_STAGE_RING");
   return ok;
 }
 
@@ -1111,16 +1151,20 @@ static int conv_tc_launch(const void* in, const void* w, const float* bias, cons
   if (g_trace_coop) pp = -1;
 #endif
 
+  a.ring = (pp >= 0 && stage_ring_allowed()) ? 1 : 0;
+
   // Pair on the ping-pong consumers: 64-channel A loads (half the TMA requests per byte) for a contiguous slice of 64k
   // channels or a chunk list of 64-channel runs, issued half-major (chunk64 = 2), so the products and their order stay
-  // those of 32-channel loads.  Only when the larger stages keep at least as many A bytes in flight and still leave two
-  // staging buffers; otherwise the launch keeps its 32-channel plan.  (Not instantiated for the Cout tile of 96: the extra
-  // copy of its MMA loop would cost that kernel spills, and dense-block launch 1 keeps more A bytes in 32-channel stages.)
-  if (pair && pair_feed_allowed() && pp >= 0 && p->ntaps == 9 && p->nt <= 64 &&
+  // those of 32-channel loads.  Only when the wider stages still leave two staging frames and hold the A loads of two
+  // tiles, one per consumer warpgroup; otherwise the launch keeps its 32-channel plan.  With whole-tile staging
+  // (a.ring = 0) the wide stages must also keep at least as many A bytes in flight as the narrow ones, and the Cout
+  // tile of 96 (dense-block launch 1: 2 wide stages against 5 narrow ones) stays on 32-channel loads.
+  if (pair && pair_feed_allowed() && pp >= 0 && p->ntaps == 9 && (a.ring || p->nt <= 64) &&
       ((p->nchunk_list == 0 && p->cin % (2 * CHUNK) == 0) || chunk_list_pairs64(p))) {
     int nbuf64 = 0;
     const int stages64 = tc_plan(a.w_bytes, (int)a_stage_bytes_for(p, 1), a.epi_bytes, a.has_res1 + a.has_res2, 0, &nbuf64);
-    if (stages64 >= 2 && nbuf64 >= 2 && 2 * stages64 >= stages) {
+    const bool enough = a.ring ? stages64 >= 2 * (a.nchunks / 2) : 2 * stages64 >= stages;
+    if (stages64 >= 2 && nbuf64 >= 2 && enough) {
       a.chunk64 = 2;
       stages = stages64;
       nbuf = nbuf64;
