@@ -725,6 +725,11 @@ static int run_loss(const float* a, const float* b, const float* w, float* loss,
 
 using namespace dasr;
 
+// a channel slice [coff, coff + C) of rows of cs channels
+static inline bool slice_ok(int C, int cs, int coff) { return coff >= 0 && coff + C <= cs; }
+// base address on an n-byte boundary (the vector loads / stores of the bf16x8, float4 and float2 kernels)
+static inline bool aligned(const void* p, uintptr_t n) { return (reinterpret_cast<uintptr_t>(p) & (n - 1)) == 0; }
+
 // launch with the programmatic-stream-serialization attribute (DASR_B200_PDL=0: plain launch semantics)
 template <typename... KArgs, typename... Args>
 static void launch_pdl(void (*kernel)(KArgs...), long grid, int block, cudaStream_t st, Args... args) {
@@ -745,7 +750,8 @@ extern "C" {
 
 int dasr_nchw_to_nhwc(const float* src, void* dst, int N, int C, int H, int W, int dst_cs, int dst_coff,
                       int dst_is_bf16, const float* mean, const float* stdv, void* stream) {
-  DASR_REQUIRE(N > 0 && C > 0 && H > 0 && W > 0 && dst_cs >= dst_coff + C, "nchw_to_nhwc: bad dims");
+  DASR_REQUIRE(N > 0 && C > 0 && H > 0 && W > 0 && slice_ok(C, dst_cs, dst_coff), "nchw_to_nhwc: bad dims");
+  DASR_REQUIRE(dst_is_bf16 >= 0 && dst_is_bf16 <= 2, "nchw_to_nhwc: dtype code %d (0 fp32, 1 bf16, 2 half)", dst_is_bf16);
   long HW = (long)H * W;
   dim3 grid(cdiv(HW, 32), cdiv(C, 32), N), block(32, 8);
   if (dst_is_bf16 == 2)
@@ -761,7 +767,8 @@ int dasr_nchw_to_nhwc(const float* src, void* dst, int N, int C, int H, int W, i
 
 int dasr_nhwc_to_nchw(const void* src, float* dst, int N, int C, int H, int W, int src_cs, int src_coff,
                       int src_is_bf16, const float* inv_std, void* stream) {
-  DASR_REQUIRE(N > 0 && C > 0 && H > 0 && W > 0 && src_cs >= src_coff + C, "nhwc_to_nchw: bad dims");
+  DASR_REQUIRE(N > 0 && C > 0 && H > 0 && W > 0 && slice_ok(C, src_cs, src_coff), "nhwc_to_nchw: bad dims");
+  DASR_REQUIRE(src_is_bf16 == 0 || src_is_bf16 == 1, "nhwc_to_nchw: dtype code %d (0 fp32, 1 bf16)", src_is_bf16);
   long HW = (long)H * W;
   dim3 grid(cdiv(HW, 32), cdiv(C, 32), N), block(32, 8);
   if (src_is_bf16)
@@ -775,7 +782,8 @@ int dasr_nhwc_to_nchw(const void* src, float* dst, int N, int C, int H, int W, i
 
 int dasr_act_bwd(void* g, const void* y, long npix, int C, int g_cs, int g_coff, int y_cs, int y_coff, float slope,
                  int is_bf16, void* stream) {
-  DASR_REQUIRE(npix > 0 && C > 0, "act_bwd: bad dims");
+  DASR_REQUIRE(npix > 0 && C > 0 && g && y && slice_ok(C, g_cs, g_coff) && slice_ok(C, y_cs, y_coff), "act_bwd: bad dims");
+  DASR_REQUIRE(is_bf16 == 0 || is_bf16 == 1, "act_bwd: dtype code %d (0 fp32, 1 bf16)", is_bf16);
   long total = npix * C;
   if (is_bf16 && C % 8 == 0 && g_cs % 8 == 0 && g_coff % 8 == 0 && y_cs % 8 == 0 && y_coff % 8 == 0 &&
       (reinterpret_cast<uintptr_t>(g) & 15) == 0 && (reinterpret_cast<uintptr_t>(y) & 15) == 0)
@@ -792,7 +800,9 @@ int dasr_act_bwd(void* g, const void* y, long npix, int C, int g_cs, int g_coff,
 
 int dasr_upsample2x_bwd(const void* src, void* dst, int N, int H, int W, int C, int src_cs, int src_coff, int dst_cs,
                         int dst_coff, int is_bf16, void* stream) {
-  DASR_REQUIRE(N > 0 && H > 0 && W > 0 && C > 0, "upsample2x_bwd: bad dims");
+  DASR_REQUIRE(N > 0 && H > 0 && W > 0 && C > 0 && src && dst && slice_ok(C, src_cs, src_coff) && slice_ok(C, dst_cs, dst_coff),
+               "upsample2x_bwd: bad dims");
+  DASR_REQUIRE(is_bf16 == 0 || is_bf16 == 1, "upsample2x_bwd: dtype code %d (0 fp32, 1 bf16)", is_bf16);
   long total = (long)N * H * W * C;
   if (is_bf16)
     upsample2x_bwd_kernel<__nv_bfloat16><<<cdiv(total, 256), 256, 0, (cudaStream_t)stream>>>(
@@ -805,7 +815,9 @@ int dasr_upsample2x_bwd(const void* src, void* dst, int N, int H, int W, int C, 
 
 int dasr_upsample2x_fwd(const void* src, void* dst, int N, int H, int W, int C, int src_cs, int src_coff, int dst_cs,
                         int dst_coff, int is_bf16, void* stream) {
-  DASR_REQUIRE(N > 0 && H > 0 && W > 0 && C > 0, "upsample2x_fwd: bad dims");
+  DASR_REQUIRE(N > 0 && H > 0 && W > 0 && C > 0 && src && dst && slice_ok(C, src_cs, src_coff) && slice_ok(C, dst_cs, dst_coff),
+               "upsample2x_fwd: bad dims");
+  DASR_REQUIRE(is_bf16 == 0 || is_bf16 == 1, "upsample2x_fwd: dtype code %d (0 fp32, 1 bf16)", is_bf16);
   long total = (long)N * 4 * H * W * C;
   if (is_bf16)
     upsample2x_fwd_kernel<__nv_bfloat16><<<cdiv(total, 256), 256, 0, (cudaStream_t)stream>>>(
@@ -818,7 +830,9 @@ int dasr_upsample2x_fwd(const void* src, void* dst, int N, int H, int W, int C, 
 
 int dasr_axpby(const void* x, const void* y, void* dst, long npix, int C, int x_cs, int x_coff, int y_cs, int y_coff,
                int d_cs, int d_coff, float a, float b, int is_bf16, void* stream) {
-  DASR_REQUIRE(npix > 0 && C > 0 && x && dst, "axpby: bad arguments");
+  DASR_REQUIRE(npix > 0 && C > 0 && x && dst && slice_ok(C, x_cs, x_coff) && slice_ok(C, d_cs, d_coff) &&
+                   (!y || slice_ok(C, y_cs, y_coff)), "axpby: bad arguments");
+  DASR_REQUIRE(is_bf16 >= 0 && is_bf16 <= 2, "axpby: dtype code %d (0 fp32, 1 bf16, 2 half)", is_bf16);
   long total = npix * C;
   if (is_bf16 == 2) {
     axpby_kernel<__half><<<cdiv(total, 256), 256, 0, (cudaStream_t)stream>>>(
@@ -843,7 +857,8 @@ int dasr_axpby(const void* x, const void* y, void* dst, long npix, int C, int x_
 
 int dasr_map_axpby(const float* x, const float* map, const float* y, float* dst, long npix, int C, int x_cs, int x_coff,
                    int y_cs, int y_coff, int d_cs, int d_coff, float a, float b, void* stream) {
-  DASR_REQUIRE(npix > 0 && C > 0 && map && dst && d_coff + C <= d_cs && (!x || x_coff + C <= x_cs) && (!y || y_coff + C <= y_cs),
+  DASR_REQUIRE(npix > 0 && C > 0 && map && dst && slice_ok(C, d_cs, d_coff) && (!x || slice_ok(C, x_cs, x_coff)) &&
+                   (!y || slice_ok(C, y_cs, y_coff)),
                "map_axpby: bad arguments");
   const long total = npix * C;
   map_axpby_kernel<<<cdiv(total, 256), 256, 0, (cudaStream_t)stream>>>(x, map, y, dst, npix, C, x_cs, x_coff, y_cs, y_coff,
@@ -894,6 +909,7 @@ int dasr_maxpool2_bwd(const float* in, const float* out, const float* dout, floa
 }
 int dasr_maxpool2_fwd_bf16(const void* in, void* out, int N, int H, int W, int C, void* stream) {
   DASR_REQUIRE(N > 0 && H >= 2 && W >= 2 && C > 0 && H % 2 == 0 && W % 2 == 0 && C % 8 == 0, "maxpool2_bf16: H,W even, C%%8==0");
+  DASR_REQUIRE(aligned(in, 16) && aligned(out, 16), "maxpool2_fwd_bf16: operands must be 16-byte aligned (uint4 vectors)");
   long total = (long)N * (H / 2) * (W / 2) * (C / 8);
   maxpool2_fwd_bf16_kernel<<<cdiv(total, 256), 256, 0, (cudaStream_t)stream>>>((const uint4*)in, (uint4*)out, N, H, W, C / 8);
   return check_launch("maxpool2_fwd_bf16");
@@ -901,6 +917,8 @@ int dasr_maxpool2_fwd_bf16(const void* in, void* out, int N, int H, int W, int C
 int dasr_maxpool2_bwd_bf16(const void* in, const void* out, const void* dout, void* din, int N, int H, int W, int C,
                            void* stream) {
   DASR_REQUIRE(N > 0 && H >= 2 && W >= 2 && C > 0 && H % 2 == 0 && W % 2 == 0 && C % 8 == 0, "maxpool2_bf16: H,W even, C%%8==0");
+  DASR_REQUIRE(aligned(in, 16) && aligned(out, 16) && aligned(dout, 16) && aligned(din, 16),
+               "maxpool2_bwd_bf16: operands must be 16-byte aligned (uint4 vectors)");
   long total = (long)N * (H / 2) * (W / 2) * (C / 8);
   maxpool2_bwd_bf16_kernel<<<cdiv(total, 256), 256, 0, (cudaStream_t)stream>>>((const uint4*)in, (const uint4*)out,
                                                                               (const uint4*)dout, (uint4*)din, N, H, W, C / 8);
@@ -925,6 +943,7 @@ int dasr_instnorm_lrelu_bwd(const float* y, const float* stats, const float* dy,
 int dasr_haar_fwd(const float* x, float* ll, float* hc, int N, int C, int H, int W, int norm, void* stream) {
   DASR_REQUIRE(N > 0 && C > 0 && H > 0 && W > 0, "haar: bad dims");
   DASR_REQUIRE(H % 2 == 0 && W % 2 == 0, "haar: odd H or W (%dx%d) would need mode='reflect' padding; unsupported", H, W);
+  DASR_REQUIRE(x && aligned(x, 8), "haar_fwd: x must be 8-byte aligned (float2 loads)");
   long total = (long)N * C * (H / 2) * (W / 2);
   haar_fwd_kernel<<<cdiv(total, 256), 256, 0, (cudaStream_t)stream>>>(x, ll, hc, N, C, H, W, norm ? 0.5f : 1.f,
                                                                        norm ? 0.5f : 0.f);
@@ -932,6 +951,7 @@ int dasr_haar_fwd(const float* x, float* ll, float* hc, int N, int C, int H, int
 }
 int dasr_haar_bwd(const float* dll, const float* dhc, float* dx, int N, int C, int H, int W, int norm, void* stream) {
   DASR_REQUIRE(N > 0 && C > 0 && H > 0 && W > 0 && H % 2 == 0 && W % 2 == 0, "haar bwd: bad dims");
+  DASR_REQUIRE(dx && aligned(dx, 8), "haar_bwd: dx must be 8-byte aligned (float2 stores)");
   long total = (long)N * C * (H / 2) * (W / 2);
   haar_bwd_kernel<<<cdiv(total, 256), 256, 0, (cudaStream_t)stream>>>(dll, dhc, dx, N, C, H, W, norm ? 0.5f : 1.f);
   return check_launch("haar_bwd");
@@ -997,6 +1017,7 @@ int dasr_prelu_bwd(const float* z, const float* dy, const float* slope, float* d
 }
 int dasr_prelu_fwd_bf16(const void* z, const float* slope, void* y, long n, void* stream) {
   DASR_REQUIRE(z && slope && y && n > 0 && n % 8 == 0, "prelu_fwd_bf16: n must be a multiple of 8");
+  DASR_REQUIRE(aligned(z, 16) && aligned(y, 16), "prelu_fwd_bf16: z and y must be 16-byte aligned (uint4 vectors)");
   long n8 = n / 8;
   int blocks = (int)((n8 + 255) / 256);
   if (blocks > 8 * num_sms()) blocks = 8 * num_sms();
@@ -1006,6 +1027,7 @@ int dasr_prelu_fwd_bf16(const void* z, const float* slope, void* y, long n, void
 int dasr_prelu_bwd_bf16(const void* z, const void* dy, const float* slope, void* dz, float* dslope, int accumulate, long n,
                         float* partials, void* stream) {
   DASR_REQUIRE(z && dy && slope && dz && dslope && partials && n > 0 && n % 8 == 0, "prelu_bwd_bf16: bad arguments");
+  DASR_REQUIRE(aligned(z, 16) && aligned(dy, 16) && aligned(dz, 16), "prelu_bwd_bf16: z, dy, dz must be 16-byte aligned (uint4 vectors)");
   long n8 = n / 8;
   int blocks = (int)((n8 + RED_THREADS - 1) / RED_THREADS);
   if (blocks > RED_BLOCKS) blocks = RED_BLOCKS;
@@ -1016,6 +1038,7 @@ int dasr_prelu_bwd_bf16(const void* z, const void* dy, const float* slope, void*
 }
 int dasr_cast_bf16_f32(const void* src, void* dst, long n, int to_bf16, void* stream) {
   DASR_REQUIRE(src && dst && n > 0 && n % 8 == 0, "cast: n must be a multiple of 8");
+  DASR_REQUIRE(aligned(src, 16) && aligned(dst, 16), "cast: src and dst must be 16-byte aligned (float4 / uint4 vectors)");
   long n8 = n / 8;
   int blocks = (int)((n8 + 255) / 256);
   if (blocks > 8 * num_sms()) blocks = 8 * num_sms();

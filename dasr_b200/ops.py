@@ -221,6 +221,7 @@ def bias_grad(dy, db, accumulate=False):
 
 def upsample2x_fwd(src, dst):
     src, dst = as_view(src), as_view(dst)
+    _check_up2('upsample2x_fwd', src, dst)
     N, H, W, _ = src.t.shape
     check(_lib.load().dasr_upsample2x_fwd(src.ptr, dst.ptr, N, H, W, dst.c, src.cs, src.coff, dst.cs, dst.coff,
                                           int(dst.t.dtype == torch.bfloat16), _stream()), 'upsample2x_fwd')
@@ -431,9 +432,45 @@ def _conv_tc_nchw(inp, w_packed, bias, nchw_out, cout, act, slope, alpha, a_mode
 # layout / elementwise
 # --------------------------------------------------------------------------------------------------
 
+_F32_BF16 = (torch.float32, torch.bfloat16)
+_F32_BF16_F16 = (torch.float32, torch.bfloat16, torch.float16)
+
+
+def _check_slices(what, ref, others, dtypes):
+    """Channel-slice operands of an elementwise kernel: `ref` in one of `dtypes`, every other View over the same pixels
+    (numel / channel stride), in the same dtype and at least as wide as `ref`."""
+    if ref.t.dtype not in dtypes:
+        raise _lib.DasrError('%s: no kernel reads %s (supported: %s)' % (what, ref.t.dtype, ', '.join(map(str, dtypes))))
+    npix = ref.t.numel() // ref.cs
+    for name, v in others:
+        if v.t.dtype != ref.t.dtype:
+            raise _lib.DasrError('%s: %s is %s, the launch is %s' % (what, name, v.t.dtype, ref.t.dtype))
+        if v.t.numel() // v.cs != npix:
+            raise _lib.DasrError('%s: %s has %d pixels, the launch has %d' % (what, name, v.t.numel() // v.cs, npix))
+        if v.c < ref.c:
+            raise _lib.DasrError('%s: %s slice has %d channels, the launch needs %d' % (what, name, v.c, ref.c))
+    return npix
+
+
+def _check_up2(what, lo, hi):
+    """upsample2x: `hi` is [N, 2H, 2W] of `lo`, both NHWC of the same dtype (fp32 or bf16), equal channel counts"""
+    if lo.t.dtype not in _F32_BF16 or hi.t.dtype != lo.t.dtype:
+        raise _lib.DasrError('%s: operands are %s / %s, the kernels read fp32 or bf16 pairs' % (what, lo.t.dtype, hi.t.dtype))
+    if lo.t.dim() != 4 or hi.t.dim() != 4:
+        raise _lib.DasrError('%s: operands must be NHWC [N, H, W, C] tensors' % what)
+    N, H, W, _ = lo.t.shape
+    if tuple(hi.t.shape[:3]) != (N, 2 * H, 2 * W) or hi.c != lo.c:
+        raise _lib.DasrError('%s: %s (%d channels) is not the 2x upsample of %s (%d channels)' % (
+            what, tuple(hi.t.shape), hi.c, tuple(lo.t.shape), lo.c))
+
+
 def nchw_to_nhwc(src, dst, mean=None, std=None):
     dst = as_view(dst)
     N, Cc, H, W = src.shape
+    if src.dtype != torch.float32 or dst.t.dtype not in _F32_BF16_F16:
+        raise _lib.DasrError('nchw_to_nhwc: fp32 source, fp32 / bf16 / half destination (got %s -> %s)' % (src.dtype, dst.t.dtype))
+    if dst.t.numel() // dst.cs != N * H * W or dst.c != Cc:
+        raise _lib.DasrError('nchw_to_nhwc: %s slice of %d channels cannot hold %s' % (tuple(dst.t.shape), dst.c, tuple(src.shape)))
     check(_lib.load().dasr_nchw_to_nhwc(_p(src), dst.ptr, N, Cc, H, W, dst.cs, dst.coff,
                                         _dt16(dst.t), _p(mean), _p(std), _stream()), 'nchw_to_nhwc')
 
@@ -441,19 +478,24 @@ def nchw_to_nhwc(src, dst, mean=None, std=None):
 def nhwc_to_nchw(src, dst, inv_std=None):
     src = as_view(src)
     N, Cc, H, W = dst.shape
+    if src.t.dtype not in _F32_BF16 or dst.dtype != torch.float32:
+        raise _lib.DasrError('nhwc_to_nchw: fp32 / bf16 source, fp32 destination (got %s -> %s)' % (src.t.dtype, dst.dtype))
+    if src.t.numel() // src.cs != N * H * W or src.c < Cc:
+        raise _lib.DasrError('nhwc_to_nchw: %s slice of %d channels cannot fill %s' % (tuple(src.t.shape), src.c, tuple(dst.shape)))
     check(_lib.load().dasr_nhwc_to_nchw(src.ptr, _p(dst), N, Cc, H, W, src.cs, src.coff,
                                         int(src.t.dtype == torch.bfloat16), _p(inv_std), _stream()), 'nhwc_to_nchw')
 
 
 def act_bwd(g, y, slope):
     g, y = as_view(g), as_view(y)
-    npix = g.t.numel() // g.cs
+    npix = _check_slices('act_bwd', g, (('y', y),), _F32_BF16)
     check(_lib.load().dasr_act_bwd(g.ptr, y.ptr, npix, g.c, g.cs, g.coff, y.cs, y.coff, slope,
                                    int(g.t.dtype == torch.bfloat16), _stream()), 'act_bwd')
 
 
 def upsample2x_bwd(src, dst):
     src, dst = as_view(src), as_view(dst)
+    _check_up2('upsample2x_bwd', dst, src)
     N, H, W, _ = dst.t.shape
     check(_lib.load().dasr_upsample2x_bwd(src.ptr, dst.ptr, N, H, W, dst.c, src.cs, src.coff, dst.cs, dst.coff,
                                           int(dst.t.dtype == torch.bfloat16), _stream()), 'upsample2x_bwd')
@@ -463,7 +505,7 @@ def axpby(x, a, y, b, dst):
     """dst = a*x + b*y on channel slices (y may be None)."""
     x, dst = as_view(x), as_view(dst)
     y = as_view(y) if y is not None else None
-    npix = dst.t.numel() // dst.cs
+    npix = _check_slices('axpby', dst, (('x', x),) + ((('y', y),) if y else ()), _F32_BF16_F16)
     check(_lib.load().dasr_axpby(x.ptr, y.ptr if y else None, dst.ptr, npix, dst.c, x.cs, x.coff,
                                  y.cs if y else 0, y.coff if y else 0, dst.cs, dst.coff, a, b,
                                  _dt16(dst.t), _stream()), 'axpby')
@@ -482,7 +524,24 @@ def map_axpby(x, amap, a, y, b, dst):
                                      dst.cs, dst.coff, a, b, _stream()), 'map_axpby')
 
 
+def _check_pool(what, x, k, s, dtypes, pooled=(), full=()):
+    """NHWC max-pool operands: x [N, H, W, C] in `dtypes`; every `pooled` tensor [N, OH, OW, C] (floor mode, no padding),
+    every `full` tensor x's shape; all of x's dtype"""
+    if x.dim() != 4 or x.dtype not in dtypes:
+        raise _lib.DasrError('%s: x must be an NHWC %s tensor (got %s %s)' % (what, ' / '.join(map(str, dtypes)), tuple(x.shape), x.dtype))
+    N, H, W, Cc = x.shape
+    want = {}
+    if H >= k and W >= k:
+        want.update((name, (N, (H - k) // s + 1, (W - k) // s + 1, Cc)) for name, _ in pooled)
+    want.update((name, tuple(x.shape)) for name, _ in full)
+    for name, t in tuple(pooled) + tuple(full):
+        if name not in want or tuple(t.shape) != want[name] or t.dtype != x.dtype:
+            raise _lib.DasrError('%s: %s is %s %s, the pool of %s needs %s' % (what, name, tuple(t.shape), t.dtype,
+                                                                             tuple(x.shape), want.get(name, 'H, W >= k')))
+
+
 def maxpool2_fwd(x, out):
+    _check_pool('maxpool2_fwd', x, 2, 2, _F32_BF16, pooled=(('out', out),))
     N, H, W, Cc = x.shape
     if x.dtype == torch.bfloat16:
         return check(_lib.load().dasr_maxpool2_fwd_bf16(_p(x), _p(out), N, H, W, Cc, _stream()), 'maxpool2_fwd_bf16')
@@ -490,6 +549,7 @@ def maxpool2_fwd(x, out):
 
 
 def maxpool2_bwd(x, out, dout, din):
+    _check_pool('maxpool2_bwd', x, 2, 2, _F32_BF16, pooled=(('out', out), ('dout', dout)), full=(('din', din),))
     N, H, W, Cc = x.shape
     if x.dtype == torch.bfloat16:
         return check(_lib.load().dasr_maxpool2_bwd_bf16(_p(x), _p(out), _p(dout), _p(din), N, H, W, Cc, _stream()),
@@ -499,11 +559,13 @@ def maxpool2_bwd(x, out, dout, din):
 
 def maxpool_fwd(x, out, k, s):
     """k x k stride-s max-pool without padding, NHWC fp32 (AlexNet's MaxPool2d(3, 2))."""
+    _check_pool('maxpool_fwd', x, k, s, (torch.float32,), pooled=(('out', out),))
     N, H, W, Cc = x.shape
     check(_lib.load().dasr_maxpool_fwd(_p(x), _p(out), N, H, W, Cc, k, s, _stream()), 'maxpool_fwd')
 
 
 def maxpool_bwd(x, out, dout, din, k, s):
+    _check_pool('maxpool_bwd', x, k, s, (torch.float32,), pooled=(('out', out), ('dout', dout)), full=(('din', din),))
     N, H, W, Cc = x.shape
     check(_lib.load().dasr_maxpool_bwd(_p(x), _p(out), _p(dout), _p(din), N, H, W, Cc, k, s, _stream()), 'maxpool_bwd')
 
@@ -511,14 +573,30 @@ def maxpool_bwd(x, out, dout, din, k, s):
 def lpips_layer_fwd(feats, lin_w, val, eps, accumulate):
     """feats: NHWC fp32 [2N,H,W,C] = [target ; pred] features; val[N] (+)= spatial mean of the lin-weighted squared
     difference of the channel-normalised features (networks_basic.py:66-79)."""
+    N = _check_lpips('lpips_layer_fwd', feats, lin_w, val=val)
     M, H, W, Cc = feats.shape
-    N = M // 2
     scratch = torch.empty(N * H * W, dtype=torch.float32, device=feats.device)
     check(_lib.load().dasr_lpips_layer_fwd(_p(feats), _p(lin_w), _p(val), _p(scratch), N, H, W, Cc, eps, int(accumulate),
                                            _stream()), 'lpips_layer_fwd', 2)
 
 
+def _check_lpips(what, feats, lin_w, val=None, dval=None, dpred=None):
+    """[target ; pred] features: an even batch of fp32 NHWC images, C lin weights, N values / value gradients, and a pred
+    gradient [N, H, W, C]; returns N"""
+    if feats.dim() != 4 or feats.dtype != torch.float32 or feats.shape[0] % 2:
+        raise _lib.DasrError('%s: feats must be fp32 [2N, H, W, C] = [target ; pred] (got %s %s)' % (what, tuple(feats.shape), feats.dtype))
+    M, H, W, Cc = feats.shape
+    N = M // 2
+    for name, t, n in (('lin_w', lin_w, Cc), ('val', val, N), ('dval', dval, N)):
+        if t is not None and (t.dtype != torch.float32 or t.numel() != n):
+            raise _lib.DasrError('%s: %s must hold %d fp32 values (got %d %s)' % (what, name, n, t.numel(), t.dtype))
+    if dpred is not None and (tuple(dpred.shape) != (N, H, W, Cc) or dpred.dtype != torch.float32):
+        raise _lib.DasrError('%s: dpred is %s %s, the pred features are %s' % (what, tuple(dpred.shape), dpred.dtype, (N, H, W, Cc)))
+    return N
+
+
 def lpips_layer_bwd(feats, lin_w, dval, dpred, eps, accumulate):
+    _check_lpips('lpips_layer_bwd', feats, lin_w, dval=dval, dpred=dpred)
     M, H, W, Cc = feats.shape
     check(_lib.load().dasr_lpips_layer_bwd(_p(feats), _p(lin_w), _p(dval), _p(dpred), M // 2, H, W, Cc, eps, int(accumulate),
                                            _stream()), 'lpips_layer_bwd')

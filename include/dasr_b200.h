@@ -248,7 +248,9 @@ int dasr_pack_filter_tc_batch(const DasrPackJob* jobs, int njobs, int blocks_per
  * ---------------------------------------------------------------------------------------------- */
 /* NCHW fp32 <-> NHWC (fp32 or bf16) with channel stride/offset; optional per-channel (x-mean)/std
  * (VGGFeatureExtractor input norm, architecture.py:1073-1086).  mean/std may be NULL. */
-/* dst_is_bf16 / is_bf16 of nchw_to_nhwc and axpby: 0 = fp32, 1 = bf16, 2 = IEEE half */
+/* dst_is_bf16 / is_bf16 of nchw_to_nhwc and axpby: 0 = fp32, 1 = bf16, 2 = IEEE half.  nhwc_to_nchw, act_bwd and
+ * upsample2x_* implement 0 and 1 only and refuse any other code (DASR_E_BADARG).  Every channel slice of these entry points,
+ * map_axpby and axpby must lie inside its rows (0 <= coff, coff + C <= cs), or the call is refused. */
 int dasr_nchw_to_nhwc(const float* src, void* dst, int N, int C, int H, int W, int dst_cs,
                       int dst_coff, int dst_is_bf16, const float* mean, const float* std, void* stream);
 int dasr_nhwc_to_nchw(const void* src, float* dst, int N, int C, int H, int W, int src_cs,
@@ -320,11 +322,13 @@ int dasr_pixel_shuffle(const float* in, float* out, int N, int H, int W, int C, 
 int dasr_ddm(const float* patch, double* out, double* scratch, const int* ilo, const int* ihi, const int* jlo, const int* jhi,
              int NC, int nfh, int nfw, int H, int W, void* stream);
 
-/* 2x2 s2 max-pool NHWC fp32 fwd / bwd (VGG19 features, architecture.py:1076) */
+/* 2x2 s2 max-pool NHWC fp32 fwd / bwd (VGG19 features, architecture.py:1076).  Max-pool results (here and dasr_maxpool_*)
+ * are compared by value: of a +0 / -0 tie the forward may return either zero, and the backward's first-maximal rule counts
+ * both as equal.  Inputs are finite (no NaN / Inf): fmaxf drops a NaN where ATen would propagate it. */
 int dasr_maxpool2_fwd(const float* in, float* out, int N, int H, int W, int C, void* stream);
 int dasr_maxpool2_bwd(const float* in, const float* out, const float* dout, float* din, int N, int H,
                       int W, int C, void* stream);
-/* the same on NHWC bf16 (C % 8 == 0) for the tensor-core VGG path */
+/* the same on NHWC bf16 (C % 8 == 0; every operand 16-byte aligned, else DASR_E_BADARG) for the tensor-core VGG path */
 int dasr_maxpool2_fwd_bf16(const void* in, void* out, int N, int H, int W, int C, void* stream);
 int dasr_maxpool2_bwd_bf16(const void* in, const void* out, const void* dout, void* din, int N, int H,
                            int W, int C, void* stream);
@@ -340,7 +344,7 @@ int dasr_instnorm_lrelu_bwd(const float* y, const float* stats, const float* dy,
 /* Haar DWT J=1 frequency split with DASR's normalisation, NCHW fp32 in/out.
  * Replaces DASR_Model.wavelet_s (DASR_model.py:442-452) -> pytorch_wavelets.DWTForward.
  * ll[N,C,H/2,W/2] = LL*(norm?0.5:1); hc[N,3C,H/2,W/2] band-major (LH_c.., HL_c.., HH_c..),
- * = band*(norm?0.5:1) + (norm?0.5:0). */
+ * = band*(norm?0.5:1) + (norm?0.5:0).  x (fwd) / dx (bwd) must be 8-byte aligned (DASR_E_BADARG otherwise). */
 int dasr_haar_fwd(const float* x, float* ll, float* hc, int N, int C, int H, int W, int norm, void* stream);
 int dasr_haar_bwd(const float* dll /*nullable*/, const float* dhc /*nullable*/, float* dx, int N, int C,
                   int H, int W, int norm, void* stream);
@@ -363,6 +367,7 @@ int dasr_bilinear_fwd(const float* src, float* dst, int NC, int H, int W, int OH
  *         (w == NULL -> plain L1 mean, nn.L1Loss :75-80, :220-222, :225-229)
  *   mse : mean((a-b)^2)
  *   bce : BCEWithLogits(x, target) mean                      loss.py:16,36-40  (GANLoss vanilla)
+ * Inputs are finite: NaN / Inf operands are outside the training domain of these losses and pools.
  */
 int dasr_wl1_loss(const float* a, const float* b, const float* w, float* loss, float* grad_a, float gscale,
                   int N, int C, int HW, float* partials, void* stream);
@@ -382,7 +387,9 @@ int dasr_prelu_fwd(const float* z, const float* slope, float* y, long n, void* s
 int dasr_prelu_bwd(const float* z, const float* dy, const float* slope, float* dz, float* dslope, int accumulate,
                    long n, float* partials, void* stream);
 /* the same on bf16 tensors (n % 8 == 0; slope and its gradient stay fp32) and a dtype cast between the bf16 tensor-core
- * layers and the fp32 layers of the mixed-precision De_resnet (to_bf16: fp32 -> bf16, else bf16 -> fp32) */
+ * layers and the fp32 layers of the mixed-precision De_resnet (to_bf16: fp32 -> bf16, else bf16 -> fp32, round to nearest
+ * even).  The tensor operands of these three are read and written as 16-byte vectors: a base address that is not 16-byte
+ * aligned is refused (DASR_E_BADARG). */
 int dasr_prelu_fwd_bf16(const void* z, const float* slope, void* y, long n, void* stream);
 int dasr_prelu_bwd_bf16(const void* z, const void* dy, const float* slope, void* dz, float* dslope, int accumulate,
                         long n, float* partials, void* stream);
