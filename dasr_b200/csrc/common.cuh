@@ -29,6 +29,7 @@ inline int check_launch(const char* what) {
   } while (0)
 
 static inline int cdiv(long a, long b) { return (int)((a + b - 1) / b); }
+static inline bool aligned_to(const void* p, uintptr_t n) { return (reinterpret_cast<uintptr_t>(p) & (n - 1)) == 0; }
 
 int num_sms();
 // programmatic dependent launch of the tensor-core conv kernels (DASR_B200_PDL=0 switches it off)

@@ -308,6 +308,9 @@ int dasr_rdb_wgrad_tc(const void* xbuf, int x_cs, const void* ga, int ga_cs, int
                    gb_cs % 8 == 0 && gb_coff % 8 == 0 && gb_coff + 64 <= gb_cs,
                "rdb_wgrad_tc: channel slices");
   for (int k = 0; k < 5; k++) DASR_REQUIRE(dw[k], "rdb_wgrad_tc: dw[%d] is null", k);
+  DASR_REQUIRE(aligned_to(xbuf, 16) && aligned_to(ga, 16) && aligned_to(gb, 16),
+               "rdb_wgrad_tc: xbuf, ga and gb must be 16-byte aligned (TMA base addresses)");
+  DASR_REQUIRE(aligned_to(workspace, 8), "rdb_wgrad_tc: workspace must be 8-byte aligned (float2 partials)");
   PFN_encodeTiled enc = get_encode();
   if (!enc) {
     set_error("rdb_wgrad_tc: cuTensorMapEncodeTiled not available");

@@ -177,6 +177,8 @@ int dasr_conv3x3_wgrad_tc(const void* x, int x_cs, int x_coff, const void* dy, i
   DASR_REQUIRE(x_cs % 8 == 0 && x_coff % 8 == 0 && dy_cs % 8 == 0 && dy_coff % 8 == 0 && x_coff + cin <= x_cs &&
                    dy_coff + cout <= dy_cs,
                "wgrad_tc: channel slices");
+  DASR_REQUIRE(aligned_to(x, 16) && aligned_to(dy, 16), "wgrad_tc: x and dy must be 16-byte aligned (TMA base addresses)");
+  DASR_REQUIRE(aligned_to(workspace, 8), "wgrad_tc: workspace must be 8-byte aligned (float2 partials)");
   DASR_REQUIRE(workspace_bytes >= dasr_conv3x3_wgrad_tc_workspace(N, H, W, cin, cout), "wgrad_tc: workspace too small");
   PFN_encodeTiled enc = get_encode();
   if (!enc) {

@@ -180,9 +180,25 @@ def conv2d_wgrad_f32(inp, dout, dw, db, k, stride, pad, ups=1, accumulate=False)
         bias_grad(dout, db, accumulate)
 
 
+def _check_wgrad_tc(what, pix, operands, dws):
+    """wgmma filter gradients: bf16 NHWC operands over the pixels `pix` = [N, H, W], and each (dw, cout, cin) an fp32
+    contiguous OIHW [cout][cin][3][3] tensor (the reduction writes 9 * cin * cout floats from its first element)"""
+    for name, t in operands:
+        if t.dtype != torch.bfloat16:
+            raise _lib.DasrError('%s: %s is %s, the kernel reads bf16' % (what, name, t.dtype))
+        if t.dim() != 4 or tuple(t.shape[:3]) != pix:
+            raise _lib.DasrError('%s: %s is %s, the launch needs [N, H, W] = %s' % (what, name, tuple(t.shape), pix))
+    for dw, cout, cin in dws:
+        if dw.dtype != torch.float32 or not dw.is_contiguous() or tuple(dw.shape) != (cout, cin, 3, 3):
+            raise _lib.DasrError('%s: the filter gradient must be a contiguous fp32 [%d, %d, 3, 3] tensor (got %s %s%s)' % (
+                what, cout, cin, dw.dtype, tuple(dw.shape), '' if dw.is_contiguous() else ', not contiguous'))
+
+
 def conv3x3_wgrad_tc(x, dy, dw, accumulate=False):
-    """wgmma filter gradient of a 3x3 s1 p1 conv: x, dy = Views of bf16 NHWC buffers (channels % 32 == 0), dw fp32 OIHW."""
+    """wgmma filter gradient of a 3x3 s1 p1 conv: x, dy = Views of bf16 NHWC buffers (channels % 32 == 0) over the same
+    pixels, dw fp32 contiguous OIHW [dy.c][x.c][3][3]."""
     x, dy = as_view(x), as_view(dy)
+    _check_wgrad_tc('conv3x3_wgrad_tc', tuple(x.t.shape[:3]), (('x', x.t), ('dy', dy.t)), ((dw, dy.c, x.c),))
     N, H, W, _ = x.t.shape
     lib = _lib.load()
     n = lib.dasr_conv3x3_wgrad_tc_workspace(N, H, W, x.c, dy.c)
@@ -192,7 +208,16 @@ def conv3x3_wgrad_tc(x, dy, dw, accumulate=False):
 
 
 def rdb_wgrad_tc(xbuf, ga, ga_coff, gb, gb_coff, dws, accumulate=False):
-    """filter gradients of the five convs of a dense block (dasr_rdb_wgrad_tc); dws = [dW1..dW5] fp32 OIHW."""
+    """filter gradients of the five convs of a dense block (dasr_rdb_wgrad_tc): xbuf, ga, gb bf16 NHWC over the same pixels
+    (xbuf: at least the 192 channels [x | x1..x4]); dws = [dW1..dW5] fp32 contiguous OIHW [32|64][64+32k][3][3]."""
+    if xbuf.dim() != 4:
+        raise _lib.DasrError('rdb_wgrad_tc: xbuf must be an NHWC [N, H, W, C] tensor (got %s)' % (tuple(xbuf.shape),))
+    if xbuf.shape[-1] < 192:
+        raise _lib.DasrError('rdb_wgrad_tc: xbuf has %d channels, the dense block needs 192' % xbuf.shape[-1])
+    if len(dws) != 5:
+        raise _lib.DasrError('rdb_wgrad_tc: %d filter gradients, the dense block has 5' % len(dws))
+    _check_wgrad_tc('rdb_wgrad_tc', tuple(xbuf.shape[:3]), (('xbuf', xbuf), ('ga', ga), ('gb', gb)),
+                    [(d, 32 if k < 4 else 64, 64 + 32 * k) for k, d in enumerate(dws)])
     N, H, W, _ = xbuf.shape
     lib = _lib.load()
     n = lib.dasr_rdb_wgrad_tc_workspace(N, H, W)

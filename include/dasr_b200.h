@@ -101,7 +101,9 @@ int dasr_conv2d_wgrad_bf16(const void* in_bf16, const void* dout_bf16, float* dw
 
 /* wgmma filter gradient of a 3x3 s1 p1 conv on bf16 NHWC channel slices (cin, cout multiples of 32):
  * dW[co][ci][dy][dx] (fp32 OIHW) = sum_pixels x[p + tap][ci] * dy[p][co], fp32 accumulation in registers, deterministic
- * split-K reduction.  Replaces autograd's weight gradient of the RRDB convs (block.py:142-143, 262-278). */
+ * split-K reduction.  Replaces autograd's weight gradient of the RRDB convs (block.py:142-143, 262-278).
+ * x and dy must be 16-byte aligned (TMA base addresses) and the workspace 8-byte aligned (float2 partials), else
+ * DASR_E_BADARG; the alignment is checked before the workspace size. */
 size_t dasr_conv3x3_wgrad_tc_workspace(int N, int H, int W, int cin, int cout);
 int dasr_conv3x3_wgrad_tc(const void* x_bf16, int x_cs, int x_coff, const void* dy_bf16, int dy_cs, int dy_coff,
                           float* dw_oihw, int N, int H, int W, int cin, int cout, int accumulate, void* workspace,
@@ -277,7 +279,9 @@ int dasr_axpby(const void* x, const void* y, void* dst, long npix, int C, int x_
 /* Filter gradients of all five convs of one ResidualDenseBlock_5C (nf 64, gc 32) in one wgmma launch + one
  * deterministic reduction (mixed-precision training).  xbuf: bf16 NHWC, channels [x 0:64 | x1..x4 64:192];
  * ga: bf16 NHWC holding the (LeakyReLU-masked) output gradients of conv1..4 in channels [ga_coff, ga_coff+128);
- * gb: output gradient of conv5 in channels [gb_coff, gb_coff+64); dw[k]: OIHW fp32 [32|64][64+32k][3][3]. */
+ * gb: output gradient of conv5 in channels [gb_coff, gb_coff+64); dw[k]: OIHW fp32 [32|64][64+32k][3][3].
+ * xbuf, ga and gb must be 16-byte aligned and the workspace 8-byte aligned, else DASR_E_BADARG (checked before the
+ * workspace size). */
 size_t dasr_rdb_wgrad_tc_workspace(int N, int H, int W);
 int dasr_rdb_wgrad_tc(const void* xbuf, int x_cs, const void* ga, int ga_cs, int ga_coff, const void* gb, int gb_cs,
                       int gb_coff, float* const* dw, int N, int H, int W, int accumulate, void* workspace,

@@ -61,8 +61,9 @@ from oracle import dsn_oracle as DO  # noqa: E402
 from oracle import srn_oracle as O  # noqa: E402
 from tests import test_gpu_elementwise_exact as EW  # noqa: E402
 from tests.test_engine_launch_plan import HOST_ONLY, _real_lib  # noqa: E402
-from tests.test_gpu_conv_tc_exact import _geometry, _wgrad64, conv_tc_ref, decode_filter  # noqa: E402
+from tests.test_gpu_conv_tc_exact import _geometry, conv_tc_ref, decode_filter  # noqa: E402
 from tests.test_gpu_f32_kernels_exact import conv_f32_ref, pack_f32_ref, wgrad_f32_ref  # noqa: E402
+from tests.test_gpu_wgrad_tc_exact import _wgrad64  # noqa: E402
 
 TOL = 1e-9
 TOL_MAP_CHANNEL = 2.0 ** -20

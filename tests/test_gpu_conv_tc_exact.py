@@ -15,9 +15,11 @@ Two regimes:
 """
 import ctypes as C
 import inspect
+import json
 import os
 import re
 import subprocess
+import sys
 import zlib
 from dataclasses import dataclass
 from typing import Optional, Tuple
@@ -496,24 +498,54 @@ def _kernel_args(name):
     return (int(a[0]), a[1] == 'true', int(a[2]), int(a[3]), int(a[4]), int(a[5]))
 
 
+def _trace_consumer_paths(ids=None):
+    """the body of test_conv_tc_consumer_paths for the cases `ids` (None: all): prints one line 'TRACE {json}' with the
+    mismatches, the cases whose sessions returned no kernel record, and the ping-pong instantiations reached"""
+    from torch.profiler import ProfilerActivity, profile
+    reached, wrong, empty = set(), [], []
+    with profile(activities=[ProfilerActivity.CUDA]):          # the first session of a process starts late: discard it
+        _run_exact(CASES[0])
+    for c in CASES:
+        if ids is not None and c.id not in ids:
+            continue
+        inp, wp, bias, out, kw, _ = _make(c)
+        for _ in range(3):          # a session that returned no kernel record at all lost its records: trace it again
+            torch.cuda.synchronize()
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                ops.conv_tc(inp, wp, bias, out, **kw)
+                torch.cuda.synchronize()
+            ran = {_kernel_args(e.name) for e in prof.events() if 'conv_tc_kernel' in e.name}
+            if ran:
+                break
+        if not ran:
+            empty.append(c.id)
+        elif ran != {c.kernel_args()}:
+            wrong.append('%s: ran %s, declared %s' % (c.id, sorted(ran), c.kernel_args()))
+        reached |= {k for k in ran if k and k[4]}
+    print('TRACE ' + json.dumps({'wrong': wrong, 'empty': empty, 'reached': sorted(reached)}))
+
+
 def test_conv_tc_consumer_paths():
     """Every case runs the conv_tc_kernel instantiation its declared path implies (ping-pong: NT = the Cout tile of a CTA),
     and the case matrix reaches every ping-pong instantiation, so a change of the selection rule cannot silently move
-    the coverage of the exact test."""
-    from torch.profiler import ProfilerActivity, profile
-    reached, wrong = set(), []
-    for c in CASES:
-        inp, wp, bias, out, kw, _ = _make(c)
-        torch.cuda.synchronize()
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            ops.conv_tc(inp, wp, bias, out, **kw)
-            torch.cuda.synchronize()
-        ran = {_kernel_args(e.name) for e in prof.events() if 'conv_tc_kernel' in e.name}
-        if ran != {c.kernel_args()}:
-            wrong.append('%s: ran %s, declared %s' % (c.id, sorted(ran), c.kernel_args()))
-        reached |= {k for k in ran if k and k[4]}
+    the coverage of the exact test.  The trace runs in a fresh interpreter, as the other path tests do: profiler sessions
+    can come back without any kernel record, sometimes for one case again and again in the same process, so such cases
+    are traced again in up to two more fresh interpreters before they count as a failure."""
+    ids, reached, wrong = None, set(), []
+    for _ in range(3):
+        code = 'import sys; sys.path[:0] = [%r, %r]; from tests.test_gpu_conv_tc_exact import _trace_consumer_paths; ' \
+               '_trace_consumer_paths(%r)' % (ROOT, os.path.join(ROOT, 'tests'), ids)
+        r = subprocess.run([sys.executable, '-c', code], capture_output=True, text=True, cwd=ROOT, timeout=900)
+        assert r.returncode == 0, r.stdout[-4000:] + r.stderr[-4000:]
+        res = json.loads([ln for ln in r.stdout.splitlines() if ln.startswith('TRACE ')][-1][6:])
+        wrong += res['wrong']
+        reached |= {tuple(k) for k in res['reached']}
+        ids = res['empty']
+        if not ids:
+            break
     print('SMs: %d; ping-pong instantiations reached <EPI, PRE, NRES, MAP, NT, NTAPS>: %s' % (_sms(), sorted(reached)))
     assert not wrong, '\n'.join(wrong)
+    assert not ids, 'cases whose profiler sessions returned no kernel record in three fresh interpreters: %s' % ids
     assert PP_KERNELS <= reached, 'not reached: %s' % sorted(PP_KERNELS - reached)
 
 
@@ -639,53 +671,6 @@ def test_dasr_conv_tc_refuses_slices_outside_their_tensors(what):
                           C.c_void_p(out.data_ptr()), C.byref(p), C.c_void_p(torch.cuda.current_stream().cuda_stream))
     torch.cuda.synchronize()
     assert rc != 0, 'dasr_conv_tc accepted %s' % what
-
-
-# ------------------------------------------------------------------------------------------------------------------------
-# filter gradients: dasr_conv3x3_wgrad_tc and dasr_rdb_wgrad_tc, exact with dyadic operands
-# ------------------------------------------------------------------------------------------------------------------------
-
-def _wgrad64(x, dy):
-    """dW[co][ci][a][b] = sum over pixels of x[y + a - 1][x + b - 1][ci] * dy[y][x][co] (zero outside the image)"""
-    N, H, W, _ = x.shape
-    xp = F.pad(x, (0, 0, 1, 1, 1, 1))
-    return torch.stack([torch.stack([torch.einsum('nhwc,nhwd->dc', xp[:, a:a + H, b:b + W], dy) for b in range(3)], -1)
-                        for a in range(3)], -2)
-
-
-@pytest.mark.parametrize('shape,cin,cout,xcoff,dycoff', [((2, 21, 13), 64, 32, 8, 16), ((1, 40, 24), 96, 64, 32, 8),
-                                                         ((3, 16, 8), 32, 32, 0, 40)])
-def test_conv3x3_wgrad_tc_exact(shape, cin, cout, xcoff, dycoff):
-    g = torch.Generator().manual_seed(cin + cout)
-    N, H, W = shape
-    xb = _dy((N, H, W, xcoff + cin + 16), g, dt=torch.bfloat16)
-    yb = _dy((N, H, W, dycoff + cout + 8), g, dt=torch.bfloat16)
-    dw0 = _dy((cout, cin, 3, 3), g)
-    dw = dw0.clone()
-    ops.conv3x3_wgrad_tc(View(xb, cin, xcoff), View(yb, cout, dycoff), dw, accumulate=True)
-    torch.cuda.synchronize()
-    ref = dw0.double() + _wgrad64(xb[..., xcoff:xcoff + cin].double(), yb[..., dycoff:dycoff + cout].double())
-    assert torch.equal(ref, ref.float().double())
-    assert torch.equal(dw.double(), ref)
-
-
-@pytest.mark.parametrize('shape,ga_coff,gb_coff', [((2, 21, 13), 8, 16), ((1, 40, 24), 64, 0)])
-def test_rdb_wgrad_tc_exact(shape, ga_coff, gb_coff):
-    g = torch.Generator().manual_seed(ga_coff + 3)
-    N, H, W = shape
-    xb = _dy((N, H, W, 200), g, dt=torch.bfloat16)
-    ga = _dy((N, H, W, ga_coff + 128 + 8), g, dt=torch.bfloat16)
-    gb = _dy((N, H, W, gb_coff + 64 + 24), g, dt=torch.bfloat16)
-    dw0 = [_dy(((32 if k < 4 else 64), 64 + 32 * k, 3, 3), g) for k in range(5)]
-    dws = [d.clone() for d in dw0]
-    ops.rdb_wgrad_tc(xb, ga, ga_coff, gb, gb_coff, dws, accumulate=True)
-    torch.cuda.synchronize()
-    for k in range(5):
-        cin = 64 + 32 * k
-        dy = ga[..., ga_coff + 32 * k:ga_coff + 32 * k + 32] if k < 4 else gb[..., gb_coff:gb_coff + 64]
-        ref = dw0[k].double() + _wgrad64(xb[..., :cin].double(), dy.double())
-        assert torch.equal(ref, ref.float().double())
-        assert torch.equal(dws[k].double(), ref), 'conv%d' % (k + 1)
 
 
 def test_selftest_check_passes():

@@ -842,7 +842,7 @@ def test_cabi_refuses_before_any_cuda_call(case):
     assert rc == -1, '%s returned %d (not DASR_E_BADARG): %s' % (sym, rc, (lib.dasr_last_error() or b'').decode())
 
 
-# symbols of include/dasr_b200.h outside the three exact modules' scope, with the reason
+# symbols of include/dasr_b200.h outside the exact modules' scope, with the reason
 OUT_OF_SCOPE = {
     'dasr_last_error': 'error text of the last failed call; read by every refusal test through _lib.check',
     'dasr_version': 'constant version number',
@@ -860,10 +860,10 @@ LEDGER = {
     'dasr_instnorm_lrelu_bwd': ('test_gpu_f32_kernels_exact', 'test_instnorm_lrelu_fwd_bwd_vs_float64_autograd'),
     'dasr_bn_lrelu_fwd': ('test_gpu_f32_kernels_exact', 'test_bn_lrelu_vs_float64_autograd'),
     'dasr_bn_lrelu_bwd': ('test_gpu_f32_kernels_exact', 'test_bn_lrelu_vs_float64_autograd'),
-    'dasr_conv3x3_wgrad_tc_workspace': ('test_gpu_conv_tc_exact', 'test_conv3x3_wgrad_tc_exact'),
-    'dasr_conv3x3_wgrad_tc': ('test_gpu_conv_tc_exact', 'test_conv3x3_wgrad_tc_exact'),
-    'dasr_rdb_wgrad_tc_workspace': ('test_gpu_conv_tc_exact', 'test_rdb_wgrad_tc_exact'),
-    'dasr_rdb_wgrad_tc': ('test_gpu_conv_tc_exact', 'test_rdb_wgrad_tc_exact'),
+    'dasr_conv3x3_wgrad_tc_workspace': ('test_gpu_wgrad_tc_exact', 'test_conv3x3_wgrad_tc_exact'),
+    'dasr_conv3x3_wgrad_tc': ('test_gpu_wgrad_tc_exact', 'test_conv3x3_wgrad_tc_exact'),
+    'dasr_rdb_wgrad_tc_workspace': ('test_gpu_wgrad_tc_exact', 'test_rdb_wgrad_tc_exact'),
+    'dasr_rdb_wgrad_tc': ('test_gpu_wgrad_tc_exact', 'test_rdb_wgrad_tc_exact'),
     'dasr_conv_tc': ('test_gpu_conv_tc_exact', 'test_conv_tc_exact'),
     'dasr_conv_tc2_supported': ('test_gpu_conv_tc_exact', 'test_shadow_vgg_bf16_forward_backward'),   # VGG Cout tiles
     'dasr_conv_tc2': ('test_gpu_conv_tc_exact', 'test_conv_tc_exact'),
@@ -912,7 +912,7 @@ LEDGER = {
 
 
 def test_coverage_ledger_names_every_header_symbol():
-    """every dasr_* symbol of the header is checked by a named test of one of the three exact modules (the batch filter
+    """every dasr_* symbol of the header is checked by a named test of one of the exact modules (the batch filter
     packer: by the parity test that compares it bit for bit with the per-filter packer), or is listed as out of scope
     with a reason: a new entry point without a model test fails here.  Whether each named test reaches its symbol is
     checked by call counts at the ctypes layer: this module's entries in test_elementwise_kernel_paths, the pair kernel's
