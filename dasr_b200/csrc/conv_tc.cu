@@ -23,7 +23,6 @@
 // Cluster pair (dasr_conv_tc2): two CTAs of a (1, 2, 1) cluster take the two Cout halves of the SAME pixel tiles; each
 // keeps only its half of the filters resident, and the leader's TMA multicasts every A halo tile into both CTAs, so an
 // activation tile crosses L2 -> SMEM once for the pair.  That is what lets a 192-wide filter set (221 KB) run as one tile.
-#include <stdlib.h>
 #include <type_traits>
 #include "tc_common.cuh"
 
@@ -64,7 +63,6 @@ struct TcKernelArgs {
   int epi_bytes;     // bytes of ONE staged epilogue tile: 128 pixels x nt channels bf16
   int has_pre, has_res1, has_res2;
   int nbuf;          // staged-epilogue tile frames (1..4): pre / residual blocks are requested nbuf tiles ahead
-  int ring;          // ping-pong: each staged block is stored and its frame slots retired on their own (0: whole tiles)
   int pair;          // 1: launched as (1, 2, 1) clusters, A tiles multicast by the leader (rank 0)
   const float* map;  // weight map [N][H][W] fp32 (image stride p.map_stride), MAP != 0 only
   const float* map_w;// MAP 1: the map channel's filter taps [9][cout] fp32
@@ -346,15 +344,15 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
   } else if (warp == EPI_TMA_WARP) {
     // =========================== epilogue TMA warp ===========================
     // Feeds the staged epilogue: pre-activation / residual blocks in (nbuf tiles ahead), finished blocks out.  A tile's
-    // frame is frame it % nbuf; its blocks go out in store units: each block on its own on the ping-pong consumers with
-    // the stage ring (a.ring), otherwise the whole tile.  Ping-pong frames have one barrier per block, so a block is
-    // stored as soon as its warpgroup has written it and its slots return (next pre / residual loads, or sfree) as soon as
-    // that store has read them; the other frames have one barrier per tile.
+    // frame is frame it % nbuf; its blocks go out in store units: each block on its own on the ping-pong consumers,
+    // otherwise the whole tile.  Ping-pong frames have one barrier per block, so a block is stored as soon as its
+    // warpgroup has written it and its slots return (next pre / residual loads, or sfree) as soon as that store has read
+    // them; the other frames have one barrier per tile.
     if constexpr (EPI_MODE == 0) {
       const int co_base = p.out_coff + ntile * nt;
       const int omap = (p.out_mul == 2) ? 3 * var : 0;      // sub-pixel variants: one strided output map triple per parity
       const int nload = (HAS_PRE ? 1 : 0) + NRES;
-      const int unit = (NT > 0 && a.ring) ? 1 : nblocks;   // blocks per store unit
+      const int unit = NT > 0 ? 1 : nblocks;   // blocks per store unit
       auto bar_of = [&](int f, int i) { return f * FRAME_BLKS + (NT > 0 ? i : 0); };
       pdl_wait();                      // pre / residual tiles and the output slots belong to earlier launches until now
       auto issue_loads = [&](long tile, int f, int i0, int i1) {      // blocks [i0, i1) of a tile into frame f; lane 0 issues
@@ -1051,25 +1049,6 @@ static int tc_plan(int w_bytes, int a_stage, int epi_bytes, int nres_loaded, int
 static int g_trace_coop = 0;   // traced build: 1 = every launch on the cooperative consumers (the before / after comparison)
 #endif
 
-static int env_switch(const char* name) {
-  const char* e = getenv(name);
-  return (e && e[0] == '0') ? 0 : 1;
-}
-static int chunk64_allowed() {
-  static const int ok = env_switch("DASR_TC_CHUNK64");
-  return ok;
-}
-// pair A feed: 64-channel loads where they pay (0: 32-channel loads on every pair launch, the A/B comparison)
-static int pair_feed_allowed() {
-  static const int ok = env_switch("DASR_TC_PAIR_FEED");
-  return ok;
-}
-// ping-pong staged epilogue stored and retired block by block (0: whole tiles and the whole-tile A plan, the A/B comparison)
-static int stage_ring_allowed() {
-  static const int ok = env_switch("DASR_TC_STAGE_RING");
-  return ok;
-}
-
 // a chunk list of 64-channel runs: pairs (c, c + 32) with c % 64 == 0
 static bool chunk_list_pairs64(const DasrConvTcParams* p) {
   if (p->nchunk_list == 0 || p->nchunk_list % 2) return false;
@@ -1106,7 +1085,7 @@ static int conv_tc_launch(const void* in, const void* w, const float* bias, cons
   a.w_bytes = p->ntaps * a.nchunks * p->nt * ROW_B;
   // single CTA: 64-channel A chunks for a contiguous input slice whose channel count is a multiple of 64 (a pair starts
   // from 32-channel stages, whose smaller footprint leaves room for the larger filter sets it exists for; see below)
-  a.chunk64 = (chunk64_allowed() && !pair && p->a_mode == 0 && p->nchunk_list == 0 && p->cin % (2 * CHUNK) == 0) ? 1 : 0;
+  a.chunk64 = (!pair && p->a_mode == 0 && p->nchunk_list == 0 && p->cin % (2 * CHUNK) == 0) ? 1 : 0;
   a.has_pre = (p->epi_mode == 0 && pre) ? 1 : 0;
   a.has_res1 = (p->epi_mode == 0 && res1) ? 1 : 0;
   a.has_res2 = (p->epi_mode == 0 && res2) ? 1 : 0;
@@ -1151,20 +1130,14 @@ static int conv_tc_launch(const void* in, const void* w, const float* bias, cons
   if (g_trace_coop) pp = -1;
 #endif
 
-  a.ring = (pp >= 0 && stage_ring_allowed()) ? 1 : 0;
-
   // Pair on the ping-pong consumers: 64-channel A loads (half the TMA requests per byte) for a contiguous slice of 64k
   // channels or a chunk list of 64-channel runs, issued half-major (chunk64 = 2), so the products and their order stay
   // those of 32-channel loads.  Only when the wider stages still leave two staging frames and hold the A loads of two
-  // tiles, one per consumer warpgroup; otherwise the launch keeps its 32-channel plan.  With whole-tile staging
-  // (a.ring = 0) the wide stages must also keep at least as many A bytes in flight as the narrow ones, and the Cout
-  // tile of 96 (dense-block launch 1: 2 wide stages against 5 narrow ones) stays on 32-channel loads.
-  if (pair && pair_feed_allowed() && pp >= 0 && p->ntaps == 9 && (a.ring || p->nt <= 64) &&
-      ((p->nchunk_list == 0 && p->cin % (2 * CHUNK) == 0) || chunk_list_pairs64(p))) {
+  // tiles, one per consumer warpgroup; otherwise the launch keeps its 32-channel plan.
+  if (pair && pp >= 0 && p->ntaps == 9 && ((p->nchunk_list == 0 && p->cin % (2 * CHUNK) == 0) || chunk_list_pairs64(p))) {
     int nbuf64 = 0;
     const int stages64 = tc_plan(a.w_bytes, (int)a_stage_bytes_for(p, 1), a.epi_bytes, a.has_res1 + a.has_res2, 0, &nbuf64);
-    const bool enough = a.ring ? stages64 >= 2 * (a.nchunks / 2) : 2 * stages64 >= stages;
-    if (stages64 >= 2 && nbuf64 >= 2 && enough) {
+    if (stages64 >= 2 && nbuf64 >= 2 && stages64 >= 2 * (a.nchunks / 2)) {
       a.chunk64 = 2;
       stages = stages64;
       nbuf = nbuf64;

@@ -6,7 +6,6 @@ weights, fp32 filter gradients.  Opt-in: De_resnet.precision = 'bf16' or DASR_B2
 import torch
 
 from dasr_b200 import ops, seqnet
-from dasr_b200 import engine as _engine
 from dasr_b200.engine import _PackCache, _pad_filter, _pick_nt_staged
 from dasr_b200.ops import ACT_NONE, TC_DGRAD, TC_FPROP, View
 
@@ -14,9 +13,8 @@ BF = torch.bfloat16
 
 
 def _pair(nf):
-    """64 -> 64 trunk convs on the cluster pair (the activation tile is read once for both Cout halves; DASR_B200_PAIR=0
-    switches back)."""
-    return _engine.PAIR_MODE and nf % 64 == 0 and nf <= 256
+    """64 -> 64 trunk convs on the cluster pair (the activation tile is read once for both Cout halves)."""
+    return nf % 64 == 0 and nf <= 256
 
 
 def forward(x, params, n_res, tail_layers, tail_params, save):

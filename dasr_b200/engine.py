@@ -449,16 +449,12 @@ class _BatchPacker:
                   'pack_filter_tc_batch')
 
 
-PAIR_MODE = os.environ.get('DASR_B200_PAIR', '1') != '0'      # run eligible launches on the CTA-pair kernel (conv_tc2)
-TILE_REV = os.environ.get('DASR_B200_TILE_REV', '1') != '0'
-
-
 def _rdb_stage1(b, w, bias, out, nf, tile_rev=False):
     """Launch 1 of a dense block: x (K = nf) against the stacked filters of conv1..5 (N = 4*GC + nf = 192), LeakyReLU on the
     first GC columns (= x1).  One CTA cannot keep the 192-wide filter set resident, so the single-CTA kernel runs it as
     two Cout tiles of 96 that each load the activation tile; the cluster pair splits the filters over two SMs and
     multicasts one load of the activation tile into both."""
-    if PAIR_MODE and nf == 64:
+    if nf == 64:
         ops.conv_tc(View(b, nf, 0), w, bias, out, act=ACT_LRELU, slope=0.2, act_cols=GC, pair=True, tile_rev=tile_rev)
     else:
         ops.conv_tc(View(b, nf, 0), w, bias, out, nt=out.c // 2, act=ACT_LRELU, slope=0.2, act_cols=GC)
@@ -495,7 +491,7 @@ def _rdb_bf16(b, dst, r, tail, params, L, cache, half, wk, bk, sched=None, tile_
     sched     : dense-block schedule (SCHED1 / SCHED3): launch j completes conv j and carries partial sums of later convs.
                 None: one launch per conv over the growing concat (the per-layer form, the reference of the tests).
     tile_rev  : consecutive launches walk the tile grid in opposite directions, so each one starts with the tiles the
-                previous one wrote last, which are still in L2 (DASR_B200_TILE_REV=0: always forwards).
+                previous one wrote last, which are still in L2.
     chunk_list: launches 2..5 name their input chunks in a chunk list (ops.conv_tc chunks=); otherwise a launch reads its
                 one chunk as a 32-channel slice of b.  The kernel treats a one-chunk list and such a slice alike."""
     nf = L.nf
@@ -509,7 +505,7 @@ def _rdb_bf16(b, dst, r, tail, params, L, cache, half, wk, bk, sched=None, tile_
         return
     tag = ('f' if sched is SCHED1 else 's3') + ('h' if half else '')
     fw = _sched_rdb_filters(cache, params, L, r, nf, sched, tag, torch.float16 if half else torch.bfloat16)
-    rev = lambda j: tile_rev and TILE_REV and PAIR_MODE and ((5 * r + j) & 1) == 1
+    rev = lambda j: tile_rev and ((5 * r + j) & 1) == 1
     w1 = sum(nf if k == 5 else GC for k in sched[0][1])            # launch 1: x1 | partial sums of the convs it starts
     _rdb_stage1(b, fw[0][0], fw[0][1], View(b, w1, nf), nf, tile_rev=rev(1))
     for j in (2, 3, 4, 5):
@@ -522,24 +518,24 @@ def _rdb_bf16(b, dst, r, tail, params, L, cache, half, wk, bk, sched=None, tile_
         if j < 5:
             ks = sched[j - 1][1]
             o = View(b, sum(nf if k == 5 else GC for k in ks), nf + (j - 1) * GC)     # slots of conv j .. ks[-1], in place
-            ops.conv_tc(inp, w, bias, o, act=ACT_LRELU, slope=0.2, act_cols=GC, pre=o, chunks=chunks, pair=PAIR_MODE,
+            ops.conv_tc(inp, w, bias, o, act=ACT_LRELU, slope=0.2, act_cols=GC, pre=o, chunks=chunks, pair=True,
                         tile_rev=rev(j))
         else:
             pre5 = View(b, nf, CS) if any(5 in kk for _, kk in sched[:4]) else None     # conv5 started earlier?
-            ops.conv_tc(inp, w, bias, dst, pre=pre5, chunks=chunks, pair=PAIR_MODE and nf % 64 == 0, tile_rev=rev(5), **tail)
+            ops.conv_tc(inp, w, bias, dst, pre=pre5, chunks=chunks, pair=nf % 64 == 0, tile_rev=rev(5), **tail)
 
 
 def _trunk_tail_bf16(bufs, fea, L, params, cache, wk, bk, hk, bf, pair=True, save=False):
     """fea + LR_conv(trunk) -> nearest-x2 upconvs -> HR_conv0 -> HR_conv1 on the wgmma kernels; the trunk is the x slot of
     bufs[-1].  Returns (out NCHW fp32, ups, h0).
-    pair: LR_conv and HR_conv0 run on the cluster pair (when PAIR_MODE and nf % 64 == 0).
+    pair: LR_conv and HR_conv0 run on the cluster pair (when nf % 64 == 0).
     save: keep what the backward reads: `bufs`, ups = [LR_conv + fea, upconv outputs...] and h0 = HR_conv0's output.
           Without it ups and h0 are None, and `bufs` (the dense-block buffers) is emptied once LR_conv has read them, so
           their memory returns to the pool before the 4x-resolution layers allocate theirs."""
     nf = L.nf
     x = fea
     N, H, W, _ = fea.shape
-    pair = pair and PAIR_MODE and nf % 64 == 0
+    pair = pair and nf % 64 == 0
     lr = _empty((N, H, W, nf), x, bf)
     ops.conv_tc(View(bufs[-1], nf, 0), wk(L.i_lr), bk(L.i_lr), lr, nt=_pick_nt(nf, nf), res1=fea, beta1=1.0, pair=pair)
     ups = [lr] if save else None
@@ -659,7 +655,7 @@ def adaptive_rrdb_forward_bf16(x, amap, params, nb, nb_ada, concat, upscale=4, c
     ext = _ada_ext(L, concat)
 
     def conv64(src, i, dst):        # 64 -> 64 conv + LeakyReLU of A / R: launched like LR_conv and HR_conv0
-        ops.conv_tc(src, wk(i), bk(i), dst, nt=_pick_nt(nf, nf), act=ACT_LRELU, slope=0.2, pair=PAIR_MODE)
+        ops.conv_tc(src, wk(i), bk(i), dst, nt=_pick_nt(nf, nf), act=ACT_LRELU, slope=0.2, pair=True)
 
     def conv_map(src, i, dst, s):   # 65 -> 64 conv + LeakyReLU: 64 channels on the MMAs, s * map in the epilogue
         w = params[2 * i]
@@ -884,7 +880,7 @@ def rrdb_backward_bf16(ctx, params, dout, cache=None, flat=None):
     # DASR_B200_FUSE_MASK=1: LeakyReLU backward of x1..x4 inside the epilogue of the dgrad launch that completes each slot (pair
     # kernel, activation in the res1 slot): 276 launches less per step, gradients within 4e-3
     # rel-L2 of the unfused ones (one rounding instead of two) -> off by default
-    fuse_mask = PAIR_MODE and nf == 64 and os.environ.get('DASR_B200_FUSE_MASK', '0') == '1'
+    fuse_mask = nf == 64 and os.environ.get('DASR_B200_FUSE_MASK', '0') == '1'
     nset = 2 if overlap else 1
     GBs = [_empty((N, H, W, CS), dev, bf) for _ in range(nset)]
     gx5s = [_empty((N, H, W, nf), dev, bf) for _ in range(nset)]
@@ -908,7 +904,7 @@ def rrdb_backward_bf16(ctx, params, dout, cache=None, flat=None):
             wgrad(View(b, CS, 0), g_x5, ci)
         elif not overlap:
             ops.bias_grad(g_x5, gB(ci))
-        if PAIR_MODE and nf == 64:                                                         # K=64 -> N=192 on a CTA pair
+        if nf == 64:                                                                       # K=64 -> N=192 on a CTA pair
             if fuse_mask:      # ... which also completes the gradient of x4: its LeakyReLU mask is applied in the epilogue
                 ops.conv_tc(g_x5, wd(ci), None, View(GB, CS, 0), kind=TC_DGRAD, pair=True, mask=View(b, CS, 0),
                             mask_c0=nf + 3 * GC, mask_c1=nf + 4 * GC, mask_slope=0.2)
@@ -1282,8 +1278,9 @@ _VGG_NT = {}
 
 
 def _vgg_pair_nt(k_ch, n_ch):
-    """Cout tile of a VGG conv (GEMM-K = k_ch, GEMM-N = n_ch channels) on the CTA-pair kernel, or None (DASR_B200_PAIR=0)."""
-    if not PAIR_MODE or os.environ.get('DASR_B200_VGG_PAIR', '1') == '0' or k_ch % 32 or n_ch % 32:
+    """Cout tile of a VGG conv (GEMM-K = k_ch, GEMM-N = n_ch channels) on the CTA-pair kernel, or None (a channel count
+    that is not a multiple of 32: the single-CTA kernel)."""
+    if k_ch % 32 or n_ch % 32:
         return None
     key = (k_ch, n_ch)
     if key not in _VGG_NT:

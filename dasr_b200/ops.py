@@ -343,9 +343,8 @@ def conv_tc(inp, w_packed, bias, out, kind=TC_FPROP, nt=None, act=ACT_NONE, slop
     p.act, p.slope, p.alpha = act, slope, alpha
     p.act_cols = (out.c if act != ACT_NONE else 0) if act_cols is None else act_cols
     # staged (TMA-store) epilogue whenever the tile is a multiple of 32 channels; the sub-pixel upconv variants (out_mul 2)
-    # take it when they carry no pre / residual inputs (DASR_B200_UP_STAGED=0: direct stores)
-    staged_up = (p.out_mul == 2 and pre is None and res1 is None and res2 is None
-                 and os.environ.get('DASR_B200_UP_STAGED', '1') != '0')
+    # take it when they carry no pre / residual inputs (otherwise direct stores)
+    staged_up = p.out_mul == 2 and pre is None and res1 is None and res2 is None
     p.epi_mode = 0 if ((p.out_mul == 1 or staged_up) and p.nt % 32 == 0 and mask is None) else 1
     if pre is not None:
         pre = as_view(pre)
@@ -423,8 +422,8 @@ def pick_nt_pair(cin, cout):
 
 
 def tapn_enabled(out_nc):
-    """Last layer with the nine taps folded into GEMM-N (dasr_conv_tc epi_mode 3): out_nc <= 3, DASR_B200_TAPN=0 switches it off."""
-    return 9 * out_nc <= 32 and os.environ.get('DASR_B200_TAPN', '1') != '0'
+    """Last layer with the nine taps folded into GEMM-N (dasr_conv_tc epi_mode 3): out_nc <= 3."""
+    return 9 * out_nc <= 32
 
 
 def _conv_tc_nchw(inp, w_packed, bias, nchw_out, cout, act, slope, alpha, a_mode, tapn=False):

@@ -690,24 +690,20 @@ def test_adaptive_generators_float64(backend, concat):
             TOL_MAP_CHANNEL if concat else TOL)
 
 
-TRAIN = [(1, '0', '0', True), (1, '1', '0', True), (1, '0', '1', True), (1, '1', '1', True),
-         (2, '0', '0', True), (2, '1', '0', True), (2, '0', '1', True), (2, '1', '1', True),
-         (2, '0', '0', False), (2, '1', '0', False)]
+TRAIN = [(1, '0', '0'), (1, '1', '0'), (1, '0', '1'), (1, '1', '1'), (2, '0', '0'), (2, '1', '0'), (2, '0', '1'), (2, '1', '1')]
 
 
-@pytest.mark.parametrize('nb,overlap,fuse,pair', TRAIN,
-                         ids=['nb%d-overlap%s-fuse%s-%s' % (c[0], c[1], c[2], 'pair' if c[3] else 'nopair') for c in TRAIN])
-def test_rrdbnet_training_float64(backend, monkeypatch, nb, overlap, fuse, pair):
-    """mixed-precision training step; overlap = DASR_B200_BWD_OVERLAP (side-stream filter gradients, checked for
-    ordering), fuse = DASR_B200_FUSE_MASK, pair = engine.PAIR_MODE"""
+@pytest.mark.parametrize('nb,overlap,fuse', TRAIN, ids=['nb%d-overlap%s-fuse%s-pair' % c for c in TRAIN])
+def test_rrdbnet_training_float64(backend, monkeypatch, nb, overlap, fuse):
+    """mixed-precision training step (nf = 64: the dense blocks on the CTA pair); overlap = DASR_B200_BWD_OVERLAP
+    (side-stream filter gradients, checked for ordering), fuse = DASR_B200_FUSE_MASK"""
     monkeypatch.setenv('DASR_B200_BWD_OVERLAP', overlap)
     monkeypatch.setenv('DASR_B200_FUSE_MASK', fuse)
-    monkeypatch.setattr(engine, 'PAIR_MODE', pair)
     t0 = time.time()
     pairs = run_train(nb)
-    _report('train nb=%d overlap=%s fuse=%s pair=%s' % (nb, overlap, fuse, pair), backend, pairs, t0)
+    _report('train nb=%d overlap=%s fuse=%s' % (nb, overlap, fuse), backend, pairs, t0)
     assert (len(backend.streams.all) > 1) == (overlap == '1')
-    assert any(e[0] == 'conv_tc' and 'mask' in e[2] for e in backend.plan) == (fuse == '1' and pair)
+    assert any(e[0] == 'conv_tc' and 'mask' in e[2] for e in backend.plan) == (fuse == '1')
 
 
 def test_rrdbnet_training_nf32_float64(backend):
@@ -724,12 +720,11 @@ def test_de_resnet_bf16_float64(backend):
     assert any('prelu' in p[0] for p in pairs) and any(p[0].startswith('down_sample') for p in pairs)
 
 
-@pytest.mark.parametrize('pair', ['1', '0'])
+@pytest.mark.parametrize('pair', ['1'])       # the convs whose channel counts are multiples of 32 run on the CTA pair
 def test_vgg19_bf16_float64(backend, monkeypatch, pair):
-    monkeypatch.setenv('DASR_B200_VGG_PAIR', pair)
     t0 = time.time()
-    _report('vgg19 pair=%s' % pair, backend, run_vgg(monkeypatch), t0)
-    assert any(e[0] == 'conv_tc' and e[2].get('pair') for e in backend.plan) == (pair == '1')
+    _report('vgg19', backend, run_vgg(monkeypatch), t0)
+    assert any(e[0] == 'conv_tc' and e[2].get('pair') for e in backend.plan)
 
 
 # ------------------------------------------------------------------------------------------------------------------------

@@ -502,10 +502,11 @@ def _trace_consumer_paths(ids=None):
     """the body of test_conv_tc_consumer_paths for the cases `ids` (None: all): prints one line 'TRACE {json}' with the
     mismatches, the cases whose sessions returned no kernel record, and the ping-pong instantiations reached"""
     from torch.profiler import ProfilerActivity, profile
+    from tests.test_gpu_conv_tc_pair_feed import CASES as FEED_CASES
     reached, wrong, empty = set(), [], []
     with profile(activities=[ProfilerActivity.CUDA]):          # the first session of a process starts late: discard it
         _run_exact(CASES[0])
-    for c in CASES:
+    for c in CASES + FEED_CASES:
         if ids is not None and c.id not in ids:
             continue
         inp, wp, bias, out, kw, _ = _make(c)
@@ -526,11 +527,12 @@ def _trace_consumer_paths(ids=None):
 
 
 def test_conv_tc_consumer_paths():
-    """Every case runs the conv_tc_kernel instantiation its declared path implies (ping-pong: NT = the Cout tile of a CTA),
-    and the case matrix reaches every ping-pong instantiation, so a change of the selection rule cannot silently move
-    the coverage of the exact test.  The trace runs in a fresh interpreter, as the other path tests do: profiler sessions
-    can come back without any kernel record, sometimes for one case again and again in the same process, so such cases
-    are traced again in up to two more fresh interpreters before they count as a failure."""
+    """Every case, here and in test_gpu_conv_tc_pair_feed.py, runs the conv_tc_kernel instantiation its declared path
+    implies (ping-pong: NT = the Cout tile of a CTA), and the case matrix reaches every ping-pong instantiation, so a
+    change of the selection rule cannot silently move the coverage of the exact tests.  The trace runs in a fresh
+    interpreter, as the other path tests do: profiler sessions can come back without any kernel record, sometimes for one
+    case again and again in the same process, so such cases are traced again in up to two more fresh interpreters before
+    they count as a failure."""
     ids, reached, wrong = None, set(), []
     for _ in range(3):
         code = 'import sys; sys.path[:0] = [%r, %r]; from tests.test_gpu_conv_tc_exact import _trace_consumer_paths; ' \
