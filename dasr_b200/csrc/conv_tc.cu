@@ -78,12 +78,24 @@ __device__ __forceinline__ uint32_t f2_to_h16x2(float a, float b, int f16) {
   else *reinterpret_cast<__nv_bfloat162*>(&u) = __floats2bfloat162_rn(a, b);
   return u;
 }
-__device__ __forceinline__ uint32_t lds32(uint32_t addr) {
-  uint32_t v;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr));
+__device__ __forceinline__ void sts32(uint32_t addr, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
+__device__ __forceinline__ float2 lds64f(uint32_t addr) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr));
   return v;
 }
-__device__ __forceinline__ void sts32(uint32_t addr, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
+// Four 8x8 16-bit matrices: lane l gives the 16-byte address of row l & 7 of matrix l >> 3, and register k of lane t holds
+// row t / 4, columns 2 (t % 4) and 2 (t % 4) + 1 of matrix k: the layout of a wgmma accumulator's 8x8 sub-tiles.  No
+// "memory" clobber, so that a staged block's loads can all be issued before its math; compiler_fence() bounds them.
+__device__ __forceinline__ void ldsm4(uint32_t addr, uint32_t* r) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
+}
+__device__ __forceinline__ void stsm4(uint32_t addr, const uint32_t* r) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r[0]), "r"(r[1]), "r"(r[2]),
+               "r"(r[3]));
+}
+__device__ __forceinline__ void compiler_fence() { asm volatile("" ::: "memory"); }
 
 // Staged tile layout: nb64 blocks of 64 channels (128 B rows, SWIZZLE_128B), then a 32-channel block (64 B rows,
 // SWIZZLE_64B) if nt & 32, then a 16-channel block (32 B rows, SWIZZLE_32B) if nt & 16.  Byte offset of (pixel m, channel c).
@@ -157,54 +169,84 @@ __device__ __forceinline__ void issue_tap_rt(int nt, float* acc, uint32_t a_addr
   }
 }
 
-// Staged epilogue of one accumulator pair (channels co, co + 1 of tile pixel m; o = their byte offset in the staged tile):
-// pre addend, weight-map channel, activation, scale, res1 (or the dgrad mask carried in its slot), weight-map scale, res2,
+// Staged epilogue of one accumulator pair with a DASR_MAP_CHANNEL weight map, which takes no pre / residual inputs
+// (channels co, co + 1 of a tile pixel; o = their byte offset in the staged tile): weight-map channel, activation, scale,
 // then the bf16 / half pair goes back into the staged tile.  v0, v1 already carry the bias.
-template <bool HAS_PRE, int NRES, int MAP>
-__device__ __forceinline__ void staged_epi_pair(float v0, float v1, int co, uint32_t o, uint32_t bS, uint32_t bR1, uint32_t bR2,
-                                                const float* mv, const DasrConvTcParams& p, const float* map_w, bool mask_mode,
-                                                int f16) {
-  if constexpr (HAS_PRE) {
-    const float2 q = h16x2_to_f2(lds32(bS + o), f16);
-    v0 += q.x; v1 += q.y;
-  }
-  if constexpr (MAP == DASR_MAP_CHANNEL) {
-    const float* wa = map_w + co;
+__device__ __forceinline__ void staged_epi_pair_map_channel(float v0, float v1, int co, uint32_t o, uint32_t bS, const float* mv,
+                                                            const DasrConvTcParams& p, const float* map_w, int f16) {
+  const float* wa = map_w + co;
 #pragma unroll
-    for (int t = 0; t < 9; t++) {
-      v0 = fmaf(mv[t], __ldg(wa + t * p.cout), v0);
-      v1 = fmaf(mv[t], __ldg(wa + t * p.cout + 1), v1);
-    }
+  for (int t = 0; t < 9; t++) {
+    v0 = fmaf(mv[t], __ldg(wa + t * p.cout), v0);
+    v1 = fmaf(mv[t], __ldg(wa + t * p.cout + 1), v1);
   }
   if (p.act != DASR_ACT_NONE && co < p.act_cols) {
     if (p.act == DASR_ACT_LRELU) { v0 = fmaxf(v0, v0 * p.slope); v1 = fmaxf(v1, v1 * p.slope); }   // 0 < slope < 1
     else { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
   }
   v0 *= p.alpha; v1 *= p.alpha;
+  sts32(bS + o, f2_to_h16x2(v0, v1, f16));
+}
+
+// Launch constants of the staged epilogue for the column pairs 8j + c, 8j + c + 1 of the Cout tile (c = this thread's first
+// column): the activation applies to them while 8j < act_lim, the dgrad mask while mask_lo <= 8j < mask_hi.  Made from the
+// kernel parameters at the start of each staged block: per-CTA copies kept through the MMA loop made it spill.
+struct EpiConst {
+  float slope, alpha, beta1, beta2, mask_slope;
+  bool has_bias, lrelu;
+  int act_lim, mask_lo, mask_hi;
+  __device__ __forceinline__ bool act(int j) const { return 8 * j < act_lim; }
+  __device__ __forceinline__ bool mask(int j) const { return 8 * j >= mask_lo && 8 * j < mask_hi; }
+};
+__device__ __forceinline__ EpiConst epi_const(const DasrConvTcParams& p, bool has_bias, bool mask_mode, int c) {
+  return {p.slope, p.alpha, p.beta1, p.beta2, p.mask_slope, has_bias, p.act == DASR_ACT_LRELU,
+          p.act != DASR_ACT_NONE ? p.act_cols - c : 0, mask_mode ? p.mask_c0 - c : 0, mask_mode ? p.mask_c1 - c : 0};
+}
+
+// c ? a : b as one select instruction: a plain ?: on the activation or the mask is compiled into a branch around its math
+__device__ __forceinline__ float select_f32(bool c, float a, float b) {
+  float r;
+  asm("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %3, 0;\n\tselp.f32 %0, %1, %2, p;\n\t}" : "=f"(r) : "f"(a), "f"(b), "r"((uint32_t)c));
+  return r;
+}
+
+// Staged epilogue of one accumulator pair without a weight-map channel, as straight-line code: bias, pre addend,
+// activation, scale, res1 (or the dgrad mask carried in its slot, MASK), weight-map scale (MSCALE: DASR_MAP_SCALE with the
+// pixel's map value ms), res2; returns the packed bf16 / half pair.  The bias pair (b0, b1) and the packed pre / res1 / res2
+// pairs (qp, q1, q2) are already in registers; do_act, do_mask: the activation / the mask applies to this column pair.
+template <bool HAS_PRE, int NRES, bool MASK, bool MSCALE>
+__device__ __forceinline__ uint32_t epi_pair(float v0, float v1, float b0, float b1, uint32_t qp, uint32_t q1, uint32_t q2,
+                                             float ms, bool do_act, bool do_mask, const EpiConst& k, int f16) {
+  if (k.has_bias) { v0 += b0; v1 += b1; }
+  if constexpr (HAS_PRE) {
+    const float2 q = h16x2_to_f2(qp, f16);
+    v0 += q.x; v1 += q.y;
+  }
+  const float t0 = select_f32(k.lrelu, v0 * k.slope, 0.f), t1 = select_f32(k.lrelu, v1 * k.slope, 0.f);   // LeakyReLU or ReLU
+  v0 = select_f32(do_act, fmaxf(v0, t0), v0);
+  v1 = select_f32(do_act, fmaxf(v1, t1), v1);
+  v0 *= k.alpha; v1 *= k.alpha;
   if constexpr (NRES >= 1) {
-    const uint32_t r = lds32(bR1 + o);
-    if (mask_mode) {
-      if (co >= p.mask_c0 && co < p.mask_c1) {    // a positive finite bf16 / half is a positive 16-bit integer
-        if (!((short)(r & 0xFFFF) > 0)) v0 *= p.mask_slope;
-        if (!((short)(r >> 16) > 0)) v1 *= p.mask_slope;
-      }
+    if constexpr (MASK) {      // a positive finite bf16 / half is a positive 16-bit integer
+      v0 = select_f32(do_mask && !((short)(q1 & 0xFFFF) > 0), v0 * k.mask_slope, v0);
+      v1 = select_f32(do_mask && !((short)(q1 >> 16) > 0), v1 * k.mask_slope, v1);
     } else {
-      const float2 q = h16x2_to_f2(r, f16);
-      v0 = fmaf(p.beta1, q.x, v0); v1 = fmaf(p.beta1, q.y, v1);
+      const float2 q = h16x2_to_f2(q1, f16);
+      v0 = fmaf(k.beta1, q.x, v0); v1 = fmaf(k.beta1, q.y, v1);
     }
   }
-  if constexpr (MAP == DASR_MAP_SCALE) { v0 *= mv[0]; v1 *= mv[0]; }
+  if constexpr (MSCALE) { v0 *= ms; v1 *= ms; }
   if constexpr (NRES >= 2) {
-    const float2 q = h16x2_to_f2(lds32(bR2 + o), f16);
-    v0 = fmaf(p.beta2, q.x, v0); v1 = fmaf(p.beta2, q.y, v1);
+    const float2 q = h16x2_to_f2(q2, f16);
+    v0 = fmaf(k.beta2, q.x, v0); v1 = fmaf(k.beta2, q.y, v1);
   }
-  sts32(bS + o, f2_to_h16x2(v0, v1, f16));
+  return f2_to_h16x2(v0, v1, f16);
 }
 
 // Tile-phase trace (only in the selftest_trace build, compiled with -DDASR_TC_TRACE; the library never records):
 // clock64 stamps of the first TRACE_CTAS CTAs (grid row 0, i.e. the leader of a pair) for their first TRACE_TILES local tiles.
 #ifdef DASR_TC_TRACE
-constexpr int TRACE_CTAS = 8, TRACE_TILES = 48, TRACE_EV = 16;
+constexpr int TRACE_CTAS = 8, TRACE_TILES = 48, TRACE_EV = 20;
 __device__ long long* g_tc_trace;
 #define TC_STAMP(lt, ev)                                                                                           \
   do {                                                                                                             \
@@ -217,8 +259,10 @@ __device__ long long* g_tc_trace;
 #endif
 // event slots of one tile: consumer warpgroup g (warp 4g, lane 0) at 5g + {0: first A wait begins, 1: last A wait ends,
 // 2: MMAs retired, 3: pre / sfree wait ends, 4: epilogue done}; producer: 15 empty wait of the first load begins,
-// 10: it ends, 11: last A load issued; epilogue TMA warp: 12 sfull wait ends, 13 stores issued, 14 stores have read the tile.
-enum { TEV_P_EMPTY = 10, TEV_P_ISSUED = 11, TEV_E_SFULL = 12, TEV_E_STORED = 13, TEV_E_READ = 14, TEV_P_EMPTY0 = 15 };
+// 10: it ends, 11: last A load issued; epilogue TMA warp: 12 sfull wait ends, 13 stores issued, 14 stores have read the tile;
+// ping-pong consumer warpgroup g: 16 + 2g staged block 0 written, 17 + 2g the slots of block 1 ready.
+enum { TEV_P_EMPTY = 10, TEV_P_ISSUED = 11, TEV_E_SFULL = 12, TEV_E_STORED = 13, TEV_E_READ = 14, TEV_P_EMPTY0 = 15,
+       TEV_C_BLK0 = 16, TEV_C_BLK1_READY = 17 };
 
 // EPI_MODE / HAS_PRE / NRES are compile-time so that each instantiation carries only its own epilogue code.
 // MAP (staged epilogue only): 0 = no weight map; DASR_MAP_CHANNEL = one more input channel map_scale * map convolved with
@@ -469,6 +513,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
     const int r0 = 16 * wi + (lane >> 2);       // this thread's accumulator rows: r0 and r0 + 8 of the warpgroup's 64
     const int cq = 2 * (lane & 3);              // and columns 8j + cq, 8j + cq + 1
     const bool rec = wi == 0 && lane == 0;      // records this warpgroup's tile-phase stamps (traced build only)
+    const uint32_t sBias_u = smem_u32(sBias);
 
     auto release = [&](int s) {                 // this warp's wgmmas reading stage s have completed
       __syncwarp();
@@ -604,7 +649,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
 
           const int sb = (int)(it % (uint32_t)nbuf);
           const uint32_t sphase = (it / (uint32_t)nbuf) & 1;
-          const uint32_t bS = sS_u + sb * a.epi_bytes, bR1 = sR1_u + sb * a.epi_bytes, bR2 = sR2_u + sb * a.epi_bytes;
+          [[maybe_unused]] const uint32_t bS = sS_u + sb * a.epi_bytes, bR1 = sR1_u + sb * a.epi_bytes, bR2 = sR2_u + sb * a.epi_bytes;
           // one staged block at a time (64-channel blocks, then the 32- / 16-channel tail): wait for its slots, write it,
           // hand it to the epilogue TMA warp, which can store it while the next block is written
           auto epi_block = [&](auto i_c) {
@@ -615,24 +660,52 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
             if (has_loads) mbar_wait(&pre_bar[bi], sphase);
             else if (it >= (uint32_t)nbuf) mbar_wait(&sfree_bar[bi], sphase ^ 1);
             if (rec && i == 0) TC_STAMP(it, 5 * wg + 3);
+            if (rec && i == 1) TC_STAMP(it, TEV_C_BLK1_READY + 2 * wg);
+            compiler_fence();
+            // Column groups j of the block in batches of JB: every bias / pre / residual load of a batch, then its math, then
+            // its stores.  Sub-tile (blk = k >> 1, h = k & 1, j) is matrix k of one ldmatrix / stmatrix, so each lane addresses
+            // row lm of the warpgroup's tile.  pre is read and overwritten in place in sS, but each element only by the lane
+            // that holds it, and its store depends on the value loaded, so no other ordering is needed.
+            auto body = [&](auto mask_c) {
+              constexpr bool MASK = decltype(mask_c)::value;
+              constexpr int NLD = (HAS_PRE ? 1 : 0) + NRES, JBLK = (c1 - c0) / 8;
+              constexpr int JREGS = 4 * NLD + 2;                              // registers loaded per column group
+              constexpr int JB = JBLK * JREGS <= 32 ? JBLK : (JBLK * JREGS <= 64 ? JBLK / 2 : 2);   // <= 32 per batch
+              const int lm = 64 * (lane >> 4) + 16 * wi + 8 * ((lane >> 3) & 1) + (lane & 7);
+              const EpiConst ek = epi_const(p, has_bias, mask_mode, co_base + cq);
 #pragma unroll
-            for (int blk = 0; blk < 2; blk++) {
+              for (int jb = c0 / 8; jb < c1 / 8; jb += JB) {
+                uint32_t qp[JB][4] = {}, q1[JB][4] = {}, q2[JB][4] = {}, r[JB][4];
+                float2 b[JB];
 #pragma unroll
-              for (int h = 0; h < 2; h++) {
-                const int m = 64 * blk + r0 + 8 * h;
-#pragma unroll
-                for (int j = c0 / 8; j < c1 / 8; j++) {
-                  const int cl = 8 * j + cq;
-                  float v0 = acc[blk * (NT / 2) + 4 * j + 2 * h], v1 = acc[blk * (NT / 2) + 4 * j + 2 * h + 1];
-                  if (has_bias) { v0 += sBias[cl]; v1 += sBias[cl + 1]; }
-                  staged_epi_pair<HAS_PRE, NRES, 0>(v0, v1, co_base + cl, staged_off(m, cl, NB64, T32), bS, bR1, bR2, nullptr,
-                                                    p, nullptr, mask_mode, F16);
+                for (int jj = 0; jj < JB; jj++) {
+                  const uint32_t o = staged_off(lm, 8 * (jb + jj), NB64, T32);
+                  b[jj] = lds64f(sBias_u + 4u * (uint32_t)(8 * (jb + jj) + cq));
+                  if constexpr (HAS_PRE) ldsm4(bS + o, qp[jj]);
+                  if constexpr (NRES >= 1) ldsm4(bR1 + o, q1[jj]);
+                  if constexpr (NRES >= 2) ldsm4(bR2 + o, q2[jj]);
                 }
+#pragma unroll
+                for (int jj = 0; jj < JB; jj++) {
+                  const int j = jb + jj;
+#pragma unroll
+                  for (int k = 0; k < 4; k++) {
+                    const float* v = acc + (k >> 1) * (NT / 2) + 4 * j + 2 * (k & 1);
+                    r[jj][k] = epi_pair<HAS_PRE, NRES, MASK, false>(v[0], v[1], b[jj].x, b[jj].y, qp[jj][k], q1[jj][k], q2[jj][k], 1.f,
+                                                                    ek.act(j), ek.mask(j), ek, F16);
+                  }
+                }
+#pragma unroll
+                for (int jj = 0; jj < JB; jj++) stsm4(bS + staged_off(lm, 8 * (jb + jj), NB64, T32), r[jj]);
               }
-            }
+            };
+            if (NRES >= 1 && mask_mode) body(std::true_type());
+            else body(std::false_type());
+            compiler_fence();
             fence_proxy_async();
             __syncwarp();
             if (lane == 0) mbar_arrive(&sfull_bar[bi]);
+            if (rec && i == 0) TC_STAMP(it, TEV_C_BLK0 + 2 * wg);
           };
           epi_block(std::integral_constant<int, 0>());
           if constexpr (NBLK > 1) epi_block(std::integral_constant<int, 1>());
@@ -698,65 +771,106 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
           else if (it >= (uint32_t)nbuf) mbar_wait(&sfree_bar[bi], sphase ^ 1); // stores of tile it-nbuf have read the frame
           if (rec) TC_STAMP(it, 5 * wg + 3);
         }
+        if constexpr (EPI_MODE == 0 && MAP != DASR_MAP_CHANNEL) {
+          compiler_fence();
+          // Column groups j, j + 1 at a time: sub-tile (h = k & 1, j + (k >> 1)) is matrix k of one ldmatrix / stmatrix, so
+          // lane l addresses row lm of the tile in column group j + (l >> 4).  pre is overwritten in place, each element
+          // only by the lane that loaded it, as on the ping-pong consumers.
+          auto body = [&](auto mask_c) {
+            constexpr bool MASK = decltype(mask_c)::value;
+            const int lm = 64 * wg + 16 * wi + 8 * ((lane >> 3) & 1) + (lane & 7), jo = lane >> 4;
+            const EpiConst ek = epi_const(p, has_bias, mask_mode, co_base + cq);
+            float ms[2] = {1.f, 1.f};                   // DASR_MAP_SCALE: the map at this thread's two pixels
+            if constexpr (MAP == DASR_MAP_SCALE) {
 #pragma unroll
-        for (int h = 0; h < 2; h++) {
-          const int m = 64 * wg + r0 + 8 * h;               // tile pixel
-          const int py = m >> 3, px = m & 7;
-          const int y = y0 + py, x = x0 + px;
-          const bool valid = (y < p.H) && (x < p.W);
-          const int oy = y * p.out_mul + p.out_py[var], ox = x * p.out_mul + p.out_px[var];
-          const long opix = ((long)n * OH + oy) * OW + ox;
-          // the map around this pixel (zero outside the image): the 3x3 neighbourhood, or the pixel's own value
-          float mv[MAP == DASR_MAP_CHANNEL ? 9 : 1];
-          if constexpr (MAP == DASR_MAP_CHANNEL) {
-            const float* mp = a.map + (long)n * p.map_stride;
-#pragma unroll
-            for (int t = 0; t < 9; t++) {
-              const int yy = y + t / 3 - 1, xx = x + t % 3 - 1;
-              mv[t] = (yy >= 0 && yy < p.H && xx >= 0 && xx < p.W) ? p.map_scale * __ldg(mp + (long)yy * p.W + xx) : 0.f;
+              for (int h = 0; h < 2; h++) {
+                const int m = 64 * wg + r0 + 8 * h, y = y0 + (m >> 3), x = x0 + (m & 7);
+                ms[h] = (y < p.H && x < p.W) ? __ldg(a.map + (long)n * p.map_stride + (long)y * p.W + x) : 0.f;
+              }
             }
-          } else if constexpr (MAP == DASR_MAP_SCALE) {
-            mv[0] = valid ? __ldg(a.map + (long)n * p.map_stride + (long)y * p.W + x) : 0.f;
-          }
 #pragma unroll
-          for (int j = 0; j < ACC_REGS / 4; j++) {
-            if (j < (nt >> 3)) {
-              const int cl = 8 * j + cq;                    // channel inside the tile
-              const int co = co_base + cl;
-              float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-              if (has_bias) { v0 += sBias[cl]; v1 += sBias[cl + 1]; }
-              const bool do_act = (act != DASR_ACT_NONE) && (co < p.act_cols);
-              if constexpr (EPI_MODE == 0) {
-                staged_epi_pair<HAS_PRE, NRES, MAP>(v0, v1, co, staged_off(m, cl, nb64, tail32), bS, bR1, bR2, mv, p, a.map_w,
-                                                    mask_mode, f16);
-              } else if (valid) {
-                if (do_act) {
-                  v0 = (act == DASR_ACT_LRELU) ? fmaxf(v0, v0 * slope) : fmaxf(v0, 0.f);
-                  v1 = (act == DASR_ACT_LRELU) ? fmaxf(v1, v1 * slope) : fmaxf(v1, 0.f);
+            for (int j = 0; j < ACC_REGS / 4; j += 2) {
+              if (j < (nt >> 3)) {
+                const uint32_t o = staged_off(lm, 8 * (j + jo), nb64, tail32);
+                uint32_t qp[4] = {}, q1[4] = {}, q2[4] = {}, r[4];
+                if constexpr (HAS_PRE) ldsm4(bS + o, qp);
+                if constexpr (NRES >= 1) ldsm4(bR1 + o, q1);
+                if constexpr (NRES >= 2) ldsm4(bR2 + o, q2);
+                const float2 b[2] = {lds64f(sBias_u + 4u * (uint32_t)(8 * j + cq)), lds64f(sBias_u + 4u * (uint32_t)(8 * j + 8 + cq))};
+#pragma unroll
+                for (int k = 0; k < 4; k++) {
+                  const int jj = j + (k >> 1), h = k & 1;
+                  r[k] = epi_pair<HAS_PRE, NRES, MASK, MAP == DASR_MAP_SCALE>(acc[4 * jj + 2 * h], acc[4 * jj + 2 * h + 1], b[k >> 1].x,
+                                                                            b[k >> 1].y, qp[k], q1[k], q2[k], ms[h], ek.act(jj), ek.mask(jj),
+                                                                            ek, f16);
                 }
-                v0 *= alpha; v1 *= alpha;
-                if constexpr (EPI_MODE == 2) {
-                  // final layer: first out_nc channels straight to NCHW fp32 (the module boundary layout)
-                  float* of = reinterpret_cast<float*>(a.out);
-                  const long plane = (long)OH * OW;
-                  if (co < p.out_nc) of[((long)n * p.out_nc + co) * plane + (long)oy * OW + ox] = v0;
-                  if (co + 1 < p.out_nc) of[((long)n * p.out_nc + co + 1) * plane + (long)oy * OW + ox] = v1;
-                } else {
-                  if (a.res1) {
-                    const float2 q = h16x2_to_f2(__ldg(reinterpret_cast<const unsigned int*>(a.res1 + opix * p.res1_cs + p.res1_coff + co)), f16);
-                    v0 = fmaf(p.beta1, q.x, v0); v1 = fmaf(p.beta1, q.y, v1);
+                stsm4(bS + o, r);
+              }
+            }
+          };
+          if (NRES >= 1 && mask_mode) body(std::true_type());
+          else body(std::false_type());
+          compiler_fence();
+        } else {
+#pragma unroll
+          for (int h = 0; h < 2; h++) {
+            const int m = 64 * wg + r0 + 8 * h;               // tile pixel
+            const int py = m >> 3, px = m & 7;
+            const int y = y0 + py, x = x0 + px;
+            const bool valid = (y < p.H) && (x < p.W);
+            const int oy = y * p.out_mul + p.out_py[var], ox = x * p.out_mul + p.out_px[var];
+            const long opix = ((long)n * OH + oy) * OW + ox;
+            // the map around this pixel (zero outside the image): the 3x3 neighbourhood, or the pixel's own value
+            float mv[MAP == DASR_MAP_CHANNEL ? 9 : 1];
+            if constexpr (MAP == DASR_MAP_CHANNEL) {
+              const float* mp = a.map + (long)n * p.map_stride;
+#pragma unroll
+              for (int t = 0; t < 9; t++) {
+                const int yy = y + t / 3 - 1, xx = x + t % 3 - 1;
+                mv[t] = (yy >= 0 && yy < p.H && xx >= 0 && xx < p.W) ? p.map_scale * __ldg(mp + (long)yy * p.W + xx) : 0.f;
+              }
+            } else if constexpr (MAP == DASR_MAP_SCALE) {
+              mv[0] = valid ? __ldg(a.map + (long)n * p.map_stride + (long)y * p.W + x) : 0.f;
+            }
+#pragma unroll
+            for (int j = 0; j < ACC_REGS / 4; j++) {
+              if (j < (nt >> 3)) {
+                const int cl = 8 * j + cq;                    // channel inside the tile
+                const int co = co_base + cl;
+                float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+                if (has_bias) { v0 += sBias[cl]; v1 += sBias[cl + 1]; }
+                const bool do_act = (act != DASR_ACT_NONE) && (co < p.act_cols);
+                if constexpr (EPI_MODE == 0) {
+                  staged_epi_pair_map_channel(v0, v1, co, staged_off(m, cl, nb64, tail32), bS, mv, p, a.map_w, f16);
+                } else if (valid) {
+                  if (do_act) {
+                    v0 = (act == DASR_ACT_LRELU) ? fmaxf(v0, v0 * slope) : fmaxf(v0, 0.f);
+                    v1 = (act == DASR_ACT_LRELU) ? fmaxf(v1, v1 * slope) : fmaxf(v1, 0.f);
                   }
-                  if (a.res2) {
-                    const float2 q = h16x2_to_f2(__ldg(reinterpret_cast<const unsigned int*>(a.res2 + opix * p.res2_cs + p.res2_coff + co)), f16);
-                    v0 = fmaf(p.beta2, q.x, v0); v1 = fmaf(p.beta2, q.y, v1);
+                  v0 *= alpha; v1 *= alpha;
+                  if constexpr (EPI_MODE == 2) {
+                    // final layer: first out_nc channels straight to NCHW fp32 (the module boundary layout)
+                    float* of = reinterpret_cast<float*>(a.out);
+                    const long plane = (long)OH * OW;
+                    if (co < p.out_nc) of[((long)n * p.out_nc + co) * plane + (long)oy * OW + ox] = v0;
+                    if (co + 1 < p.out_nc) of[((long)n * p.out_nc + co + 1) * plane + (long)oy * OW + ox] = v1;
+                  } else {
+                    if (a.res1) {
+                      const float2 q = h16x2_to_f2(__ldg(reinterpret_cast<const unsigned int*>(a.res1 + opix * p.res1_cs + p.res1_coff + co)), f16);
+                      v0 = fmaf(p.beta1, q.x, v0); v1 = fmaf(p.beta1, q.y, v1);
+                    }
+                    if (a.res2) {
+                      const float2 q = h16x2_to_f2(__ldg(reinterpret_cast<const unsigned int*>(a.res2 + opix * p.res2_cs + p.res2_coff + co)), f16);
+                      v0 = fmaf(p.beta2, q.x, v0); v1 = fmaf(p.beta2, q.y, v1);
+                    }
+                    if (a.mask_src) {
+                      const __nv_bfloat16* mp = a.mask_src + opix * p.mask_cs + p.mask_coff + (co - p.mask_c0);
+                      if (co >= p.mask_c0 && co < p.mask_c1 && !(__bfloat162float(mp[0]) > 0.f)) v0 *= p.mask_slope;
+                      if (co + 1 >= p.mask_c0 && co + 1 < p.mask_c1 && !(__bfloat162float(mp[1]) > 0.f)) v1 *= p.mask_slope;
+                    }
+                    __nv_bfloat16* ob16 = reinterpret_cast<__nv_bfloat16*>(a.out);
+                    *reinterpret_cast<uint32_t*>(ob16 + opix * p.out_cs + p.out_coff + co) = f2_to_h16x2(v0, v1, f16);
                   }
-                  if (a.mask_src) {
-                    const __nv_bfloat16* mp = a.mask_src + opix * p.mask_cs + p.mask_coff + (co - p.mask_c0);
-                    if (co >= p.mask_c0 && co < p.mask_c1 && !(__bfloat162float(mp[0]) > 0.f)) v0 *= p.mask_slope;
-                    if (co + 1 >= p.mask_c0 && co + 1 < p.mask_c1 && !(__bfloat162float(mp[1]) > 0.f)) v1 *= p.mask_slope;
-                  }
-                  __nv_bfloat16* ob16 = reinterpret_cast<__nv_bfloat16*>(a.out);
-                  *reinterpret_cast<uint32_t*>(ob16 + opix * p.out_cs + p.out_coff + co) = f2_to_h16x2(v0, v1, f16);
                 }
               }
             }

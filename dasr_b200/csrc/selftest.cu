@@ -560,7 +560,7 @@ static void trace_rdb(int coop) {
   printf("trace (%s consumers): median per tile, us; first %d CTAs (leader of each pair), tiles 2..%d\n",
          coop ? "cooperative" : "ping-pong", ctas, tiles - 1);
   printf("launch  K   N  us/launch us/tile | A-wait  MMA  epi-in-wait epilogue busy  period | prod: empty-wait issue-gap | "
-         "epi-TMA: sfull-lag store-issue read\n");
+         "epi-TMA: sfull-lag store-issue read | ping-pong blocks: blk0-math blk1-wait blk1-math\n");
   for (int li = 0; li < 5; li++) {
     const Launch& L = ls[li];
     std::vector<float> w((size_t)L.cout * L.cin * 9);
@@ -611,7 +611,7 @@ static void trace_rdb(int coop) {
     dasr_tc_trace_attach(nullptr, coop, &ctas, &tiles, &nev);
     std::vector<long long> tr((size_t)ctas * tiles * nev);
     CK(cudaMemcpy(tr.data(), dtr, tr.size() * 8, cudaMemcpyDeviceToHost));
-    std::vector<double> ph[11];
+    std::vector<double> ph[14];
     for (int c = 0; c < ctas; c++) {
       auto ev = [&](int t, int e) { return tr[((size_t)c * tiles + t) * nev + e]; };
       auto cons = [&](int t, int e) { return ev(t, 4) ? ev(t, e) : ev(t, 5 + e); };   // whichever warpgroup ran tile t
@@ -624,15 +624,24 @@ static void trace_rdb(int coop) {
                               (double)(ev(t, 12) - cons(t, 4)),  (double)(ev(t, 13) - ev(t, 12)),
                               (double)(ev(t, 14) - ev(t, 13))};
         for (int k = 0; k < 11; k++) ph[k].push_back(v[k] / cyc_per_us);
+        // ping-pong staged blocks (events 16 + 2g: block 0 written, 17 + 2g: block 1's slots ready; g = the warpgroup)
+        const int g = ev(t, 4) ? 0 : 1;
+        const long long b0 = ev(t, 16 + 2 * g), b1 = ev(t, 17 + 2 * g);
+        if (b0) ph[11].push_back((b0 - cons(t, 3)) / cyc_per_us);
+        if (b0 && b1) {
+          ph[12].push_back((b1 - b0) / cyc_per_us);
+          ph[13].push_back((cons(t, 4) - b1) / cyc_per_us);
+        }
       }
     }
     int sms = 0;
     CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0));
     const double tiles_per_cta = (double)N * (H / 16) * (W / 8) / (sms / 2);
-    printf("  %d   %3d %3d  %8.1f %6.2f  | %6.2f %5.2f %6.2f %9.2f %6.2f %6.2f | %6.2f %9.2f          | %6.2f %9.2f %6.2f\n",
+    printf("  %d   %3d %3d  %8.1f %6.2f  | %6.2f %5.2f %6.2f %9.2f %6.2f %6.2f | %6.2f %9.2f          | %6.2f %9.2f %6.2f |"
+           " %9.2f %9.2f %9.2f\n",
            li + 1, L.cin, L.cout, ms * 1e3, ms * 1e3 / tiles_per_cta, median(ph[0]), median(ph[1]), median(ph[2]),
            median(ph[3]), median(ph[4]), median(ph[5]), median(ph[6]), median(ph[7]), median(ph[8]), median(ph[9]),
-           median(ph[10]));
+           median(ph[10]), median(ph[11]), median(ph[12]), median(ph[13]));
     cudaFree(dw); cudaFree(dwp); cudaFree(bias);
   }
   cudaFree(dtr); cudaFree(b); cudaFree(dst); cudaFree(rin);
