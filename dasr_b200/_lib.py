@@ -125,6 +125,12 @@ SYMBOLS = {
     'dasr_sigmoid_bwd': (_i, [_vp, _vp, _vp, _l, _vp]),
 }
 
+# engine-internal entry points: exported by the library for the Python engines, not part of the public C ABI of
+# include/dasr_b200.h (the SRResNet mixed-precision backward's pixel-shuffle + ReLU gradient)
+INTERNAL_SYMBOLS = {
+    'dasr_pixel_unshuffle_mask_bf16': (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),
+}
+
 
 def load():
     """Load the shared library (once).  Raises DasrError if it has not been built."""
@@ -135,7 +141,7 @@ def load():
         raise DasrError('dasr_b200: %s not found — build it first (python -c "import __graft_entry__ as g; g.build()"). '
                         'There is no fallback path.' % LIB_PATH)
     lib = C.CDLL(LIB_PATH)
-    for name, (res, args) in SYMBOLS.items():
+    for name, (res, args) in list(SYMBOLS.items()) + list(INTERNAL_SYMBOLS.items()):
         fn = getattr(lib, name)  # AttributeError if the header and the library disagree
         fn.restype = res
         fn.argtypes = args

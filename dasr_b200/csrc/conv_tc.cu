@@ -270,7 +270,11 @@ enum { TEV_P_EMPTY = 10, TEV_P_ISSUED = 11, TEV_E_SFULL = 12, TEV_E_STORED = 13,
 // NT: 0 = cooperative consumers (both warpgroups on every tile, one 64-pixel half each; Cout tile p.nt at run time);
 // NT > 0 = ping-pong consumers for the staged epilogue without a map: warpgroup (it & 1) owns local tile it whole, the Cout
 // tile is NT and the tap loop (NTAPS taps) is unrolled, so one warpgroup's epilogue overlaps the other's MMAs.
-template <int EPI_MODE, bool HAS_PRE, int NRES, int MAP = 0, int NT = 0, int NTAPS = 9>
+// PS: 3x3 conv followed by PixelShuffle(2) (dasr_conv_tc_setup kind 4, filter rows packed parity-major): the Cout tiles of
+// parity b = 2i + j store through parity b's strided output map, into channels [out_coff, out_coff + cout / 4) of the
+// 2H x 2W tensor.  Only the bias index (the bias stays in the conv's channel order) and the epilogue TMA warp's choice of
+// map and column differ from a plain conv.
+template <int EPI_MODE, bool HAS_PRE, int NRES, int MAP = 0, int NT = 0, int NTAPS = 9, bool PS = false>
 __global__ void __launch_bounds__(TCK_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ CUtensorMap tmap_w,
                const __grid_constant__ EpiMaps em, const TcKernelArgs a) {
@@ -329,7 +333,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
       sTap[t] = (p.a_mode == 0) ? (uint32_t)(p.tap_dy[var][tt] * HALO_W + p.tap_dx[var][tt]) * a_row : (uint32_t)(tt * A_TAP_BYTES);
     }
   }
-  for (int i = threadIdx.x; i < nt; i += TCK_THREADS) sBias[i] = a.bias ? a.bias[ntile * nt + i] : 0.f;
+  for (int i = threadIdx.x; i < nt; i += TCK_THREADS) {
+    int bi = ntile * nt + i;
+    if constexpr (PS) bi = (bi % (p.cout >> 2)) * 4 + bi / (p.cout >> 2);   // packed row b * cout / 4 + c: conv channel 4c + b
+    sBias[i] = a.bias ? a.bias[bi] : 0.f;
+  }
   __syncthreads();
   if (pair) cluster_sync();              // both CTAs' barriers initialised before any multicast or remote arrive
   pdl_launch_dependents();               // the next launch may start its prologue on SMs this grid has left
@@ -393,8 +401,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
     // warpgroup has written it and its slots return (next pre / residual loads, or sfree) as soon as that store has read
     // them; the other frames have one barrier per tile.
     if constexpr (EPI_MODE == 0) {
-      const int co_base = p.out_coff + ntile * nt;
-      const int omap = (p.out_mul == 2) ? 3 * var : 0;      // sub-pixel variants: one strided output map triple per parity
+      int par = var, cb_out = ntile * nt;
+      if constexpr (PS) {                                   // n_ntiles / 4 Cout tiles per parity, parity-major
+        const int tpp = a.n_ntiles >> 2;
+        par = ntile / tpp;
+        cb_out = (ntile - par * tpp) * nt;
+      }
+      const int co_base = p.out_coff + cb_out;
+      const int omap = (p.out_mul == 2) ? 3 * par : 0;      // sub-pixel variants: one strided output map triple per parity
       const int nload = (HAS_PRE ? 1 : 0) + NRES;
       const int unit = NT > 0 ? 1 : nblocks;   // blocks per store unit
       auto bar_of = [&](int f, int i) { return f * FRAME_BLKS + (NT > 0 ? i : 0); };
@@ -941,6 +955,23 @@ __global__ void pack_filter_tc_kernel(const float* __restrict__ w, unsigned shor
   o[i] = f16 ? __half_as_ushort(__float2half_rn(v)) : __bfloat16_as_ushort(__float2bfloat16(v));
 }
 
+// kind 4: 3x3 conv followed by PixelShuffle(2): kind 0's layout with the filter rows in parity-major order, packed row
+// b * (cout / 4) + c <- OIHW row 4c + b (b = 2i + j, the sub-pixel (i, j) that output channel c of the shuffle takes it from)
+__global__ void pack_filter_tc_ps_kernel(const float* __restrict__ w, unsigned short* __restrict__ o, int cout, int cin, int f16) {
+  const int nchunks = cin / CHUNK, q = cout >> 2;
+  const long total = 9L * nchunks * cout * CHUNK;
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const int kc = (int)(i % CHUNK);
+  long r = i / CHUNK;
+  const int nn = (int)(r % cout); r /= cout;
+  const int c = (int)(r % nchunks);
+  const int tap = (int)(r / nchunks);
+  const int src = (nn % q) * 4 + nn / q;
+  const float v = w[((long)src * cin + c * CHUNK + kc) * 9 + tap];
+  o[i] = f16 ? __half_as_ushort(__float2half_rn(v)) : __bfloat16_as_ushort(__float2bfloat16(v));
+}
+
 // Batched form: one launch re-packs every filter of a network from a device-resident job table (training re-packs
 // all filters every step; ~850 tiny launches per generator step otherwise).  A job reads input channels
 // [ci_lo, ci_lo + ci_n) of an OIHW fp32 filter (zero beyond its real extents) and writes rows
@@ -1068,6 +1099,18 @@ int dasr_conv_tc_setup(DasrConvTcParams* p, int kind) {
         p->tap_dx[v][t] = (int8_t)(px + (t & 1));
       }
     }
+  } else if (kind == 4) {      // 3x3 conv + PixelShuffle(2): plain taps, Cout tile b of 4 stores to output parity b
+    p->nvar = 1;
+    p->ntaps = 9;
+    p->out_mul = 2;
+    for (int t = 0; t < 9; t++) {
+      p->tap_dy[0][t] = (int8_t)(t / 3);
+      p->tap_dx[0][t] = (int8_t)(t % 3);
+    }
+    for (int b = 0; b < 4; b++) {
+      p->out_py[b] = b >> 1;
+      p->out_px[b] = b & 1;
+    }
   } else if (kind == 3) {      // last layer with the taps folded into GEMM-N (epi_mode 3): one plain pass over the halo tile
     p->nvar = 1;
     p->ntaps = 1;
@@ -1090,11 +1133,16 @@ size_t dasr_pack_filter_tc_bytes(int cout, int cin, int kind) {
 int dasr_pack_filter_tc(const float* w, void* o, int cout, int cin, int kind, void* stream) {
   const int f16 = (kind & DASR_TC_PACK_F16) != 0;      // IEEE half instead of bf16 (inference precision 'fp16')
   kind &= ~DASR_TC_PACK_F16;
-  DASR_REQUIRE(kind >= 0 && kind <= 3, "pack_filter_tc: kind");
+  DASR_REQUIRE(kind >= 0 && kind <= 4, "pack_filter_tc: kind");
   DASR_REQUIRE(kind != 3 || (cout >= 1 && 9 * cout <= 32), "pack_filter_tc: kind 3 (taps in N) needs cout <= 3");
+  DASR_REQUIRE(kind != 4 || (cout >= 4 && cout % 4 == 0), "pack_filter_tc: kind 4 (pixel shuffle) needs cout %% 4 == 0");
   int gk = (kind == 1) ? cout : cin;
   DASR_REQUIRE(gk % CHUNK == 0, "pack_filter_tc: contraction channels (%d) must be a multiple of 32", gk);
   long total = (long)dasr_pack_filter_tc_bytes(cout, cin, kind) / 2;
+  if (kind == 4) {
+    pack_filter_tc_ps_kernel<<<cdiv(total, 256), 256, 0, (cudaStream_t)stream>>>(w, (unsigned short*)o, cout, cin, f16);
+    return check_launch("pack_filter_tc");
+  }
   pack_filter_tc_kernel<<<cdiv(total, 256), 256, 0, (cudaStream_t)stream>>>(w, (unsigned short*)o, cout, cin, kind, f16);
   return check_launch("pack_filter_tc");
 }
@@ -1243,6 +1291,14 @@ static int conv_tc_launch(const void* in, const void* w, const float* bias, cons
 #ifdef DASR_TC_TRACE
   if (g_trace_coop) pp = -1;
 #endif
+  // 3x3 conv + PixelShuffle(2) (setup kind 4): its own instantiations, on the ping-pong consumers with Cout tiles of 32 / 64
+  const bool ps = p->out_mul == 2 && p->nvar == 1;
+  static const KernelFn ps_kernels[2] = {conv_tc_kernel<0, false, 0, 0, 32, 9, true>, conv_tc_kernel<0, false, 0, 0, 64, 9, true>};
+  const int psi = !ps ? -1 : (pp == 1 ? 0 : pp == 2 ? 1 : -1);
+  if (ps && psi < 0) {
+    set_error("conv_tc: the pixel-shuffle conv needs a Cout tile of 32 or 64 and two staging frames (nt=%d, nbuf=%d)", p->nt, nbuf);
+    return DASR_E_SMEM;
+  }
 
   // Pair on the ping-pong consumers: 64-channel A loads (half the TMA requests per byte) for a contiguous slice of 64k
   // channels or a chunk list of 64-channel runs, issued half-major (chunk64 = 2), so the products and their order stay
@@ -1304,8 +1360,9 @@ static int conv_tc_launch(const void* in, const void* w, const float* bias, cons
     const int used[4] = {1, a.has_pre, a.has_res1, a.has_res2};
     const char* names[4] = {"output", "pre", "res1", "res2"};
     if (p->out_mul == 2) {
-      // one output map triple per parity variant (slots 3v..3v+2; no pre / residual maps in this mode)
-      for (int v = 0; v < p->nvar && v < 4; v++) {
+      // one output map triple per parity variant, or per parity of the pixel shuffle (slots 3v..3v+2; no pre / residual
+      // maps in this mode)
+      for (int v = 0; v < (ps ? 4 : p->nvar) && v < 4; v++) {
         const char* vb = (const char*)out + ((size_t)p->out_py[v] * (2 * p->W) + p->out_px[v]) * p->out_cs * 2;
         int rc = encode_staged_maps(enc, &em.m[3 * v], vb, p->out_cs, p->nt, p->W, p->H, p->N, "output", 2);
         if (rc) return rc;
@@ -1319,10 +1376,11 @@ static int conv_tc_launch(const void* in, const void* w, const float* bias, cons
     }
   }
 
-  const KernelFn fn = pp >= 0 ? pp_kernels[pp][ki] : kernels[ki];
+  const KernelFn fn = psi >= 0 ? ps_kernels[psi] : pp >= 0 ? pp_kernels[pp][ki] : kernels[ki];
   static bool attr_set[12] = {false, false, false, false, false, false, false, false, false, false, false, false};
   static bool attr_set_pp[5][6] = {};
-  bool& attr = pp >= 0 ? attr_set_pp[pp][ki] : attr_set[ki];
+  static bool attr_set_ps[2] = {};
+  bool& attr = psi >= 0 ? attr_set_ps[psi] : pp >= 0 ? attr_set_pp[pp][ki] : attr_set[ki];
   if (!attr) {
     cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
     if (e != cudaSuccess) {
@@ -1388,6 +1446,13 @@ static int conv_tc_run(const void* in, const void* w, const float* bias, const v
     DASR_REQUIRE(p->out_nc >= 1 && 9 * p->out_nc <= 32 && p->nt == 32 && p->cout == 32 && p->ntaps == 1 && p->nvar == 1 &&
                      p->a_mode == 0 && p->out_mul == 1 && !res1 && !res2 && !pre && !mask_src && !p->tile_rev,
                  "conv_tc: epi_mode 3 (taps in N, NCHW fp32 out) needs dasr_conv_tc_setup kind 3, out_nc <= 3, nt = cout = 32");
+  } else if (p->out_mul == 2 && p->nvar == 1) {
+    // 3x3 conv + PixelShuffle(2): cout = 4 x the shuffled channels; Cout tile t stores parity t / (cout / 4 / nt)
+    DASR_REQUIRE(p->epi_mode == 0 && p->ntaps == 9 && p->a_mode == 0 && p->cout % 4 == 0 && (p->nt == 32 || p->nt == 64) &&
+                     (p->cout / 4) % p->nt == 0 && !pre && !res1 && !res2 && !mask_src,
+                 "conv_tc: the pixel-shuffle conv (setup kind 4) needs the staged epilogue, nt 32 or 64 dividing cout / 4 (nt=%d "
+                 "cout=%d) and no pre / residual / mask inputs", p->nt, p->cout);
+    DASR_REQUIRE(p->out_cs % 8 == 0 && p->out_coff % 8 == 0 && p->out_coff + p->cout / 4 <= p->out_cs, "conv_tc: output slice");
   } else {
     DASR_REQUIRE(p->out_cs % 8 == 0 && p->out_coff % 8 == 0 && p->out_coff + p->cout <= p->out_cs, "conv_tc: output slice");
   }

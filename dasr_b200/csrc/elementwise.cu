@@ -123,6 +123,43 @@ __global__ void act_bwd_bf16x8_kernel(__nv_bfloat16* __restrict__ g, const __nv_
   }
   *gp = f_to_bf8(gf);
 }
+// backward of nn.PixelShuffle(2) + ReLU on bf16 NHWC: g_lr[n, h, w, 4c + 2i + j] = g_hr[n, 2h + i, 2w + j, c] * (y_hr[...] > 0)
+// (y_hr nullable: no mask).  One thread: channels [8k, 8k + 8) of the four high-resolution pixels of (n, h, w) in, low-
+// resolution channels [32k, 32k + 32) out, 16-byte loads and stores.  The mask multiplies in fp32 (exact: by 1 or 0).
+__global__ void pixel_unshuffle_mask_bf16x8_kernel(const __nv_bfloat16* __restrict__ g, const __nv_bfloat16* __restrict__ y,
+                                                   __nv_bfloat16* __restrict__ o, long npix, int H, int W, int C8) {
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");      // see act_bwd_bf16x8_kernel
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= npix * C8) return;
+  const long pix = i / C8;
+  const int k = (int)(i - pix * C8);
+  const int w = (int)(pix % W);
+  const long r = pix / W;
+  const int h = (int)(r % H);
+  const long n = r / H;
+  const int C = 8 * C8;
+  float v[4][8];
+#pragma unroll
+  for (int b = 0; b < 4; b++) {
+    const long hp = (n * 2 * H + 2 * h + (b >> 1)) * (2L * W) + 2 * w + (b & 1);
+    bf8_to_f(*reinterpret_cast<const uint4*>(g + hp * C + 8 * k), v[b]);
+    if (y) {
+      float yf[8];
+      bf8_to_f(*reinterpret_cast<const uint4*>(y + hp * C + 8 * k), yf);
+#pragma unroll
+      for (int m = 0; m < 8; m++) v[b][m] *= (yf[m] > 0.f) ? 1.f : 0.f;
+    }
+  }
+  uint4* op = reinterpret_cast<uint4*>(o + pix * 4 * C + 32 * k);
+#pragma unroll
+  for (int q = 0; q < 4; q++) {          // output channels 32k + 8q + e = 4 (8k + m) + b with m = 2q + e / 4, b = e % 4
+    float f[8];
+#pragma unroll
+    for (int e = 0; e < 8; e++) f[e] = v[e & 3][2 * q + (e >> 2)];
+    op[q] = f_to_bf8(f);
+  }
+}
 __global__ void axpby_bf16x8_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ y,
                                     __nv_bfloat16* __restrict__ d, long npix, int C8, int x_cs, int x_coff, int y_cs,
                                     int y_coff, int d_cs, int d_coff, float a, float b) {
@@ -811,6 +848,20 @@ int dasr_upsample2x_bwd(const void* src, void* dst, int N, int H, int W, int C, 
     upsample2x_bwd_kernel<float><<<cdiv(total, 256), 256, 0, (cudaStream_t)stream>>>(
         (const float*)src, (float*)dst, N, H, W, C, src_cs, src_coff, dst_cs, dst_coff);
   return check_launch("upsample2x_bwd");
+}
+
+// Engine-internal entry point (bound by dasr_b200/_lib.py's INTERNAL_SYMBOLS, not declared in include/dasr_b200.h):
+// backward of nn.PixelShuffle(2) followed by ReLU on bf16 NHWC (contiguous, C % 8 == 0, 16-byte aligned):
+//   g_lr[n, h, w, 4c + 2i + j] = g_hr[n, 2h + i, 2w + j, c] * (y_hr[n, 2h + i, 2w + j, c] > 0)
+// H, W are the LOW-resolution dims, C the high-resolution channels (g_lr has 4C).  y_hr NULL: no mask.
+int dasr_pixel_unshuffle_mask_bf16(const void* g_hr, const void* y_hr, void* g_lr, int N, int H, int W, int C, void* stream) {
+  DASR_REQUIRE(N > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0 && g_hr && g_lr, "pixel_unshuffle_mask: bad dims (C %% 8 == 0)");
+  DASR_REQUIRE(aligned(g_hr, 16) && aligned(g_lr, 16) && (!y_hr || aligned(y_hr, 16)),
+               "pixel_unshuffle_mask: tensors must be 16-byte aligned");
+  const long npix = (long)N * H * W;
+  launch_pdl(pixel_unshuffle_mask_bf16x8_kernel, cdiv(npix * (C / 8), 256), 256, (cudaStream_t)stream,
+             (const __nv_bfloat16*)g_hr, (const __nv_bfloat16*)y_hr, (__nv_bfloat16*)g_lr, npix, H, W, C / 8);
+  return check_launch("pixel_unshuffle_mask");
 }
 
 int dasr_upsample2x_fwd(const void* src, void* dst, int N, int H, int W, int C, int src_cs, int src_coff, int dst_cs,

@@ -371,59 +371,15 @@ class _BatchPacker:
     ones seen at construction — i.e. for graph capture right after; replays call launch() from inside the graph)."""
 
     def __init__(self, params, L, nf):
-        from ._lib import PackJob
-        dev = params[0].device
-        self.cache = _PackCache()
-        jobs, keep = [], []
+        self._begin(params)
         W = lambda i: params[2 * i]
         Bv = lambda i: params[2 * i + 1]
-        ver = _PackCache.version
-
-        def add(key, param, kind, rows_total, k_ch, parts, nvar_taps):
-            # parts: [(src param, ci_lo, ci_n, cout_rows, k_pad, row_off)]
-            dst = torch.zeros(nvar_taps * (k_ch // 32) * rows_total * 32, dtype=torch.bfloat16, device=dev)
-            for (src, ci_lo, ci_n, cout_rows, k_pad, row_off) in parts:
-                j = PackJob()
-                j.src, j.dst = src.data_ptr(), dst.data_ptr()
-                j.cout, j.cin, j.kind = src.shape[0], src.shape[1], kind
-                j.ci_lo, j.ci_n, j.cout_rows, j.k_pad = ci_lo, ci_n, cout_rows, k_pad
-                j.dst_rows, j.dst_row_off = rows_total, row_off
-                jobs.append(j)
-            self.cache.d[key] = (ver(param), dst)
-            keep.append(dst)
-
-        def fprop(i, kind=TC_FPROP, cout_to=None, cin_to=None):
-            w = W(i)
-            co, ci = cout_to or w.shape[0], cin_to or w.shape[1]
-            add(('w', i, kind), w, kind, co, ci, [(w, 0, ci, co, 0, 0)], 16 if kind == TC_UPCONV else 9)
-
-        def dgrad(i, cout_to=None):
-            w = W(i)
-            kp = cout_to or w.shape[0]
-            add(('wd', i), w, TC_DGRAD, w.shape[1], kp, [(w, 0, w.shape[1], 0, kp, 0)], 9)
-
-        def bias_alias(i):
-            self.cache.d[('b', i, None)] = (ver(Bv(i)), Bv(i))
-
-        def bias_copy(key, param, src, n):
-            dst = torch.zeros(n, dtype=torch.float32, device=dev)
-            j = PackJob()
-            j.src, j.dst, j.cout, j.kind = src.data_ptr(), dst.data_ptr(), src.shape[0], 3
-            jobs.append(j)
-            self.cache.d[key] = (ver(param), dst)
-            keep.append(dst)
-
-        fprop(L.i_fea, cin_to=32); bias_alias(L.i_fea)
-        fprop(L.i_lr); bias_alias(L.i_lr); dgrad(L.i_lr)
+        self.fprop(L.i_fea, cin_to=32); self.bias_alias(L.i_fea)
+        self.fprop(L.i_lr); self.bias_alias(L.i_lr); self.dgrad(L.i_lr)
         for u in range(L.n_up):
-            fprop(L.i_up0 + u, TC_UPCONV); bias_alias(L.i_up0 + u); dgrad(L.i_up0 + u)
-        fprop(L.i_hr0); bias_alias(L.i_hr0); dgrad(L.i_hr0)
-        if ops.tapn_enabled(W(L.i_hr1).shape[0]):
-            # last layer with the taps in GEMM-N: its 4 KB filter pack (kind 3) is made by the single-filter kernel inside the graph
-            bias_copy(('b', L.i_hr1, 32), Bv(L.i_hr1), Bv(L.i_hr1), 32)
-        else:
-            fprop(L.i_hr1, cout_to=16); bias_copy(('b', L.i_hr1, 16), Bv(L.i_hr1), Bv(L.i_hr1), 16)
-        dgrad(L.i_hr1, cout_to=32)
+            self.fprop(L.i_up0 + u, TC_UPCONV); self.bias_alias(L.i_up0 + u); self.dgrad(L.i_up0 + u)
+        self.fprop(L.i_hr0); self.bias_alias(L.i_hr0); self.dgrad(L.i_hr0)
+        self.last_layer(L.i_hr1)
         for r in range(L.n_rdb):
             # the filter stacks of the training schedule, under the keys _sched_rdb_filters(..., SCHED1, 'f') uses
             for j, (chunks, ks) in enumerate(SCHED1, start=1):
@@ -435,18 +391,96 @@ class _BatchPacker:
                     co = W(L.rdb_conv(r, k)).shape[0]
                     parts.append((W(L.rdb_conv(r, k)), lo, n, co, 0, off))
                     off += co
-                add(('fw', r, j), [W(L.rdb_conv(r, k)) for k in ks], TC_FPROP, off, n, parts, 9)
-                bias_copy(('fb', r, j), Bv(L.rdb_conv(r, j)), Bv(L.rdb_conv(r, j)), off)
-                dgrad(L.rdb_conv(r, j))
-        arr = (PackJob * len(jobs))(*jobs)
+                self.add(('fw', r, j), [W(L.rdb_conv(r, k)) for k in ks], TC_FPROP, off, n, parts, 9)
+                self.bias_copy(('fb', r, j), Bv(L.rdb_conv(r, j)), Bv(L.rdb_conv(r, j)), off)
+                self.dgrad(L.rdb_conv(r, j))
+        self._finish()
+
+    def _begin(self, params):
+        self.params, self.dev = params, params[0].device
+        self.cache = _PackCache()
+        self.jobs, self.keep = [], []
+
+    def _finish(self):
+        from ._lib import PackJob
+        arr = (PackJob * len(self.jobs))(*self.jobs)
         host = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8)
-        self.table = host.to(dev)
-        self.njobs = len(jobs)
-        self.keep = keep
+        self.table = host.to(self.dev)
+        self.njobs = len(self.jobs)
+        del self.jobs, self.params
+
+    def add(self, key, param, kind, rows_total, k_ch, parts, nvar_taps):
+        """one packed tensor under `key`; parts: [(src param, ci_lo, ci_n, cout_rows, k_pad, row_off)], one job each"""
+        from ._lib import PackJob
+        dst = torch.zeros(nvar_taps * (k_ch // 32) * rows_total * 32, dtype=torch.bfloat16, device=self.dev)
+        for (src, ci_lo, ci_n, cout_rows, k_pad, row_off) in parts:
+            j = PackJob()
+            j.src, j.dst = src.data_ptr(), dst.data_ptr()
+            j.cout, j.cin, j.kind = src.shape[0], src.shape[1], kind
+            j.ci_lo, j.ci_n, j.cout_rows, j.k_pad = ci_lo, ci_n, cout_rows, k_pad
+            j.dst_rows, j.dst_row_off = rows_total, row_off
+            self.jobs.append(j)
+        self.cache.d[key] = (_PackCache.version(param), dst)
+        self.keep.append(dst)
+
+    def fprop(self, i, kind=TC_FPROP, cout_to=None, cin_to=None):
+        w = self.params[2 * i]
+        co, ci = cout_to or w.shape[0], cin_to or w.shape[1]
+        self.add(('w', i, kind), w, kind, co, ci, [(w, 0, ci, co, 0, 0)], 16 if kind == TC_UPCONV else 9)
+
+    def dgrad(self, i, cout_to=None):
+        w = self.params[2 * i]
+        kp = cout_to or w.shape[0]
+        self.add(('wd', i), w, TC_DGRAD, w.shape[1], kp, [(w, 0, w.shape[1], 0, kp, 0)], 9)
+
+    def bias_alias(self, i):
+        b = self.params[2 * i + 1]
+        self.cache.d[('b', i, None)] = (_PackCache.version(b), b)
+
+    def bias_copy(self, key, param, src, n):
+        from ._lib import PackJob
+        dst = torch.zeros(n, dtype=torch.float32, device=self.dev)
+        j = PackJob()
+        j.src, j.dst, j.cout, j.kind = src.data_ptr(), dst.data_ptr(), src.shape[0], 3
+        self.jobs.append(j)
+        self.cache.d[key] = (_PackCache.version(param), dst)
+        self.keep.append(dst)
+
+    def last_layer(self, i):
+        """HR_conv1's copies for _last_layer and its dgrad (K padded to 32)"""
+        b = self.params[2 * i + 1]
+        if ops.tapn_enabled(self.params[2 * i].shape[0]):
+            # last layer with the taps in GEMM-N: its 4 KB filter pack (kind 3) is made by the single-filter kernel inside the
+            # captured forward (_TrainGraphs drops the warm-up's copy before capture)
+            self.bias_copy(('b', i, 32), b, b, 32)
+        else:
+            self.fprop(i, cout_to=16); self.bias_copy(('b', i, 16), b, b, 16)
+        self.dgrad(i, cout_to=32)
 
     def launch(self):
         ops.check(ops._lib.load().dasr_pack_filter_tc_batch(ops._p(self.table), self.njobs, 16, ops._stream()),
                   'pack_filter_tc_batch')
+
+
+class _SRResNetPacker(_BatchPacker):
+    """_BatchPacker of one SRResNet training step, under the keys srresnet_forward_bf16_train / srresnet_backward_bf16 use.
+    A pixel-shuffle conv's parity-major pack (ops.TC_PS) is four kind-0 jobs: the OIHW [4C][cin] filter read as
+    [C][4 cin], parity b = input channels [b cin, (b + 1) cin), written to rows [b C, (b + 1) C)."""
+
+    def __init__(self, params, L):
+        self._begin(params)
+        self.fprop(0, cin_to=32); self.bias_alias(0)
+        for i in list(range(1, L.i_up0)) + [L.i_hr0]:          # ResNet block convs, LR_conv, HR_conv0
+            self.fprop(i); self.bias_alias(i); self.dgrad(i)
+        for u in range(L.n_up):
+            i = L.i_up0 + u
+            w = params[2 * i]
+            c, cin = w.shape[0] // 4, w.shape[1]
+            wv = w.view(c, 4 * cin, 3, 3)
+            self.add(('w', i, ops.TC_PS), w, TC_FPROP, 4 * c, cin, [(wv, b * cin, cin, c, 0, b * c) for b in range(4)], 9)
+            self.bias_alias(i); self.dgrad(i)
+        self.last_layer(L.i_hr1)
+        self._finish()
 
 
 def _rdb_stage1(b, w, bias, out, nf, tile_rev=False):
@@ -608,6 +642,232 @@ def rrdb_forward_bf16(x, params, nb, upscale=4, cache=None, per_layer=False, hal
     out, _, _ = _trunk_tail_bf16(bufs, fea, L, params, cache, wk, bk, hk, bf)
     _mark('tc_end')
     return out
+
+
+# ==================================================================================================
+# SRResNet  (architecture.py:18-49; block.py:158-190 ResNetBlock, 838-851 pixelshuffle_block): norm None, CNA, ReLU,
+# pixel-shuffle upsampling.  Flat parameter list [w0, b0, w1, b1, ...] in state_dict order: fea_conv, the two convs of each
+# ResNet block, LR_conv, one conv per pixel-shuffle block, HR_conv0, HR_conv1.
+# ==================================================================================================
+
+class SRResNetLayout:
+    """Conv indices of SRResNet's flat parameter list: fea_conv 0, ResNet block k convs 1 + 2k and 2 + 2k, LR_conv, one conv
+    per pixel-shuffle block, HR_conv0, HR_conv1."""
+
+    def __init__(self, nb, upscale):
+        if upscale not in (2, 4):
+            raise ops._lib.DasrError('SRResNet wgmma path: upscale 2 or 4 (got %s)' % (upscale,))
+        self.nb = nb
+        self.n_up = int(math.log(upscale, 2))
+        self.i_lr = 1 + 2 * nb
+        self.i_up0 = self.i_lr + 1
+        self.i_hr0 = self.i_up0 + self.n_up
+        self.i_hr1 = self.i_hr0 + 1
+        self.n_conv = self.i_hr1 + 1
+
+
+def _ps_nt(nf):
+    """Cout tile of the pixel-shuffle conv (nf -> 4nf; a tile stays inside one output parity): 64 or 32, the largest that
+    divides nf and whose resident filters, staged-epilogue tiles and 4 halo stages fit one SM (as _pick_nt_staged); None if
+    neither does"""
+    for nt in (64, 32):
+        if nf % nt == 0 and _pick_nt_staged(nt, nf) == nt:
+            return nt
+    return None
+
+
+def srresnet_tc_reason(nf):
+    """Why the SRResNet wgmma path (inference and training) cannot run nf feature channels; None if it can.  Every launch
+    needs a Cout tile whose resident filters fit one SM, and the trunk dgrads, which add the skip gradient through `pre`,
+    need a staged-epilogue tile (a multiple of 32): nf 32, 64 and 128 qualify."""
+    if nf % 32:
+        return 'nf %d (the wgmma path needs nf %% 32 == 0)' % nf
+    if _ps_nt(nf) is None:
+        return "nf %d (the pixel-shuffle conv's filters do not fit one SM in Cout tiles of 32)" % nf
+    try:
+        trunk = _pick_nt_staged(nf, nf)
+        _pick_nt_staged(nf, 4 * nf)                   # dgrad of the pixel-shuffle conv
+    except ops._lib.DasrError:
+        return 'nf %d (a dgrad of the training step has no Cout tile whose filters fit one SM)' % nf
+    if trunk % 32:
+        return 'nf %d (the trunk convs would run in Cout tiles of %d; the staged epilogue needs multiples of 32)' % (nf, trunk)
+    return None
+
+
+def _srresnet_forward(x, params, nb, upscale, cache, half, res_scale, save):
+    _need_cuda(x, 'SRResNet')
+    L = SRResNetLayout(nb, upscale)
+    nf = params[0].shape[0]
+    reason = srresnet_tc_reason(nf)
+    if reason:
+        raise ops._lib.DasrError('SRResNet wgmma path cannot run %s' % reason)
+    if len(params) != 2 * L.n_conv:
+        raise ops._lib.DasrError('SRResNet wgmma path: %d parameters are not the %d convs of nb = %d, upscale = %d'
+                                 % (len(params), L.n_conv, nb, upscale))
+    cache = cache if cache is not None else _PackCache()
+    N, in_nc, H, W = x.shape
+    bf = torch.float16 if half else torch.bfloat16
+    hk = 'h' if half else ''
+    wk, bk = _tc_packers(params, cache, hk, bf)
+    nt = _pick_nt_staged(nf, nf)
+    xin = torch.zeros((N, H, W, 32), dtype=bf, device=x.device)       # Cin <= 32 -> one zero-padded 32-channel chunk
+    ops.nchw_to_nhwc(x.contiguous().float(), View(xin, in_nc, 0))
+    fea = _empty((N, H, W, nf), x, bf)
+    _mark('tc_begin')
+    ops.conv_tc(xin, wk(0, cin_to=32), bk(0), fea, nt=nt)
+    # inference: one mid buffer and two alternating block outputs; training keeps every block's mid and output
+    mids, outs = [], []
+    new = lambda: _empty((N, H, W, nf), x, bf)
+    if not save:
+        ring = [new(), new()]
+        mids, outs = [new()] * nb, [ring[k % 2] for k in range(nb + 1)]
+    cur = fea
+    for k in range(nb):
+        mid = mids[k] if not save else new()
+        nxt = outs[k] if not save else new()
+        ops.conv_tc(cur, wk(1 + 2 * k), bk(1 + 2 * k), mid, nt=nt, act=ACT_RELU)
+        ops.conv_tc(mid, wk(2 + 2 * k), bk(2 + 2 * k), nxt, nt=nt, alpha=res_scale, res1=cur, beta1=1.0)
+        if save:
+            mids.append(mid)
+            outs.append(nxt)
+        cur = nxt
+    lr = outs[nb] if not save else new()
+    ops.conv_tc(cur, wk(L.i_lr), bk(L.i_lr), lr, nt=nt, res1=fea, beta1=1.0)
+    if not save:
+        del mids, outs, fea, cur
+    cur, h, w, hrs = lr, H, W, []
+    for u in range(L.n_up):
+        i = L.i_up0 + u
+        h, w = 2 * h, 2 * w
+        hr = _empty((N, h, w, nf), x, bf)
+        ops.conv_tc_ps(cur, wk(i, ops.TC_PS), bk(i), hr, nt=_ps_nt(nf), act=ACT_RELU)
+        if save:
+            hrs.append(hr)
+        cur = hr
+    h0 = _empty((N, h, w, nf), x, bf)
+    ops.conv_tc(cur, wk(L.i_hr0), bk(L.i_hr0), h0, nt=nt, act=ACT_RELU)
+    del cur
+    out_nc = params[2 * L.i_hr1].shape[0]
+    out = _empty((N, out_nc, h, w), x)
+    _last_layer(h0, out, params[2 * L.i_hr1], L.i_hr1, cache, wk, bk, hk, bf)
+    _mark('tc_end')
+    if not save:
+        return out, None
+    return out, dict(L=L, nf=nf, res_scale=res_scale, xin=xin, fea=fea, mids=mids, outs=outs, lr=lr, hrs=hrs, h0=h0,
+                     shape=(N, in_nc, H, W))
+
+
+def srresnet_forward_bf16(x, params, nb, upscale=4, cache=None, half=False, res_scale=1.0):
+    """wgmma forward (inference) of SRResNet (norm None, CNA, ReLU, pixel-shuffle upsampling).  NCHW fp32 in -> NCHW fp32
+    out; bf16 (half: IEEE half) NHWC in between.  A ResNet block is conv + ReLU, then a conv whose epilogue gives
+    res_scale * (acc + bias) + x; LR_conv adds the trunk skip the same way.  A pixelshuffle_block (conv nf -> 4nf,
+    PixelShuffle(2), ReLU) is ONE launch whose epilogue stores each sub-pixel parity of the shuffle through its own strided
+    TMA map (ops.conv_tc_ps), so the 4nf-channel tensor is never written.  Filters are packed once per parameter version
+    (`cache`)."""
+    return _srresnet_forward(x, params, nb, upscale, cache, half, res_scale, save=False)[0]
+
+
+def srresnet_forward_bf16_train(x, params, nb, upscale=4, cache=None, res_scale=1.0):
+    """Forward of the mixed-precision training mode (bf16): the launches of srresnet_forward_bf16, with every activation
+    the backward reads kept (block inputs / ReLU outputs, the pixel-shuffle outputs, HR_conv0's output)."""
+    return _srresnet_forward(x, params, nb, upscale, cache, False, res_scale, save=True)
+
+
+def _dgrad_relu(g, w, out, mask, nf):
+    """dgrad launch whose epilogue applies the ReLU backward of `mask` (the layer's output) to all nf output channels"""
+    nt = ops.pick_nt_pair(ops.as_view(g).c, nf) if nf % 64 == 0 else None
+    if nt:
+        ops.conv_tc(g, w, None, out, kind=TC_DGRAD, pair=True, nt=nt, mask=mask, mask_c0=0, mask_c1=nf, mask_slope=0.0)
+    else:
+        ops.conv_tc(g, w, None, out, kind=TC_DGRAD, nt=_pick_nt(nf, ops.as_view(g).c), mask=mask, mask_c0=0, mask_c1=nf,
+                    mask_slope=0.0)
+
+
+def srresnet_backward_bf16(ctx, params, dout, cache=None, flat=None):
+    """Backward of the mixed-precision SRResNet step: dgrad launches on the wgmma kernel with the ReLU masks in their
+    epilogues and the skip gradients added through `pre` / res1, the pixel-shuffle + ReLU backward as one unshuffle-and-mask
+    kernel (the pixel-shuffle conv's dgrad, filter and bias gradients are then those of a plain conv with 4nf outputs),
+    filter gradients on the wgmma wgrad kernel.  Returns (None, fp32 gradients in parameters() order, the flat fp32 tensor
+    they are views of: [filters in conv order | biases in conv order]).  No input-image gradient."""
+    L, nf, rs = ctx['L'], ctx['nf'], ctx['res_scale']
+    N, in_nc, H, W = ctx['shape']
+    bf = torch.bfloat16
+    Wt = lambda i: params[2 * i]
+    grads, flat, _ = _grad_arena(params, dout.device, flat, 'srresnet_backward_bf16')
+    gW = lambda i: grads[2 * i]
+    gB = lambda i: grads[2 * i + 1]
+    cache = cache if cache is not None else _PackCache()
+    dev = dout
+
+    def wd(i, cout_to=None):
+        return cache.get(('wd', i), Wt(i), lambda: ops.pack_filter_tc(_pad_filter(Wt(i), cout_to, None).float(), TC_DGRAD))
+
+    def wgrad(xv, gv, i, cin_real=None, cout_real=None):
+        """filter + bias gradient of conv i (zero-padded channel chunks cut off)"""
+        xv, gv = ops.as_view(xv), ops.as_view(gv)
+        if cin_real is None and cout_real is None:
+            ops.conv3x3_wgrad_tc(xv, gv, gW(i))
+        else:
+            tmp = torch.empty((gv.c, xv.c, 3, 3), dtype=torch.float32, device=dout.device)
+            ops.conv3x3_wgrad_tc(xv, gv, tmp)
+            gW(i).copy_(tmp[:cout_real or gv.c, :cin_real or xv.c])
+        ops.bias_grad(View(gv.t, cout_real or gv.c, gv.coff), gB(i))
+    h0, hrs, lr, fea = ctx['h0'], ctx['hrs'], ctx['lr'], ctx['fea']
+    out_nc = Wt(L.i_hr1).shape[0]
+    hh, ww = dout.shape[2], dout.shape[3]
+    g_o = torch.zeros((N, hh, ww, 32), dtype=bf, device=dout.device)      # Cout <= 3 -> one zero-padded 32-channel K chunk
+    ops.nchw_to_nhwc(dout.contiguous().float(), View(g_o, out_nc, 0))
+    wgrad(h0, g_o, L.i_hr1, cout_real=out_nc)
+    g_h0 = _empty((N, hh, ww, nf), dev, bf)
+    _dgrad_relu(g_o, wd(L.i_hr1, cout_to=32), g_h0, h0, nf)               # HR_conv0's ReLU
+    top = hrs[-1] if hrs else lr
+    wgrad(top, g_h0, L.i_hr0)
+    g_cur = _empty((N, hh, ww, nf), dev, bf)
+    ops.conv_tc(g_h0, wd(L.i_hr0), None, g_cur, kind=TC_DGRAD, nt=_pick_nt_staged(nf, nf))
+    del g_h0, g_o
+    h, w = hh, ww
+    for u in reversed(range(L.n_up)):
+        i = L.i_up0 + u
+        h, w = h // 2, w // 2
+        x_u = hrs[u - 1] if u > 0 else lr
+        g_ps = _empty((N, h, w, 4 * nf), dev, bf)
+        ops.pixel_unshuffle_mask(g_cur, hrs[u], g_ps)                     # PixelShuffle + ReLU backward, conv channel order
+        wgrad(x_u, g_ps, i)
+        g_nxt = _empty((N, h, w, nf), dev, bf)
+        ops.conv_tc(g_ps, wd(i), None, g_nxt, kind=TC_DGRAD, nt=_pick_nt_staged(nf, 4 * nf))
+        del g_ps
+        g_cur = g_nxt
+    g_lr = g_cur                                   # gradient of lr = trunk + fea
+    mids, outs = ctx['mids'], ctx['outs']
+    xs = [fea] + outs[:-1]                         # input of block k
+    trunk = outs[-1] if outs else fea
+    wgrad(trunk, g_lr, L.i_lr)
+    g_y = _empty((N, H, W, nf), dev, bf)
+    if L.nb == 0:
+        ops.conv_tc(g_lr, wd(L.i_lr), None, g_y, kind=TC_DGRAD, nt=_pick_nt_staged(nf, nf), pre=g_lr)
+    else:
+        ops.conv_tc(g_lr, wd(L.i_lr), None, g_y, kind=TC_DGRAD, nt=_pick_nt_staged(nf, nf))
+    g_s = _empty((N, H, W, nf), dev, bf) if rs != 1.0 else None
+    g_mid = _empty((N, H, W, nf), dev, bf)
+    for k in reversed(range(L.nb)):
+        # out_k = x_k + rs * (conv1(mid_k) + b1),  mid_k = relu(conv0(x_k) + b0)
+        i0, i1 = 1 + 2 * k, 2 + 2 * k
+        if g_s is not None:
+            ops.axpby(g_y, rs, None, 0.0, g_s)
+            gs = g_s
+        else:
+            gs = g_y
+        wgrad(mids[k], gs, i1)
+        _dgrad_relu(gs, wd(i1), g_mid, mids[k], nf)
+        wgrad(xs[k], g_mid, i0)
+        g_x = _empty((N, H, W, nf), dev, bf)
+        if k > 0:     # + the block's skip, through the pre-activation addend
+            ops.conv_tc(g_mid, wd(i0), None, g_x, kind=TC_DGRAD, nt=_pick_nt_staged(nf, nf), pre=g_y)
+        else:         # block 0's input is fea: + the skip + the trunk skip of LR_conv
+            ops.conv_tc(g_mid, wd(i0), None, g_x, kind=TC_DGRAD, nt=_pick_nt_staged(nf, nf), pre=g_y, res1=g_lr, beta1=1.0)
+        g_y = g_x
+    wgrad(ctx['xin'], g_y, 0, cin_real=in_nc)      # g_y is now the gradient of fea
+    return None, grads, flat
 
 
 # ==================================================================================================
@@ -788,6 +1048,28 @@ def _side_stream(device):
     return s
 
 
+def _grad_arena(params, device, flat, who):
+    """(gradients in parameters() order, flat, offset of each bias in flat): views of ONE flat fp32 tensor [filters in conv
+    order | biases in conv order] over the flat [w0, b0, w1, b1, ...] parameter list; `flat` is allocated when None."""
+    n_conv = len(params) // 2
+    w_off, b_off, o = [], [], 0
+    for i in range(n_conv):
+        w_off.append(o)
+        o += params[2 * i].numel()
+    for i in range(n_conv):
+        b_off.append(o)
+        o += params[2 * i + 1].numel()
+    if flat is None:
+        flat = torch.empty(o, dtype=torch.float32, device=device)
+    elif flat.numel() != o or flat.dtype != torch.float32:
+        raise ops._lib.DasrError('%s: gradient arena has %d elements, the network has %d' % (who, flat.numel(), o))
+    grads = []
+    for i in range(n_conv):
+        grads.append(flat[w_off[i]:w_off[i] + params[2 * i].numel()].view_as(params[2 * i]))
+        grads.append(flat[b_off[i]:b_off[i] + params[2 * i + 1].numel()])
+    return grads, flat, b_off
+
+
 def rrdb_backward_bf16(ctx, params, dout, cache=None, flat=None):
     """Backward of the mixed-precision mode: input gradients (dgrad) on the wgmma kernel (3x3 conv with flipped,
     transposed filters; gradient contributions of a dense block accumulate in place in one bf16 buffer), filter
@@ -800,22 +1082,7 @@ def rrdb_backward_bf16(ctx, params, dout, cache=None, flat=None):
     CS = nf + 4 * GC
     # all gradients are views of ONE flat fp32 buffer [filters in conv order | biases in conv order]: one copy hands them to
     # autograd, and the four LeakyReLU convs of a dense block get their bias gradients from a single reduction
-    n_conv = len(params) // 2
-    w_off, b_off, o = [], [], 0
-    for i in range(n_conv):
-        w_off.append(o)
-        o += params[2 * i].numel()
-    for i in range(n_conv):
-        b_off.append(o)
-        o += params[2 * i + 1].numel()
-    if flat is None:
-        flat = torch.empty(o, dtype=torch.float32, device=dout.device)
-    elif flat.numel() != o or flat.dtype != torch.float32:
-        raise ops._lib.DasrError('rrdb_backward_bf16: gradient arena has %d elements, the network has %d' % (flat.numel(), o))
-    grads = []
-    for i in range(n_conv):
-        grads.append(flat[w_off[i]:w_off[i] + params[2 * i].numel()].view_as(params[2 * i]))
-        grads.append(flat[b_off[i]:b_off[i] + params[2 * i + 1].numel()])
+    grads, flat, b_off = _grad_arena(params, dout.device, flat, 'rrdb_backward_bf16')
     gW = lambda i: grads[2 * i]
     gB = lambda i: grads[2 * i + 1]
     cache = cache if cache is not None else _PackCache()
@@ -966,42 +1233,63 @@ def rrdb_backward_bf16(ctx, params, dout, cache=None, flat=None):
 
 
 class _TrainGraphs:
-    """CUDA graphs of the mixed-precision forward and backward of one RRDBNet for one input shape.  A training step
-    launches ~4000 small kernels for G alone (filter re-packing, 345 fused convs, dgrad/wgrad/bias-grad per conv);
-    replaying two graphs removes that host cost.  Filters are re-packed INSIDE the forward graph (the parameters
-    change every step, their addresses do not); activations live in the graphs' private pool."""
+    """CUDA graphs of the mixed-precision forward and backward of one generator for one input shape.  A training step
+    launches thousands of small kernels for G alone (RRDBNet: filter re-packing, 345 fused convs, dgrad/wgrad/bias-grad
+    per conv); replaying two graphs removes that host cost.  Filters are re-packed INSIDE the forward graph (the
+    parameters change every step, their addresses do not); activations live in the graphs' private pool.
+    packer(plist)            -> a _BatchPacker of every filter copy the pair reads (one launch per step)
+    forward(x, plist, cache) -> (out, ctx);  backward(ctx, plist, dout, cache) -> (_, grads, flat gradient tensor)"""
 
-    def __init__(self, x, params, nb, upscale):
+    def __init__(self, x, params, packer, forward, backward):
         self.params = params
         self.x = x.detach().clone()
         cur = torch.cuda.current_stream()
         side = torch.cuda.Stream()
         side.wait_stream(cur)
         plist = [p.detach() for p in params]
-        L = RRDBLayout(nb, params[0].shape[0], upscale)
-        self.packer = _BatchPacker(plist, L, L.nf)          # every filter copy of the step from ONE launch
+        self.packer = packer(plist)              # every filter copy of the step from ONE launch
+        batched = set(self.packer.cache.d)
         with torch.cuda.stream(side):            # eager warm-up: workspaces, function attributes, allocator
             self.packer.launch()
-            out, ctx = rrdb_forward_bf16_train(self.x, plist, nb, upscale, self.packer.cache)
-            rrdb_backward_bf16(ctx, plist, torch.zeros_like(out), self.packer.cache)
+            out, ctx = forward(self.x, plist, self.packer.cache)
+            backward(ctx, plist, torch.zeros_like(out), self.packer.cache)
             del out, ctx
         cur.wait_stream(side)
         torch.cuda.synchronize()
+        # Copies the warm-up made outside the job table (the last layer's taps-in-N pack) are dropped, so the captured pass
+        # makes them again and the graph re-packs them from the live parameters on every replay; a copy cached from the
+        # warm-up would be captured as a constant and go stale after the first optimizer step.
+        for key in set(self.packer.cache.d) - batched:
+            del self.packer.cache.d[key]
         self.pool = torch.cuda.graph_pool_handle()
         self.fwd = torch.cuda.CUDAGraph()
         from . import _lib
         l0 = _lib.LAUNCHES
         with torch.cuda.graph(self.fwd, pool=self.pool):
             self.packer.launch()
-            self.out, self.ctx = rrdb_forward_bf16_train(self.x, plist, nb, upscale, self.packer.cache)
+            self.out, self.ctx = forward(self.x, plist, self.packer.cache)
         self.n_fwd = _lib.LAUNCHES - l0          # kernels of ours inside the forward graph (counted again per replay)
         self.dout = torch.zeros_like(self.out)
         self.bwd = torch.cuda.CUDAGraph()
         l0 = _lib.LAUNCHES
         with torch.cuda.graph(self.bwd, pool=self.pool):
-            _, self.grads, self.gflat = rrdb_backward_bf16(self.ctx, plist, self.dout, self.packer.cache)
+            _, self.grads, self.gflat = backward(self.ctx, plist, self.dout, self.packer.cache)
         self.n_bwd = _lib.LAUNCHES - l0
         self.pending = None
+
+    @classmethod
+    def rrdbnet(cls, x, params, nb, upscale):
+        L = RRDBLayout(nb, params[0].shape[0], upscale)
+        return cls(x, params, lambda plist: _BatchPacker(plist, L, L.nf),
+                   lambda x, plist, cache: rrdb_forward_bf16_train(x, plist, nb, upscale, cache),
+                   lambda ctx, plist, dout, cache: rrdb_backward_bf16(ctx, plist, dout, cache))
+
+    @classmethod
+    def srresnet(cls, x, params, nb, upscale, res_scale):
+        L = SRResNetLayout(nb, upscale)
+        return cls(x, params, lambda plist: _SRResNetPacker(plist, L),
+                   lambda x, plist, cache: srresnet_forward_bf16_train(x, plist, nb, upscale, cache, res_scale),
+                   lambda ctx, plist, dout, cache: srresnet_backward_bf16(ctx, plist, dout, cache))
 
     def mark_pending(self, out):
         import weakref
@@ -1010,6 +1298,28 @@ class _TrainGraphs:
     def busy(self):
         """True while a forward's output is still alive and its backward has not run."""
         return self.pending is not None and self.pending() is not None
+
+    def replay_forward(self, x):
+        self.x.copy_(x)
+        self.fwd.replay()
+        ops._lib.LAUNCHES += self.n_fwd
+        out = self.out.clone()
+        self.mark_pending(out)
+        return out
+
+    def replay_backward(self, dout, arena):
+        """gradients of the replayed backward, as views of `arena` (None: of a fresh flat tensor)"""
+        self.pending = None
+        self.dout.copy_(dout)
+        self.bwd.replay()
+        ops._lib.LAUNCHES += self.n_bwd
+        if arena is not None:
+            fl = arena
+            fl.copy_(self.gflat)                                 # one copy out of the graph's static buffer, into the bucket
+        else:
+            fl = self.gflat.clone()                              # one copy out of the graph's static buffer
+        base = self.gflat.data_ptr()
+        return [fl[(t.data_ptr() - base) // 4:(t.data_ptr() - base) // 4 + t.numel()].view(t.shape) for t in self.grads]
 
 
 class RRDBNetFunctionBF16(torch.autograd.Function):
@@ -1029,12 +1339,7 @@ class RRDBNetFunctionBF16(torch.autograd.Function):
             graphs = None
         ctx.params, ctx.cache, ctx.graphs = params, cache, graphs
         if graphs is not None:
-            graphs.x.copy_(x)
-            graphs.fwd.replay()
-            ops._lib.LAUNCHES += graphs.n_fwd
-            out = graphs.out.clone()
-            graphs.mark_pending(out)
-            return out
+            return graphs.replay_forward(x)
         out, saved = rrdb_forward_bf16_train(x, [p.detach() for p in params], nb, upscale, cache)
         ctx.saved = saved
         return out
@@ -1043,19 +1348,37 @@ class RRDBNetFunctionBF16(torch.autograd.Function):
     def backward(ctx, dout):
         g = ctx.graphs
         if g is not None:
-            g.pending = None
-            g.dout.copy_(dout)
-            g.bwd.replay()
-            ops._lib.LAUNCHES += g.n_bwd
-            if ctx.arena is not None:
-                fl = ctx.arena
-                fl.copy_(g.gflat)                                 # one copy out of the graph's static buffer, into the bucket
-            else:
-                fl = g.gflat.clone()                              # one copy out of the graph's static buffer
-            base = g.gflat.data_ptr()
-            grads = [fl[(t.data_ptr() - base) // 4:(t.data_ptr() - base) // 4 + t.numel()].view(t.shape) for t in g.grads]
+            grads = g.replay_backward(dout, ctx.arena)
         else:
             _, grads, _ = rrdb_backward_bf16(ctx.saved, [p.detach() for p in ctx.params], dout, ctx.cache, flat=ctx.arena)
+            ctx.saved = None
+        return (None, None, None, None, None, None) + tuple(gr.to(p.dtype) for gr, p in zip(grads, ctx.params))
+
+
+class SRResNetFunctionBF16(torch.autograd.Function):
+    """Mixed-precision SRResNet training node (wgmma fprop + dgrad + wgrad, fp32 filter gradients); graphs = None runs
+    eagerly.  No input-image gradient."""
+
+    @staticmethod
+    def forward(ctx, x, nb, upscale, res_scale, cache, graphs, *params):
+        if x.requires_grad:
+            raise ops._lib.DasrError('bf16 training mode does not return the input-image gradient; use precision fp32')
+        if graphs is not None and graphs.busy():
+            graphs = None          # a second forward before the pending backward: eager, on fresh buffers
+        ctx.params, ctx.cache, ctx.graphs = params, cache, graphs
+        if graphs is not None:
+            return graphs.replay_forward(x)
+        out, saved = srresnet_forward_bf16_train(x, [p.detach() for p in params], nb, upscale, cache, res_scale)
+        ctx.saved = saved
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        g = ctx.graphs
+        if g is not None:
+            grads = g.replay_backward(dout, None)
+        else:
+            _, grads, _ = srresnet_backward_bf16(ctx.saved, [p.detach() for p in ctx.params], dout, ctx.cache)
             ctx.saved = None
         return (None, None, None, None, None, None) + tuple(gr.to(p.dtype) for gr, p in zip(grads, ctx.params))
 

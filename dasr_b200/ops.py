@@ -13,7 +13,7 @@ from ._lib import ConvF32Params, ConvTcParams, check
 
 ACT_NONE, ACT_LRELU, ACT_RELU = 0, 1, 2
 FWD, DGRAD = 0, 1
-TC_FPROP, TC_DGRAD, TC_UPCONV, TC_TAPN = 0, 1, 2, 3
+TC_FPROP, TC_DGRAD, TC_UPCONV, TC_TAPN, TC_PS = 0, 1, 2, 3, 4
 
 
 def _stream():
@@ -395,6 +395,31 @@ def conv_tc(inp, w_packed, bias, out, kind=TC_FPROP, nt=None, act=ACT_NONE, slop
                            res2.ptr if res2 else None, mask.ptr if mask else None, out.ptr, C.byref(p), _stream()), 'conv_tc')
 
 
+def conv_tc_ps(inp, w_packed, bias, out, nt=None, act=ACT_NONE, slope=0.2, alpha=1.0):
+    """wgmma 3x3 conv with 4 * out.c output channels followed by nn.PixelShuffle(2), stored by the conv's epilogue:
+    out[n, 2h + i, 2w + j, c] = alpha * act(conv[n, 4c + 2i + j, h, w] + bias) on the channel slice `out` of the 2H x 2W NHWC
+    tensor.  w_packed: pack_filter_tc(w, TC_PS) (rows in parity-major order); bias: the conv's 4 * out.c fp32 biases in their own
+    order (nn.Conv2d's).  nt: Cout tile, 32 or 64 dividing out.c (default 64 when it divides out.c, else 32)."""
+    inp, out = as_view(inp), as_view(out)
+    N, H, W, _ = inp.t.shape
+    p = ConvTcParams()
+    lib = _lib.load()
+    check(lib.dasr_conv_tc_setup(C.byref(p), TC_PS), 'conv_tc_setup', 0)
+    p.N, p.H, p.W = N, H, W
+    p.f16 = int(inp.t.dtype == torch.float16)
+    for t in (w_packed, out.t):
+        if t.dtype != inp.t.dtype:
+            raise _lib.DasrError('conv_tc_ps: operands of different 16-bit types (%s vs %s)' % (t.dtype, inp.t.dtype))
+    _check_operand('output', out, (N, 2 * H, 2 * W), out.c, inp.t.dtype)
+    p.cin, p.in_cs, p.in_coff = inp.c, inp.cs, inp.coff
+    p.cout, p.out_cs, p.out_coff = 4 * out.c, out.cs, out.coff
+    p.nt = nt if nt else (64 if out.c % 64 == 0 else 32)
+    p.act, p.slope, p.alpha = act, slope, alpha
+    p.act_cols = p.cout if act != ACT_NONE else 0
+    p.epi_mode = 0
+    check(lib.dasr_conv_tc(inp.ptr, _p(w_packed), _p(bias), None, None, None, None, out.ptr, C.byref(p), _stream()), 'conv_tc')
+
+
 MAP_CHANNEL, MAP_SCALE = 1, 2      # DASR_MAP_CHANNEL / DASR_MAP_SCALE
 
 
@@ -643,6 +668,20 @@ def pixel_shuffle(src, dst, r, inverse=False):
     lo = dst if inverse else src
     N, H, W, CC = lo.shape
     check(_lib.load().dasr_pixel_shuffle(_p(src), _p(dst), N, H, W, CC // (r * r), r, int(bool(inverse)), _stream()), 'pixel_shuffle')
+
+
+def pixel_unshuffle_mask(g_hr, y_hr, g_lr):
+    """Backward of nn.PixelShuffle(2) + ReLU on bf16 NHWC: g_lr [N,H,W,4C][4c + 2i + j] = g_hr [N,2H,2W,C][c] at (2h + i, 2w + j),
+    times (y_hr > 0) there (y_hr None: no mask).  Whole contiguous tensors."""
+    N, H, W, C4 = g_lr.shape
+    C = g_hr.shape[-1]
+    if tuple(g_hr.shape) != (N, 2 * H, 2 * W, C) or C4 != 4 * C or (y_hr is not None and y_hr.shape != g_hr.shape):
+        raise _lib.DasrError('pixel_unshuffle_mask: g_hr %s / y_hr %s / g_lr %s do not form a 2x pixel shuffle' % (
+            tuple(g_hr.shape), None if y_hr is None else tuple(y_hr.shape), tuple(g_lr.shape)))
+    for t in (g_hr, y_hr, g_lr):
+        if t is not None and t.dtype != torch.bfloat16:
+            raise _lib.DasrError('pixel_unshuffle_mask: bf16 tensors only (got %s)' % t.dtype)
+    check(_lib.load().dasr_pixel_unshuffle_mask_bf16(_p(g_hr), _p(y_hr), _p(g_lr), N, H, W, C, _stream()), 'pixel_unshuffle_mask')
 
 
 def ddm(patch, H, W, ilo, ihi, jlo, jhi):

@@ -105,7 +105,7 @@ class RRDBNet(nn.Module):
                     graphs = self._train_graphs.get(key)
                     if graphs is None:
                         self._train_graphs.clear()
-                        graphs = self._train_graphs[key] = engine._TrainGraphs(x.contiguous().float(), params, self.nb, self.upscale)
+                        graphs = self._train_graphs[key] = engine._TrainGraphs.rrdbnet(x.contiguous().float(), params, self.nb, self.upscale)
                 arena = self._grad_arena if all(p.requires_grad for p in params) else None
                 return engine.RRDBNetFunctionBF16.apply(x, self.nb, self.upscale, self._pack_cache, graphs, arena, *params)
             return engine.RRDBNetFunction.apply(x, self.nb, self.upscale, *params)

@@ -5,12 +5,17 @@ Discriminator_VGG_192; block.py:158-190 ResNetBlock, :838-851 pixelshuffle_block
 Same constructor signatures and state_dict keys.  Each network is ONE autograd node (dasr_b200.seqnet): its module
 tree is compiled into a layer list — convs (+ fused LeakyReLU / ReLU epilogues), BatchNorm+activation kernels,
 nn.PixelShuffle as a gather kernel with the activation folded into the preceding conv, nn.Linear as the k x k valid
-convolution over the feature map it flattens — and run on the fp32 kernels."""
-import math
+convolution over the feature map it flattens — and run on the fp32 kernels.
 
+SRResNet (norm None, CNA, pixel shuffle) can also run on the wgmma kernels: inference with SRResNet.precision 'bf16' / 'fp16'
+(engine.srresnet_forward_bf16), mixed-precision training with SRResNet.train_precision 'bf16' (engine.SRResNetFunctionBF16)."""
+import math
+import os
+
+import torch
 import torch.nn as nn
 
-from dasr_b200 import seqnet
+from dasr_b200 import _lib, engine, seqnet
 from . import block as B
 
 
@@ -76,9 +81,30 @@ class _Compiled(nn.Module):
 
 
 class SRResNet(_Compiled):
+    """precision (inference without gradients): None -> DASR_B200_PRECISION if set, else 'fp32'.
+      'fp32'          : the layer list on the fp32 kernels.
+      'bf16' / 'fp16' : engine.srresnet_forward_bf16 on the wgmma kernels (16-bit activations, fp32 accumulation; fp16 needs
+                        every activation inside half's range, |x| < 65504).
+    train_precision (forwards that need gradients): None -> DASR_B200_TRAIN_PRECISION if set, else 'fp32'.
+      'fp32'          : the layer list on the fp32 kernels (also returns the input-image gradient).
+      'bf16'          : mixed precision (engine.SRResNetFunctionBF16): wgmma fprop / dgrad / wgrad with bf16 activations and
+                        gradients, fp32 accumulation, fp32 filter and bias gradients; no input-image gradient.
+    The 16-bit modes replay CUDA graphs from the second forward of a shape on.  They cover norm_type None, mode 'CNA',
+    ReLU, pixel-shuffle upsampling, upscale 2 / 4, nf 32 / 64 / 128 (engine.srresnet_tc_reason), in_nc <= 32, out_nc <= 3.  Set on the module, a 16-bit
+    mode raises DasrError for any other configuration; chosen by the environment, it keeps the fp32 layer list."""
+
     def __init__(self, in_nc, out_nc, nf, nb, upscale=4, norm_type='batch', act_type='relu', mode='NAC', res_scale=1,
                  upsample_mode='upconv'):
         super().__init__()
+        self.nb, self.upscale, self.res_scale = nb, upscale, float(res_scale)
+        self._tc_unsupported = self._tc_reason(in_nc, out_nc, nf, upscale, norm_type, act_type, mode, upsample_mode)
+        self.precision = None
+        self.train_precision = None
+        self._pack_cache = engine._PackCache()
+        self._graphs = {}
+        self._graph_seen = None
+        self._train_graphs = {}
+        self._train_seen = None
         n_upscale = 1 if upscale == 3 else int(math.log(upscale, 2))
         fea_conv = B.conv_block(in_nc, nf, kernel_size=3, norm_type=None, act_type=None)
         resnet_blocks = [ResNetBlock(nf, nf, nf, norm_type=norm_type, act_type=act_type, mode=mode, res_scale=res_scale) for _ in range(nb)]
@@ -98,6 +124,82 @@ class SRResNet(_Compiled):
 
     def _children(self):
         return [('model.', self.model)]
+
+    @staticmethod
+    def _tc_reason(in_nc, out_nc, nf, upscale, norm_type, act_type, mode, upsample_mode):
+        """why the wgmma path cannot run this configuration (None: it can)"""
+        if norm_type is not None:
+            return 'norm_type %r (the wgmma path has no BatchNorm)' % (norm_type,)
+        if mode != 'CNA':
+            return "mode %r (the wgmma path runs 'CNA')" % (mode,)
+        if act_type != 'relu':
+            return "act_type %r (the wgmma path runs 'relu')" % (act_type,)
+        if upsample_mode != 'pixelshuffle':
+            return "upsample_mode %r (the wgmma path runs 'pixelshuffle')" % (upsample_mode,)
+        if upscale not in (2, 4):
+            return 'upscale %s (the wgmma path runs 2 and 4)' % (upscale,)
+        reason = engine.srresnet_tc_reason(nf)
+        if reason:
+            return reason
+        if in_nc > 32 or out_nc > 3:
+            return 'in_nc %d / out_nc %d (the wgmma path needs in_nc <= 32, out_nc <= 3)' % (in_nc, out_nc)
+        return None
+
+    def _resolve(self, attr, env, modes):
+        """the precision of module attribute `attr`, else of environment variable `env` if set, else 'fp32'"""
+        prec = getattr(self, attr)
+        if prec is not None:
+            if prec not in modes:
+                raise _lib.DasrError('SRResNet: %s %r is not supported (%s)' % (attr, prec, ' | '.join(modes)))
+            if prec != 'fp32' and self._tc_unsupported:
+                raise _lib.DasrError('SRResNet: %s %r needs the wgmma path, which does not run %s'
+                                     % (attr, prec, self._tc_unsupported))
+            return prec
+        prec = os.environ.get(env)
+        if prec in modes and prec != 'fp32' and not self._tc_unsupported:
+            return prec
+        return 'fp32'
+
+    def forward(self, x):
+        params = list(self.parameters())
+        need_grad = torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in params))
+        if need_grad:
+            if self._resolve('train_precision', 'DASR_B200_TRAIN_PRECISION', ('bf16', 'fp32')) == 'fp32':
+                return super().forward(x)
+            return self._train_bf16(x, params)
+        prec = self._resolve('precision', 'DASR_B200_PRECISION', ('bf16', 'fp16', 'fp32'))
+        if prec == 'fp32':
+            return super().forward(x)
+        fn = lambda t: engine.srresnet_forward_bf16(t, params, self.nb, self.upscale, self._pack_cache, half=prec == 'fp16',
+                                                    res_scale=self.res_scale)
+        if os.environ.get('DASR_B200_GRAPH', '1') == '0' or not x.is_cuda or engine.PROFILE is not None:
+            return fn(x)
+        from .architecture import _GraphedForward
+        key = (tuple(x.shape), x.dtype, x.device.index, prec, tuple(p._version for p in params),
+               params[0].data_ptr(), params[len(params) // 2].data_ptr(), params[-1].data_ptr())
+        g = self._graphs.get(key)
+        if g is None:
+            # capture on the second sighting of a (shape, parameter version), as RRDBNet does
+            if self._graph_seen != key:
+                self._graph_seen = key
+                return fn(x)
+            if len(self._graphs) >= 2:        # each graph pins its activation pool: keep at most two shapes
+                self._graphs.clear()
+            g = self._graphs[key] = _GraphedForward(fn, x.contiguous().float())
+        return g(x)
+
+    def _train_bf16(self, x, params):
+        graphs = None
+        if os.environ.get('DASR_B200_GRAPH', '1') != '0' and x.is_cuda and not x.requires_grad:
+            # the graphs hold raw parameter addresses: re-capture if any parameter storage moved (.to(), .float(), ...)
+            key = (tuple(x.shape), x.device.index, params[0].data_ptr(), params[len(params) // 2].data_ptr(), params[-1].data_ptr())
+            graphs = self._train_graphs.get(key)
+            if graphs is None and self._train_seen == key:       # capture on the second sighting of a shape
+                self._train_graphs.clear()
+                graphs = self._train_graphs[key] = engine._TrainGraphs.srresnet(x.contiguous().float(), params, self.nb,
+                                                                                self.upscale, self.res_scale)
+            self._train_seen = key
+        return engine.SRResNetFunctionBF16.apply(x, self.nb, self.upscale, self.res_scale, self._pack_cache, graphs, *params)
 
 
 class Discriminator_VGG_128(nn.Module):

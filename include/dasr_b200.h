@@ -218,6 +218,16 @@ int dasr_conv_tc2_map(const void* in_bf16, const void* w_packed_bf16, const floa
  *                                            2 = nearest-x2-upsample + 3x3 (4 variants x 4 taps, pre-summed)
  *                                            3 = last layer, taps in GEMM-N (cout <= 3): [chunk][tap * cout + c, padded to 32][32]
  *                                                for dasr_conv_tc epi_mode 3 (dasr_pack_filter_tc only, not the batch form)
+ *                                            4 = 3x3 conv followed by nn.PixelShuffle(2): kind 0's layout with the rows in
+ *                                                parity-major order, packed row b * (cout / 4) + c <- OIHW row 4c + b
+ *                                                (b = 2i + j; dasr_pack_filter_tc only).  dasr_conv_tc then writes
+ *                                                out[n, 2h + i, 2w + j, out_coff + c] = conv[n, 4c + 2i + j, h, w] into the
+ *                                                2H x 2W NHWC tensor: cout = 4 x the shuffled channels, nt 32 or 64 divides cout / 4,
+ *                                                staged epilogue without pre / residual inputs; the bias is the conv's
+ *                                                4C biases in their own (OIHW) order; act / alpha apply elementwise
+ *                                                after the shuffle.  Batch form: kind 0 jobs over the filter viewed as
+ *                                                [C][4 cin][3][3] (src unchanged, cin = 4 cin), parity b = input channels
+ *                                                ci_lo = b cin, ci_n = cin -> dst rows b C .. b C + C of 4C.
  * Fills the tap tables / variant fields of *p as well (host side). */
 int dasr_conv_tc_setup(DasrConvTcParams* p, int kind);
 size_t dasr_pack_filter_tc_bytes(int cout, int cin, int kind);
