@@ -37,17 +37,20 @@ def rank():
 
 
 def broadcast_module(net, src=0):
-    """Every parameter and buffer of `net` from rank `src` (two flat broadcasts: parameters, floating buffers)."""
+    """Every parameter and buffer of `net` from rank `src` (two flat broadcasts: parameters, floating buffers).  The
+    tensors are written in place under no_grad, not through .data, so their version counters move and every cache
+    keyed on them (packed filters, CUDA graphs) rebuilds."""
     net = _unwrap(net)
-    for group in ([p.data for p in net.parameters()], [b.data for b in net.buffers() if b.is_floating_point()]):
-        if not group:
-            continue
-        flat = torch.cat([t.reshape(-1).float() for t in group])
-        dist.broadcast(flat, src)
-        o = 0
-        for t in group:
-            t.copy_(flat[o:o + t.numel()].view_as(t))
-            o += t.numel()
+    with torch.no_grad():
+        for group in (list(net.parameters()), [b for b in net.buffers() if b.is_floating_point()]):
+            if not group:
+                continue
+            flat = torch.cat([t.reshape(-1).float() for t in group])
+            dist.broadcast(flat, src)
+            o = 0
+            for t in group:
+                t.copy_(flat[o:o + t.numel()].view_as(t))
+                o += t.numel()
 
 
 class GradBucket:

@@ -13,6 +13,7 @@ precision:
 """
 import math
 import os
+import weakref
 
 import torch
 
@@ -1275,7 +1276,7 @@ class _TrainGraphs:
         with torch.cuda.graph(self.bwd, pool=self.pool):
             _, self.grads, self.gflat = backward(self.ctx, plist, self.dout, self.packer.cache)
         self.n_bwd = _lib.LAUNCHES - l0
-        self.pending = None
+        self.owner = None                        # weakref to the autograd node whose activations the static buffers hold
 
     @classmethod
     def rrdbnet(cls, x, params, nb, upscale):
@@ -1291,25 +1292,27 @@ class _TrainGraphs:
                    lambda x, plist, cache: srresnet_forward_bf16_train(x, plist, nb, upscale, cache, res_scale),
                    lambda ctx, plist, dout, cache: srresnet_backward_bf16(ctx, plist, dout, cache))
 
-    def mark_pending(self, out):
-        import weakref
-        self.pending = weakref.ref(out)
-
     def busy(self):
-        """True while a forward's output is still alive and its backward has not run."""
-        return self.pending is not None and self.pending() is not None
+        """True while the node of the last replayed forward is alive and its backward has not run: its backward reads the
+        static activations, which another replay would overwrite.  The node, not its output tensor, is tracked: autograd
+        keeps the node (and the need for its activations) alive after the caller has dropped the output."""
+        node = self.owner() if self.owner is not None else None
+        return node is not None and node.pending
 
-    def replay_forward(self, x):
+    def replay_forward(self, ctx, x):
         self.x.copy_(x)
         self.fwd.replay()
         ops._lib.LAUNCHES += self.n_fwd
-        out = self.out.clone()
-        self.mark_pending(out)
-        return out
+        self.owner = weakref.ref(ctx)
+        return self.out.clone()
 
-    def replay_backward(self, dout, arena):
-        """gradients of the replayed backward, as views of `arena` (None: of a fresh flat tensor)"""
-        self.pending = None
+    def replay_backward(self, ctx, dout, arena):
+        """gradients of the replayed backward of node `ctx`, as views of `arena` (None: of a fresh flat tensor).  Raises
+        DasrError if a later forward has replayed since ctx's (a backward with retain_graph=True, a forward, then a second
+        backward through ctx): the static activations are no longer ctx's."""
+        if self.owner is None or self.owner() is not ctx:
+            raise ops._lib.DasrError('backward through a CUDA-graph training node whose activations a later forward has '
+                                     'overwritten (retain_graph=True, then another forward of the same generator)')
         self.dout.copy_(dout)
         self.bwd.replay()
         ops._lib.LAUNCHES += self.n_bwd
@@ -1322,6 +1325,60 @@ class _TrainGraphs:
         return [fl[(t.data_ptr() - base) // 4:(t.data_ptr() - base) // 4 + t.numel()].view(t.shape) for t in self.grads]
 
 
+def _save_activations(ctx, saved):
+    """Keep the eager forward's activations (a dict of tensors, lists of tensors and plain values) through
+    save_for_backward: autograd then frees them after a backward without retain_graph, refuses a second backward
+    through the node, and keeps them for one with retain_graph=True."""
+    tensors, slots = [], {}
+    for k, v in saved.items():
+        if isinstance(v, torch.Tensor):
+            slots[k] = len(tensors)
+            tensors.append(v)
+        elif isinstance(v, list) and v and all(isinstance(t, torch.Tensor) for t in v):
+            slots[k] = slice(len(tensors), len(tensors) + len(v))
+            tensors += v
+    ctx.save_for_backward(*tensors)
+    ctx.saved_rest = {k: v for k, v in saved.items() if k not in slots}
+    ctx.saved_slots = slots
+
+
+def _saved_activations(ctx):
+    t = ctx.saved_tensors
+    saved = dict(ctx.saved_rest)
+    for k, s in ctx.saved_slots.items():
+        saved[k] = list(t[s]) if isinstance(s, slice) else t[s]
+    return saved
+
+
+_ARENA_NODES = []        # weakrefs to the live training nodes that were handed a gradient arena
+
+
+def _overlaps(t, lo, hi):
+    a = t.data_ptr()
+    return a < hi and lo < a + t.numel() * t.element_size()
+
+
+def _arena_for(ctx):
+    """The gradient arena node `ctx` may write into, else None (its backward then writes a fresh flat tensor and
+    autograd sums).  Every backward returns views of the same arena, so a second writer would overwrite gradients
+    autograd still holds: the arena is refused while another live node that was handed it has not run its backward
+    (two generator calls in one loss), or while a parameter's .grad aliases it (accumulation without zero_grad, a
+    second backward with retain_graph=True)."""
+    arena = ctx.arena
+    if arena is None:
+        return None
+    lo = arena.data_ptr()
+    hi = lo + arena.numel() * arena.element_size()
+    _ARENA_NODES[:] = [r for r in _ARENA_NODES if r() is not None]
+    for r in _ARENA_NODES:
+        node = r()
+        if node is not None and node is not ctx and node.pending and _overlaps(node.arena, lo, hi):
+            return None
+    if any(p.grad is not None and _overlaps(p.grad, lo, hi) for p in ctx.params):
+        return None
+    return arena
+
+
 class RRDBNetFunctionBF16(torch.autograd.Function):
     """Mixed-precision training node (wgmma fprop + dgrad + wgrad); graphs = None runs eagerly."""
 
@@ -1329,29 +1386,33 @@ class RRDBNetFunctionBF16(torch.autograd.Function):
     def forward(ctx, x, nb, upscale, cache, graphs, arena, *params):
         """arena: optional flat fp32 tensor (numel = all parameters) that receives the gradients in the layout
         [filters in conv order | biases in conv order]; the returned gradients are then views of it (data-parallel
-        bucket segment, dasr_b200.dp) instead of views of a fresh tensor."""
-        ctx.arena = arena
+        bucket segment, dasr_b200.dp) instead of views of a fresh tensor, unless another holder of the arena still
+        needs it (_arena_for)."""
         if x.requires_grad:
             raise ops._lib.DasrError('bf16 training mode does not return the input-image gradient; use precision fp32')
         if graphs is not None and graphs.busy():
             # the graphs own ONE set of static activations: a second forward before the pending backward would overwrite
             # what that backward reads, so this call runs eagerly on fresh buffers instead
             graphs = None
-        ctx.params, ctx.cache, ctx.graphs = params, cache, graphs
+        ctx.params, ctx.cache, ctx.graphs, ctx.arena, ctx.pending = params, cache, graphs, arena, True
+        if arena is not None:
+            _ARENA_NODES.append(weakref.ref(ctx))
         if graphs is not None:
-            return graphs.replay_forward(x)
+            return graphs.replay_forward(ctx, x)
         out, saved = rrdb_forward_bf16_train(x, [p.detach() for p in params], nb, upscale, cache)
-        ctx.saved = saved
+        _save_activations(ctx, saved)
         return out
 
     @staticmethod
     def backward(ctx, dout):
         g = ctx.graphs
+        arena = _arena_for(ctx)
         if g is not None:
-            grads = g.replay_backward(dout, ctx.arena)
+            grads = g.replay_backward(ctx, dout, arena)
         else:
-            _, grads, _ = rrdb_backward_bf16(ctx.saved, [p.detach() for p in ctx.params], dout, ctx.cache, flat=ctx.arena)
-            ctx.saved = None
+            _, grads, _ = rrdb_backward_bf16(_saved_activations(ctx), [p.detach() for p in ctx.params], dout, ctx.cache,
+                                             flat=arena)
+        ctx.pending = False
         return (None, None, None, None, None, None) + tuple(gr.to(p.dtype) for gr, p in zip(grads, ctx.params))
 
 
@@ -1365,21 +1426,21 @@ class SRResNetFunctionBF16(torch.autograd.Function):
             raise ops._lib.DasrError('bf16 training mode does not return the input-image gradient; use precision fp32')
         if graphs is not None and graphs.busy():
             graphs = None          # a second forward before the pending backward: eager, on fresh buffers
-        ctx.params, ctx.cache, ctx.graphs = params, cache, graphs
+        ctx.params, ctx.cache, ctx.graphs, ctx.pending = params, cache, graphs, True
         if graphs is not None:
-            return graphs.replay_forward(x)
+            return graphs.replay_forward(ctx, x)
         out, saved = srresnet_forward_bf16_train(x, [p.detach() for p in params], nb, upscale, cache, res_scale)
-        ctx.saved = saved
+        _save_activations(ctx, saved)
         return out
 
     @staticmethod
     def backward(ctx, dout):
         g = ctx.graphs
         if g is not None:
-            grads = g.replay_backward(dout, None)
+            grads = g.replay_backward(ctx, dout, None)
         else:
-            _, grads, _ = srresnet_backward_bf16(ctx.saved, [p.detach() for p in ctx.params], dout, ctx.cache)
-            ctx.saved = None
+            _, grads, _ = srresnet_backward_bf16(_saved_activations(ctx), [p.detach() for p in ctx.params], dout, ctx.cache)
+        ctx.pending = False
         return (None, None, None, None, None, None) + tuple(gr.to(p.dtype) for gr, p in zip(grads, ctx.params))
 
 

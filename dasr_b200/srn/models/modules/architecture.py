@@ -22,6 +22,18 @@ def _precision(module_default):
     return os.environ.get('DASR_B200_PRECISION', module_default)
 
 
+def graph_key(x, params, *extra, versions):
+    """Cache key of a CUDA graph of a generator for input `x`.  The graphs read every parameter through its raw address,
+    so the key holds every parameter's storage address: replacing any one by a new nn.Parameter re-captures.  An
+    inference graph also bakes in the kernel-layout filters packed before capture, so with `versions` the key holds every
+    version counter too: an in-place update (optimizer step, load_state_dict) re-captures.  Writes through .data move
+    neither and stay invisible (INTEGRATION.md)."""
+    key = (tuple(x.shape), x.dtype, x.device.index) + extra + tuple(map(torch.Tensor.data_ptr, params))
+    if versions:
+        key += tuple(p._version for p in params)
+    return key
+
+
 class _GraphedForward:
     """One inference forward captured into a CUDA graph (the wgmma path launches ~350-2800 small kernels per
     forward; replaying a graph removes the per-launch host cost).  Inputs are copied into a static buffer; the
@@ -101,7 +113,7 @@ class RRDBNet(nn.Module):
                 graphs = None
                 if os.environ.get('DASR_B200_GRAPH', '1') != '0' and x.is_cuda and not x.requires_grad:
                     # the graphs hold raw parameter addresses: re-capture if any parameter storage moved (.to(), .float(), ...)
-                    key = (tuple(x.shape), x.device.index, params[0].data_ptr(), params[len(params) // 2].data_ptr(), params[-1].data_ptr())
+                    key = graph_key(x, params, versions=False)
                     graphs = self._train_graphs.get(key)
                     if graphs is None:
                         self._train_graphs.clear()
@@ -117,8 +129,7 @@ class RRDBNet(nn.Module):
                                                     per_layer=prec.endswith('_layer'), half=prec.startswith('fp16'))
             if os.environ.get('DASR_B200_GRAPH', '1') == '0' or not x.is_cuda or engine.PROFILE is not None:
                 return fn(x)
-            key = (tuple(x.shape), x.dtype, x.device.index, prec, tuple(p._version for p in params),
-                   params[0].data_ptr(), params[len(params) // 2].data_ptr(), params[-1].data_ptr())
+            key = graph_key(x, params, prec, versions=True)
             g = self._graphs.get(key)
             if g is None:
                 # capture only the SECOND time a (shape, parameter version) is seen: validation over differently sized
@@ -215,8 +226,7 @@ class _AdaptiveRRDBNet(nn.Module):
                                                             self._pack_cache, half=prec == 'fp16')
         if os.environ.get('DASR_B200_GRAPH', '1') == '0' or not x.is_cuda or engine.PROFILE is not None:
             return fn(x, adaptive_weights)
-        key = (tuple(x.shape), tuple(adaptive_weights.shape), x.device.index, prec, tuple(p._version for p in params),
-               params[0].data_ptr(), params[len(params) // 2].data_ptr(), params[-1].data_ptr())
+        key = graph_key(x, params, tuple(adaptive_weights.shape), prec, versions=True)
         g = self._graphs.get(key)
         if g is None:
             # capture on the second sighting of a (shape, parameter version), like RRDBNet

@@ -174,9 +174,8 @@ class SRResNet(_Compiled):
                                                     res_scale=self.res_scale)
         if os.environ.get('DASR_B200_GRAPH', '1') == '0' or not x.is_cuda or engine.PROFILE is not None:
             return fn(x)
-        from .architecture import _GraphedForward
-        key = (tuple(x.shape), x.dtype, x.device.index, prec, tuple(p._version for p in params),
-               params[0].data_ptr(), params[len(params) // 2].data_ptr(), params[-1].data_ptr())
+        from .architecture import _GraphedForward, graph_key
+        key = graph_key(x, params, prec, versions=True)
         g = self._graphs.get(key)
         if g is None:
             # capture on the second sighting of a (shape, parameter version), as RRDBNet does
@@ -192,7 +191,8 @@ class SRResNet(_Compiled):
         graphs = None
         if os.environ.get('DASR_B200_GRAPH', '1') != '0' and x.is_cuda and not x.requires_grad:
             # the graphs hold raw parameter addresses: re-capture if any parameter storage moved (.to(), .float(), ...)
-            key = (tuple(x.shape), x.device.index, params[0].data_ptr(), params[len(params) // 2].data_ptr(), params[-1].data_ptr())
+            from .architecture import graph_key
+            key = graph_key(x, params, versions=False)
             graphs = self._train_graphs.get(key)
             if graphs is None and self._train_seen == key:       # capture on the second sighting of a shape
                 self._train_graphs.clear()
