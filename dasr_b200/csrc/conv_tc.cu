@@ -23,6 +23,8 @@
 // Cluster pair (dasr_conv_tc2): two CTAs of a (1, 2, 1) cluster take the two Cout halves of the SAME pixel tiles; each
 // keeps only its half of the filters resident, and the leader's TMA multicasts every A halo tile into both CTAs, so an
 // activation tile crosses L2 -> SMEM once for the pair.  That is what lets a 192-wide filter set (221 KB) run as one tile.
+// A dasr_conv_tc2 launch whose whole filter set fits one SM and whose grid has many tiles per SM runs one CTA per tile
+// instead (tc2_single).
 #include <type_traits>
 #include "tc_common.cuh"
 
@@ -1219,9 +1221,11 @@ static bool chunk_list_pairs64(const DasrConvTcParams* p) {
   return true;
 }
 
-// pair = 1: (1, 2, 1) clusters, p->nt is the Cout tile of ONE CTA (half of the pair's tile)
+// pair = 1: (1, 2, 1) clusters, p->nt is the Cout tile of ONE CTA (half of the pair's tile).
+// order32: every output element sums its products in the order of 32-channel A loads (dasr_conv_tc2's launches, on the
+// pair or on one CTA), so a contiguous slice never takes the tap-major 64-channel loads.
 static int conv_tc_launch(const void* in, const void* w, const float* bias, const void* pre, const void* res1, const void* res2,
-                          const void* mask_src, void* out, const DasrConvTcParams* p, void* stream, int pair,
+                          const void* mask_src, void* out, const DasrConvTcParams* p, void* stream, int pair, bool order32,
                           const float* map = nullptr, const float* map_w = nullptr) {
   PFN_encodeTiled enc = get_encode();
   if (!enc) {
@@ -1245,9 +1249,10 @@ static int conv_tc_launch(const void* in, const void* w, const float* bias, cons
   a.tiles_y = cdiv(p->H, TILE_H);
   a.ntiles = (long)p->N * a.tiles_x * a.tiles_y;
   a.w_bytes = p->ntaps * a.nchunks * p->nt * ROW_B;
-  // single CTA: 64-channel A chunks for a contiguous input slice whose channel count is a multiple of 64 (a pair starts
-  // from 32-channel stages, whose smaller footprint leaves room for the larger filter sets it exists for; see below)
-  a.chunk64 = (!pair && p->a_mode == 0 && p->nchunk_list == 0 && p->cin % (2 * CHUNK) == 0) ? 1 : 0;
+  // dasr_conv_tc: 64-channel A chunks for a contiguous input slice whose channel count is a multiple of 64, K steps
+  // tap-major.  dasr_conv_tc2 starts from 32-channel stages, whose smaller footprint leaves room for the larger filter sets
+  // the pair exists for, and takes 64-channel rows only in 32-channel order (see below).
+  a.chunk64 = (!order32 && p->a_mode == 0 && p->nchunk_list == 0 && p->cin % (2 * CHUNK) == 0) ? 1 : 0;
   a.has_pre = (p->epi_mode == 0 && pre) ? 1 : 0;
   a.has_res1 = (p->epi_mode == 0 && res1) ? 1 : 0;
   a.has_res2 = (p->epi_mode == 0 && res2) ? 1 : 0;
@@ -1300,11 +1305,11 @@ static int conv_tc_launch(const void* in, const void* w, const float* bias, cons
     return DASR_E_SMEM;
   }
 
-  // Pair on the ping-pong consumers: 64-channel A loads (half the TMA requests per byte) for a contiguous slice of 64k
-  // channels or a chunk list of 64-channel runs, issued half-major (chunk64 = 2), so the products and their order stay
-  // those of 32-channel loads.  Only when the wider stages still leave two staging frames and hold the A loads of two
+  // Ping-pong consumers: 64-channel A loads (half the TMA requests per byte) for a chunk list of 64-channel runs, and for a
+  // contiguous slice of 64k channels in 32-channel order, issued half-major (chunk64 = 2), so the products and their order
+  // stay those of 32-channel loads.  Only when the wider stages still leave two staging frames and hold the A loads of two
   // tiles, one per consumer warpgroup; otherwise the launch keeps its 32-channel plan.
-  if (pair && pp >= 0 && p->ntaps == 9 && ((p->nchunk_list == 0 && p->cin % (2 * CHUNK) == 0) || chunk_list_pairs64(p))) {
+  if (pp >= 0 && p->ntaps == 9 && ((order32 && p->nchunk_list == 0 && p->cin % (2 * CHUNK) == 0) || chunk_list_pairs64(p))) {
     int nbuf64 = 0;
     const int stages64 = tc_plan(a.w_bytes, (int)a_stage_bytes_for(p, 1), a.epi_bytes, a.has_res1 + a.has_res2, 0, &nbuf64);
     if (stages64 >= 2 && nbuf64 >= 2 && stages64 >= 2 * (a.nchunks / 2)) {
@@ -1485,7 +1490,7 @@ static int conv_tc_run(const void* in, const void* w, const float* bias, const v
                "conv_tc: pointers must be 16-byte aligned");
   DasrConvTcParams q = *p;
   if (p->epi_mode == 0) q.mask_c0 = q.mask_c1 = 0;   // the staged epilogue's mask mode belongs to dasr_conv_tc2
-  return conv_tc_launch(in, w, bias, pre, res1, res2, mask_src, out, &q, stream, 0, map, map_w);
+  return conv_tc_launch(in, w, bias, pre, res1, res2, mask_src, out, &q, stream, 0, false, map, map_w);
 }
 
 int dasr_conv_tc(const void* in, const void* w, const float* bias, const void* pre, const void* res1, const void* res2,
@@ -1532,6 +1537,27 @@ static int tc2_fits(const DasrConvTcParams* p, int nres) {
   return tc_plan(w_bytes, (int)a_stage_bytes_for(p, 0), half * 128 * 2, nres, 0, &nbuf) >= 2;
 }
 
+// Work per SM, in pixel tiles x Cout tiles, from which a dasr_conv_tc2 launch runs one CTA per tile instead of the pair.
+// On the pair the leader's TMA unit issues the A tiles of two SMs and each CTA runs MMAs half as wide; below about one wave
+// the pair puts twice as many SMs on the work.  Measured on an H100 SXM (tools/time_pair_vs_single.py, DESIGN §6), one CTA
+// per tile takes 0.63-1.00 of the pair's time at 8 waves and 0.58-0.81 at 16 and 62, while up to 4 waves neither side
+// wins consistently.  16 rather than 8 keeps the pair's own exact-test launches (up to 8.5 waves) on the pair; no workload
+// of the project runs a qualifying launch between 8 and 16 waves.
+constexpr int TC2_SINGLE_WAVES = 16;
+
+// dasr_conv_tc2 on one CTA per tile, with the pair's whole Cout tile p->nt on each CTA: when a ping-pong instantiation
+// exists for that tile, the launch carries no dgrad mask (the pair's epilogue mode) and no weight map, the whole filter set
+// still leaves two staging frames and the 32-channel A stages of two tiles, and the grid has TC2_SINGLE_WAVES waves of tiles.
+static bool tc2_single(const DasrConvTcParams* p, int nres, const float* map) {
+  if ((p->nt != 16 && p->nt != 32 && p->nt != 64) || p->mask_c1 > p->mask_c0 || map) return false;
+  const int nchunks = p->cin / CHUNK;
+  int nbuf;
+  const int stages = tc_plan(9 * nchunks * p->nt * ROW_B, (int)a_stage_bytes_for(p, 0), p->nt * 128 * 2, nres, 0, &nbuf);
+  if (nbuf < 2 || stages < 2 * nchunks) return false;
+  const long work = (long)p->N * cdiv(p->W, TILE_W) * cdiv(p->H, TILE_H) * (p->cout / p->nt);
+  return work >= (long)TC2_SINGLE_WAVES * num_sms();
+}
+
 int dasr_conv_tc2_supported(const DasrConvTcParams* p) {
   // plain 3x3 fprop/dgrad geometry, staged bf16 epilogue; pre / residual tensors are announced through their channel
   // strides (pre_cs, res1_cs, res2_cs > 0), as dasr_conv_tc2 callers fill them
@@ -1572,8 +1598,10 @@ static int conv_tc2_run(const void* in, const void* w, const float* bias, const 
     return DASR_E_SMEM;
   }
   DasrConvTcParams q = *p;
+  if (tc2_single(p, (res1 ? 1 : 0) + (res2 ? 1 : 0), map))   // grid (SMs / (cout / nt), cout / nt), no cluster
+    return conv_tc_launch(in, w, bias, pre, res1, res2, nullptr, out, &q, stream, 0, true, map, map_w);
   q.nt = p->nt / 2;                     // per CTA; grid.y = cout / (nt / 2), consecutive CTAs form the clusters
-  return conv_tc_launch(in, w, bias, pre, res1, res2, nullptr, out, &q, stream, 1, map, map_w);
+  return conv_tc_launch(in, w, bias, pre, res1, res2, nullptr, out, &q, stream, 1, true, map, map_w);
 }
 
 int dasr_conv_tc2(const void* in, const void* w, const float* bias, const void* pre, const void* res1, const void* res2,

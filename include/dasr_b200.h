@@ -200,7 +200,12 @@ int dasr_conv_tc(const void* in_bf16, const void* w_packed_bf16, const float* bi
  * Supported: plain 3x3 geometry (dasr_conv_tc_setup kind 0/1), epi_mode 0; `nt` = Cout tile of a CTA pair (multiple of
  * 32, <= 256, divides cout; grid.y walks the tiles — VGG's 256/512-channel layers run as tiles of 32..128); pre / res1 /
  * res2 as in dasr_conv_tc (nullable).  dasr_conv_tc2_supported answers for the loads announced by pre_cs / res1_cs /
- * res2_cs > 0. */
+ * res2_cs > 0.
+ * The library plans the launch from its shape: it runs on one CTA per tile, with the whole Cout tile nt on each CTA, grid
+ * (SMs / (cout / nt), cout / nt) and no cluster, when nt is 16, 32 or 64, there is no dgrad mask (mask_c1 > mask_c0) and
+ * no weight map, the whole filter set still leaves two staging frames and the 32-channel A stages of two tiles, and the
+ * grid has at least 16 waves of work (N * ceil(H / 16) * ceil(W / 8) * cout / nt >= 16 * SMs).  Either way every output
+ * element sums the same products in the same order (that of 32-channel loads), so the results do not depend on the plan. */
 int dasr_conv_tc2_supported(const DasrConvTcParams* p);
 int dasr_conv_tc2(const void* in_bf16, const void* w_packed_bf16, const float* bias, const void* pre_bf16,
                   const void* res1_bf16, const void* res2_bf16, void* out_bf16, const DasrConvTcParams* p, void* stream);

@@ -1,4 +1,5 @@
-"""Per-stage device time of the dense-block launches of one forward (torch profiler, launch order folded modulo 5)."""
+"""Per-stage device time of the dense-block launches of one forward (torch profiler, launch order folded modulo 5), and
+of LR_conv and HR_conv0."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -23,3 +24,5 @@ trunk = durs[1:1 + 5 * 69]
 per = [sum(trunk[j::5]) / 69 for j in range(5)]
 print('stage us:', ' '.join('%.0f' % t for t in per), '| RDB %.0f us | trunk %.1f ms | other convs %.1f ms' %
       (sum(per), sum(trunk) / 1e3, (sum(durs) - sum(trunk)) / 1e3), flush=True)
+# after the trunk: LR_conv, the two upconvs, HR_conv0, HR_conv1
+print('LR_conv %.0f us | HR_conv0 %.0f us' % (durs[1 + 5 * 69], durs[1 + 5 * 69 + 3]), flush=True)
