@@ -126,9 +126,15 @@ SYMBOLS = {
 }
 
 # engine-internal entry points: exported by the library for the Python engines, not part of the public C ABI of
-# include/dasr_b200.h (the SRResNet mixed-precision backward's pixel-shuffle + ReLU gradient)
+# include/dasr_b200.h (the SRResNet mixed-precision backward's pixel-shuffle + ReLU gradient; the WGAN-GP penalty's
+# normalisation double backward and penalty reduction, csrc/grad_penalty.cu)
 INTERNAL_SYMBOLS = {
     'dasr_pixel_unshuffle_mask_bf16': (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),
+    'dasr_norm_lrelu_bwd2_workspace': (_sz, [_i, _l, _i]),
+    'dasr_instnorm_lrelu_bwd2': (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _f, _vp, _sz, _vp]),
+    'dasr_bn_lrelu_bwd2': (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _l, _i, _i, _f, _vp, _sz, _vp]),
+    'dasr_grad_penalty_workspace': (_sz, [_i, _l]),
+    'dasr_grad_penalty': (_i, [_vp, _vp, _vp, _f, _i, _l, _vp, _sz, _vp]),
 }
 
 

@@ -6,9 +6,9 @@ import warnings
 import torch
 from torch import nn
 
-from dasr_b200 import engine, ops
+from dasr_b200 import engine, ops, seqnet
 from dasr_b200.srn.models.modules.architecture import FilterLow
-from dasr_b200.srn.models.modules.loss import L1Loss, MSELoss, haar_split, mean
+from dasr_b200.srn.models.modules.loss import L1Loss, MSELoss, grad_penalty, haar_split, mean
 
 
 class _LogLoss(torch.autograd.Function):
@@ -45,12 +45,26 @@ def discriminator_loss(reals, fakes, wasserstein=False, grad_penalties=None, wei
         fakes = (fakes,)
     if weights is None:
         weights = [1.0 / len(fakes)] * len(fakes)
-    if wasserstein:
-        raise NotImplementedError('WGAN-GP (double backward through D) is not on the H100 path')
     loss = 0.0
+    if wasserstein:
+        if not isinstance(grad_penalties, list):
+            grad_penalties = (grad_penalties,)
+        for real, fake, weight, grad_penalty in zip(reals, fakes, weights, grad_penalties):
+            loss = loss + weight * (-1 * mean(real) + mean(fake) + grad_penalty)
+        return loss
     for real, fake, weight in zip(reals, fakes, weights):
         loss = loss + weight * (_LogLoss.apply(real, False) + _LogLoss.apply(fake, True))
     return loss
+
+
+def gradient_penalty(model_d, sample, weight=10.0):
+    """The WGAN-GP term of DSN/train.py:234-237, weight * (||d mean(D(sample)) / d sample||_2 - 1)^2 with the norm over the
+    whole batch, kept differentiable with respect to D's parameters.  sample must require grad."""
+    score = model_d(sample)
+    grad_outputs = torch.full_like(score, 1.0 / score.numel())       # d mean(score) / d score
+    with seqnet.input_gradient_only():
+        gradient = torch.autograd.grad(score, sample, grad_outputs, create_graph=True)[0]
+    return grad_penalty(gradient, 1, weight)
 
 
 VGG16_CFG = [64, 64, 'M', 128, 128, 'M', 256, 256, 256, 'M', 512, 512, 512, 'M', 512, 512, 512, 'M']

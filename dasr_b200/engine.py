@@ -1567,6 +1567,9 @@ class NLayerDFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dout):
+        if torch.is_grad_enabled():         # create_graph=True: this backward is not differentiable, refuse it loudly
+            raise NotImplementedError('double backward through the NLayer patch discriminator is not implemented (the WGAN-GP '
+                                      'penalty runs on the layer-list discriminators)')
         dx, grads = nlayer_d_backward(ctx.saved, [p.detach() for p in ctx.params], dout, ctx.need_dx, ctx.need_dw)
         ctx.saved = None
         return (dx, None) + tuple(grads)

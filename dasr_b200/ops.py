@@ -663,6 +663,44 @@ def bn_lrelu_bwd(x, y, dy, gamma, stats, dx, dgamma, dbeta, training, slope=0.2)
                                         int(bool(training)), slope, _stream()), 'bn_lrelu_bwd')
 
 
+def _check_bwd2(what, ref, named):
+    for name, t in named:
+        if t is not None and (tuple(t.shape) != tuple(ref.shape) or t.dtype != torch.float32):
+            raise _lib.DasrError('%s: %s is %s %s, the activation is fp32 %s' % (what, name, tuple(t.shape), t.dtype, tuple(ref.shape)))
+
+
+def instnorm_lrelu_bwd2(y, stats, g, v, dg, dz, slope=0.2):
+    """Double backward of InstanceNorm2d + LeakyReLU (NHWC fp32): dg = adjoint of the output gradient g, dz = gradient at
+    the pre-norm activation, for the adjoint v of the first backward's input gradient."""
+    _check_bwd2('instnorm_lrelu_bwd2', y, (('g', g), ('v', v), ('dg', dg), ('dz', dz)))
+    N, H, W, Cc = y.shape
+    lib = _lib.load()
+    ws = _workspace(lib.dasr_norm_lrelu_bwd2_workspace(N, H * W, Cc), y.device)
+    check(lib.dasr_instnorm_lrelu_bwd2(_p(y), _p(stats), _p(g), _p(v), _p(dg), _p(dz), N, H * W, Cc, slope, _p(ws), ws.numel(),
+                                       _stream()), 'instnorm_lrelu_bwd2', 3)
+
+
+def bn_lrelu_bwd2(x, y, gamma, stats, g, v, dg, dz, dgamma, training, slope=0.2):
+    """Double backward of BatchNorm2d + LeakyReLU (NHWC fp32); dgamma (nullable) is accumulated into."""
+    _check_bwd2('bn_lrelu_bwd2', x, (('y', y), ('g', g), ('v', v), ('dg', dg), ('dz', dz)))
+    M, Cc = x.numel() // x.shape[-1], x.shape[-1]
+    lib = _lib.load()
+    ws = _workspace(lib.dasr_norm_lrelu_bwd2_workspace(1, M, Cc), x.device)
+    check(lib.dasr_bn_lrelu_bwd2(_p(x), _p(y), _p(gamma), _p(stats), _p(g), _p(v), _p(dg), _p(dz), _p(dgamma), M, Cc,
+                                 int(bool(training)), slope, _p(ws), ws.numel(), _stream()), 'bn_lrelu_bwd2', 3)
+
+
+def grad_penalty(g, loss, grad, weight, groups):
+    """loss = weight * mean_k (||g_k|| - 1)^2 over `groups` equal slices of the fp32 tensor g; grad (nullable) its gradient."""
+    if g.dtype != torch.float32 or g.numel() % groups or (grad is not None and (grad.shape != g.shape or grad.dtype != g.dtype)):
+        raise _lib.DasrError('grad_penalty: g must be fp32 with a multiple of %d values and grad its shape' % groups)
+    lib = _lib.load()
+    n = g.numel() // groups
+    ws = _workspace(lib.dasr_grad_penalty_workspace(groups, n), g.device)
+    check(lib.dasr_grad_penalty(_p(g), _p(loss), _p(grad), float(weight), groups, n, _p(ws), ws.numel(), _stream()),
+          'grad_penalty', 3 if grad is not None else 2)
+
+
 def pixel_shuffle(src, dst, r, inverse=False):
     """nn.PixelShuffle(r) on NHWC fp32: src [N,H,W,C*r*r] -> dst [N,H*r,W*r,C]; inverse: dst [N,H,W,C*r*r] <- src [N,H*r,W*r,C]."""
     lo = dst if inverse else src

@@ -13,6 +13,8 @@ A net is a list of layer dicts:
   NHWC feature map it flattens (Linear(512*4*4, 100) after .view(N, -1) == conv k=4 with the weight viewed [100,512,4,4])
   {'op': 'res_begin'} ... {'op': 'res_end'}    y = x_at_begin + y
 """
+import contextlib
+
 import torch
 
 from . import ops
@@ -115,13 +117,13 @@ def forward_nhwc(a, layers, params, save=True):
     return acts[-1], ctx
 
 
-def backward(ctx, layers, params, dout, need_dx=True, need_dw=True):
+def backward(ctx, layers, params, dout, need_dx=True, need_dw=True, keep=None):
     """Returns (dx NCHW | None, grads list aligned with params (None where a param got no gradient))."""
     acts = ctx['acts']
     N, C0, H, W = ctx['shape']
     g = torch.empty(tuple(acts[-1].shape), dtype=torch.float32, device=dout.device)
     ops.nchw_to_nhwc(dout.contiguous().float(), g)
-    g, grads = backward_nhwc(ctx, layers, params, g, need_dx, need_dw)
+    g, grads = backward_nhwc(ctx, layers, params, g, need_dx, need_dw, keep=keep)
     dx = None
     if need_dx:
         dx = torch.empty((N, C0, H, W), dtype=torch.float32, device=dout.device)
@@ -129,16 +131,25 @@ def backward(ctx, layers, params, dout, need_dx=True, need_dw=True):
     return dx, grads
 
 
-def backward_nhwc(ctx, layers, params, g, need_dx=True, need_dw=True):
-    """g: NHWC fp32 gradient of the output (may be modified in place).  Returns (NHWC input gradient | None, grads)."""
+def backward_nhwc(ctx, layers, params, g, need_dx=True, need_dw=True, keep=None, inject=None, grads=None):
+    """g: NHWC fp32 gradient of the output (may be modified in place).  Returns (NHWC input gradient | None, grads).
+
+    For the double backward of the gradient penalty: `keep` (a dict) receives, per conv / norm layer index, the gradient
+    that layer back-propagated (a conv's after its activation mask, a norm's as it reached the norm's output).  `inject`
+    ({layer index: NHWC tensor}) adds a gradient at the input of those layers; then g is None, the sweep starts at the
+    topmost injection and accumulates into `grads`, the parameter gradients of the tangent sweep."""
     acts, aux = ctx['acts'], ctx['aux']
-    dout = g
-    grads = [None] * len(params)
+    dout = acts[0] if g is None else g
+    grads = [None] * len(params) if grads is None else grads
     skip_stack = []
     first_conv = next(i for i, L in enumerate(layers) if L['op'] == 'conv')
-    for li in reversed(range(len(layers))):
+    top = len(layers) if inject is None else max(inject) + 1
+    for li in reversed(range(top)):
         L = layers[li]
         op = L['op']
+        if g is None:                       # the topmost injection: nothing reached this layer's output
+            g = inject[li]
+            continue
         if op == 'conv':
             if L.get('act', ACT_NONE) == ACT_LRELU:
                 if skip_stack and skip_stack[-1] is g:
@@ -152,7 +163,14 @@ def backward_nhwc(ctx, layers, params, g, need_dx=True, need_dw=True):
                 if skip_stack and skip_stack[-1] is g:
                     g = g.clone()
                 ops.act_bwd(g, acts[li + 1], 0.0)
-            if need_dw:
+            if keep is not None:
+                keep[li] = g
+            if need_dw and grads[L['w']] is not None:       # second sweep of the double backward
+                ops.conv2d_wgrad_f32(acts[li], g, grads[L['w']].view_as(wt), None, L['k'], L['s'], L['p'], accumulate=True)
+                if L['b'] is not None:
+                    grads[L['b']] = torch.empty_like(params[L['b']], dtype=torch.float32)
+                    ops.bias_grad(g, grads[L['b']])
+            elif need_dw:
                 gw = torch.empty_like(wt, dtype=torch.float32)
                 grads[L['w']] = gw.view_as(params[L['w']])
                 db = None
@@ -178,15 +196,22 @@ def backward_nhwc(ctx, layers, params, g, need_dx=True, need_dw=True):
                 grads[L['a']] = da
             g = gz
         elif op == 'in_lrelu':
+            if keep is not None:
+                keep[li] = g
             gz = torch.empty_like(g)
             ops.instnorm_lrelu_bwd(acts[li + 1], aux[li], g, gz, 0.2)
             g = gz
         elif op == 'bn_lrelu':
+            if keep is not None:
+                keep[li] = g
             gz = torch.empty_like(g)
             dgm = torch.empty_like(params[L['w']], dtype=torch.float32) if need_dw else None
             dbt = torch.empty_like(params[L['b']], dtype=torch.float32) if need_dw else None
             ops.bn_lrelu_bwd(acts[li], acts[li + 1], g, params[L['w']], aux[li], gz, dgm, dbt, L['training'], L.get('slope', 0.2))
-            if need_dw:
+            if need_dw and grads[L['w']] is not None:       # second sweep: add to the tangent sweep's gamma term
+                ops.axpby(dgm, 1.0, grads[L['w']], 1.0, grads[L['w']])
+                grads[L['b']] = dbt
+            elif need_dw:
                 grads[L['w']], grads[L['b']] = dgm, dbt
             g = gz
         elif op == 'sigmoid':
@@ -206,6 +231,8 @@ def backward_nhwc(ctx, layers, params, g, need_dx=True, need_dw=True):
         elif op == 'res_begin':
             gs = skip_stack.pop()
             ops.axpby(g, 1.0, gs, 1.0, g)
+        if inject is not None and li in inject:
+            ops.axpby(g, 1.0, inject[li], 1.0, g)
     return (g if need_dx else None), grads
 
 
@@ -217,14 +244,120 @@ class SeqFunction(torch.autograd.Function):
         ctx.need_dx = x.requires_grad
         ctx.need_dw = any(p.requires_grad for p in params)
         out, saved = forward(x, layers, [p.detach() for p in params], save=ctx.need_dx or ctx.need_dw)
-        ctx.saved, ctx.params, ctx.layers = saved, params, layers
+        ctx.saved, ctx.params, ctx.layers, ctx.x = saved, params, layers, x
         return out
 
     @staticmethod
     def backward(ctx, dout):
+        if torch.is_grad_enabled():         # create_graph=True: the gradient penalty differentiates this backward
+            out = _SeqBackward.apply(ctx, ctx.need_dw and not _INPUT_GRADIENT_ONLY[0], dout, ctx.x, *ctx.params)
+            return (out[0], None) + tuple(out[1:])
         # ctx.saved is kept: the DSN iteration back-propagates through D(fake) twice (D loss, then G loss)
         dx, grads = backward(ctx.saved, ctx.layers, [p.detach() for p in ctx.params], dout, ctx.need_dx, ctx.need_dw)
         return (dx, None) + tuple(grads)
+
+
+_INPUT_GRADIENT_ONLY = [0]
+
+
+@contextlib.contextmanager
+def input_gradient_only():
+    """For an autograd.grad(D(x), x, create_graph=True) inside the block, which asks for the input gradient only (the
+    gradient penalty): the layer-list nodes skip the filter gradients of that first backward and return None for them.
+    A plain flag rather than a thread-local one: the backward runs on autograd's device threads while the caller waits."""
+    _INPUT_GRADIENT_ONLY[0] += 1
+    try:
+        yield
+    finally:
+        _INPUT_GRADIENT_ONLY[0] -= 1
+
+
+# ops whose second derivative the layer-list executor does not implement (none occurs in a discriminator)
+_NO_DOUBLE_BACKWARD = ('prelu', 'sigmoid', 'pixel_shuffle', 'res_begin', 'res_end')
+
+
+class _SeqBackward(torch.autograd.Function):
+    """The backward of a SeqFunction as a differentiable node: (dout, x, *params) -> (dx, *param grads).
+
+    Its own backward takes the adjoint v of dx (the gradient penalty never differentiates the parameter gradients) and
+    returns the gradients of <v, dx> for dout, x and the parameters in two sweeps:
+      1. tangent sweep in layer order: u = v is pushed forward through the linearised net (u <- conv(u, W) masked by a
+         fused activation; dg of instnorm_lrelu_bwd2 / bn_lrelu_bwd2 at the norms), adding wgrad(u_in, g_out) to each
+         conv's filter gradient and the gamma term at BatchNorms; each norm also yields dz, the gradient at its input;
+      2. the first-order backward sweep of the dz injections, from the topmost one down, accumulating into the same
+         parameter gradients and giving the gradient for x.
+    The tangent that leaves the top layer is the gradient for dout."""
+
+    @staticmethod
+    def forward(ctx, st, need_dw, dout, x, *params):
+        ctx.set_materialize_grads(False)
+        keep = {}
+        dx, grads = backward(st.saved, st.layers, [p.detach() for p in params], dout, st.need_dx, need_dw, keep=keep)
+        ctx.st, ctx.keep = st, keep
+        return (dx,) + tuple(grads)
+
+    @staticmethod
+    def backward(ctx, v_dx, *v_params):
+        st, keep = ctx.st, ctx.keep
+        layers = st.layers
+        if any(v is not None for v in v_params):
+            raise NotImplementedError('double backward through a parameter gradient of a layer-list network')
+        if v_dx is None:
+            return (None,) * (4 + len(v_params))
+        for L in layers:
+            if L['op'] in _NO_DOUBLE_BACKWARD or L.get('ups', 1) != 1:
+                raise NotImplementedError('double backward through %s is not implemented' % (
+                    'an upsampling conv' if L['op'] == 'conv' else 'a residual block' if L['op'].startswith('res') else L['op']))
+        params = [p.detach() for p in st.params]
+        acts, aux = st.saved['acts'], st.saved['aux']
+        dev = v_dx.device
+        u = torch.empty(tuple(acts[0].shape), dtype=torch.float32, device=dev)
+        ops.nchw_to_nhwc(v_dx.contiguous().float(), u)
+        grads, inject = [None] * len(params), {}
+        need_dout = ctx.needs_input_grad[2]
+        for li, L in enumerate(layers):
+            op = L['op']
+            if op == 'conv':
+                wt = params[L['w']]
+                if L.get('view') is not None:
+                    wt = wt.view(*L['view'])
+                gw = torch.empty_like(wt, dtype=torch.float32)
+                grads[L['w']] = gw.view_as(params[L['w']])
+                ops.conv2d_wgrad_f32(u, keep[li], gw, None, L['k'], L['s'], L['p'])
+                if li == len(layers) - 1 and not need_dout:
+                    break
+                o = torch.empty(tuple(acts[li + 1].shape), dtype=torch.float32, device=dev)
+                ops.conv2d_f32(u, ops.pack_filter_f32(wt), None, o, L['k'], L['s'], L['p'])
+                act = L.get('act', ACT_NONE)
+                if act != ACT_NONE:
+                    ops.act_bwd(o, acts[li + 1], 0.2 if act == ACT_LRELU else 0.0)
+                u = o
+            elif op == 'in_lrelu':
+                dg, dz = torch.empty_like(u), torch.empty_like(u)
+                ops.instnorm_lrelu_bwd2(acts[li + 1], aux[li], keep[li], u, dg, dz, 0.2)
+                inject[li], u = dz, dg
+            elif op == 'bn_lrelu':
+                dg = torch.empty_like(u)
+                dz = torch.empty_like(u) if L['training'] else None
+                dgm = grads[L['w']] = torch.zeros_like(params[L['w']], dtype=torch.float32)
+                ops.bn_lrelu_bwd2(acts[li], acts[li + 1], params[L['w']], aux[li], keep[li], u, dg, dz, dgm, L['training'],
+                                  L.get('slope', 0.2))
+                if dz is not None:
+                    inject[li] = dz
+                u = dg
+        d_dout = None
+        if need_dout:
+            d_dout = torch.empty(st.saved['acts'][-1].shape[:1] + (u.shape[3], u.shape[1], u.shape[2]), dtype=torch.float32,
+                                 device=dev)
+            ops.nhwc_to_nchw(u, d_dout)
+        d_x = None
+        if inject:
+            need_x = ctx.needs_input_grad[3]
+            gx, grads = backward_nhwc(st.saved, layers, params, None, need_x, True, inject=inject, grads=grads)
+            if need_x:
+                d_x = torch.empty(st.saved['shape'], dtype=torch.float32, device=dev)
+                ops.nhwc_to_nchw(gx, d_x)
+        return (None, None, d_dout, d_x) + tuple(grads)
 
 
 # --------------------------------------------------------------------------------------------------

@@ -78,7 +78,11 @@ class DASR_Model(BaseModel):
         if self.is_train:
             self.cri_gan = L.GANLoss(train_opt['gan_type'], 1.0, 0.0).to(self.device)
             if train_opt['gan_type'] == 'wgan-gp':
-                raise NotImplementedError('wgan-gp gradient penalty (double backward) is not on the H100 path')
+                # built as in the reference (DASR_model.py:114-118), whose step never applies it (:319 is commented
+                # out): with wgan-gp the step trains on the Wasserstein critic losses alone
+                self.random_pt = torch.Tensor(1, 1, 1, 1).to(self.device)
+                self.cri_gp = L.GradientPenaltyLoss(device=self.device).to(self.device)
+                self.l_gp_w = train_opt['gp_weigth']
 
         self.netG = networks.define_G(opt).to(self.device)
         if self.is_train:

@@ -6,7 +6,11 @@ Same attributes / methods / log keys / checkpoint names (`{iter}_G.pth`, `{iter}
 the dasr_b200 kernels; the relativistic terms `pred - mean(other)` are arithmetic on the [N, 1] logits.  Differences, all
 behaviour-preserving: while G's loss is back-propagated through D, D's filter gradients (which the reference computes and
 then discards with optimizer_D.zero_grad()) are not computed; the BatchNorm running statistics of D see the same sequence
-of forward passes as in the reference (2 + 2 per step, 1 + 2 for SRGAN).  wgan-gp (double backward) raises."""
+of forward passes as in the reference (2 + 2 per step, 1 + 2 for SRGAN, one more D forward with wgan-gp).
+
+gan_type wgan-gp adds the reference's gradient penalty (SRRaGAN_model.py:156-165): gp_weigth * GradientPenaltyLoss at
+interp = r * fake_H + (1 - r) * var_ref, one uniform r per sample drawn on the device, differentiated twice through
+the layer-list discriminator; logged as l_d_gp."""
 import logging
 from collections import OrderedDict
 
@@ -52,7 +56,12 @@ class SRRaGANModel(BaseModel):
             else:
                 self.netF = networks.define_F(opt, use_bn=False).to(self.device)
             if train_opt['gan_type'] == 'wgan-gp':
-                raise NotImplementedError('wgan-gp gradient penalty (double backward) is not on the H100 path')
+                if opt['network_D']['which_model_D'] == 'discriminator_patch':
+                    raise NotImplementedError('wgan-gp needs a twice-differentiable discriminator: discriminator_vgg_128 / '
+                                              '_192 (the NLayer patch discriminator has no double backward)')
+                self.random_pt = torch.Tensor(1, 1, 1, 1).to(self.device)
+                self.cri_gp = L.GradientPenaltyLoss(device=self.device).to(self.device)
+                self.l_gp_w = train_opt['gp_weigth']
             self.cri_gan = L.GANLoss(train_opt['gan_type'], 1.0, 0.0).to(self.device)
             self.l_gan_w = train_opt['gan_weight']
             self.D_update_ratio = train_opt['D_update_ratio'] or 1
@@ -109,6 +118,17 @@ class SRRaGANModel(BaseModel):
             l_d_real = self.cri_gan(pred_d_real, True)
             l_d_fake = self.cri_gan(pred_d_fake, False)
             l_d_total = l_d_real + l_d_fake
+        wgan_gp = self.opt['train']['gan_type'] == 'wgan-gp'
+        if wgan_gp:
+            batch_size = self.var_ref.size(0)
+            if self.random_pt.size(0) != batch_size:
+                self.random_pt.resize_(batch_size, 1, 1, 1)
+            self.random_pt.uniform_()
+            interp = self.random_pt * self.fake_H.detach() + (1 - self.random_pt) * self.var_ref
+            interp.requires_grad = True
+            interp_crit = self.netD(interp)
+            l_d_gp = self.l_gp_w * self.cri_gp(interp, interp_crit)
+            l_d_total = l_d_total + l_d_gp
         l_d_total.backward()
         self.optimizer_D.step()
         if do_g:
@@ -119,6 +139,8 @@ class SRRaGANModel(BaseModel):
             self.log_dict['l_g_gan'] = l_g_gan.item()
         self.log_dict['l_d_real'] = l_d_real.item()
         self.log_dict['l_d_fake'] = l_d_fake.item()
+        if wgan_gp:
+            self.log_dict['l_d_gp'] = l_d_gp.item()
         self.log_dict['D_real'] = torch.mean(pred_d_real.detach())
         self.log_dict['D_fake'] = torch.mean(pred_d_fake.detach())
 

@@ -368,6 +368,8 @@ class _DWFilterFunction(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dout):
         taps, k, mode, include_pad, valid, shape = ctx.cfg
+        if torch.is_grad_enabled():         # create_graph=True (gradient penalty): a differentiable backward
+            return (_DWFilterBackward.apply(dout, ctx.cfg), None, None, None, None, None)
         dout = dout.contiguous().float()
         if valid:
             p = (k - 1) // 2
@@ -377,6 +379,35 @@ class _DWFilterFunction(torch.autograd.Function):
         dx = torch.empty_like(dout)
         ops.dwfilter(dout, dx, taps, k, mode, include_pad, backward=True)
         return dx, None, None, None, None, None
+
+
+class _DWFilterBackward(torch.autograd.Function):
+    """The backward of _DWFilterFunction as a node of its own, for the gradient penalty's double backward.  The backward
+    is linear in dout; its transpose is the forward filter without the 0.5 offset: mode 0 -> low(v), mode 1 ->
+    0.5 v - 0.5 low(v).  (A box filter without count_include_pad is not self-adjoint, so the forward, not the backward,
+    kernel is the transpose.)"""
+
+    @staticmethod
+    def forward(ctx, dout, cfg):
+        taps, k, mode, include_pad, valid, shape = cfg
+        if valid:
+            raise NotImplementedError('double backward of the un-padded filter is not implemented')
+        ctx.cfg = cfg
+        dx = torch.empty(shape, dtype=torch.float32, device=dout.device)
+        ops.dwfilter(dout.contiguous().float(), dx, taps, k, mode, include_pad, backward=True)
+        return dx
+
+    @staticmethod
+    def backward(ctx, v):
+        taps, k, mode, include_pad, _, _ = ctx.cfg
+        v = v.contiguous().float()
+        low = torch.empty_like(v)
+        ops.dwfilter(v, low, taps, k, 0, include_pad)
+        if mode == 0:
+            return low, None
+        out = torch.empty_like(v)
+        ops.axpby(v, 0.5, low, -0.5, out)
+        return out, None
 
 
 class GaussianFilter(nn.Module):
