@@ -127,8 +127,14 @@ SYMBOLS = {
 
 # engine-internal entry points: exported by the library for the Python engines, not part of the public C ABI of
 # include/dasr_b200.h (the SRResNet mixed-precision backward's pixel-shuffle + ReLU gradient; the WGAN-GP penalty's
-# normalisation double backward and penalty reduction, csrc/grad_penalty.cu)
+# normalisation double backward and penalty reduction, csrc/grad_penalty.cu; the adaptive generators' weight-map
+# gradients and bf16 map product, csrc/map_bwd.cu)
 INTERNAL_SYMBOLS = {
+    'dasr_map_channel_dgrad_bf16': (_i, [_vp, _i, _i, _vp, _vp, _i, _i, _i, _i, _f, _i, _vp]),
+    'dasr_map_channel_wgrad_workspace': (_sz, [_i, _i, _i, _i]),
+    'dasr_map_channel_wgrad_bf16': (_i, [_vp, _i, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _i, _vp, _sz, _vp]),
+    'dasr_map_scale_bwd': (_i, [_vp, _i, _i, _vp, _i, _i, _vp, _vp, _i, _i, _vp, _l, _i, _i, _i, _vp]),
+    'dasr_map_axpby_bf16': (_i, [_vp, _vp, _vp, _vp, _l, _i, _i, _i, _i, _i, _i, _i, _f, _f, _vp]),
     'dasr_pixel_unshuffle_mask_bf16': (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     'dasr_norm_lrelu_bwd2_workspace': (_sz, [_i, _l, _i]),
     'dasr_instnorm_lrelu_bwd2': (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _f, _vp, _sz, _vp]),

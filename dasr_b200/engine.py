@@ -148,8 +148,9 @@ def rrdb_forward_f32(x, params, nb, upscale=4, save=False):
     return out, ctx
 
 
-def rrdb_backward_f32(ctx, params, dout, need_dx=False):
-    """Returns (dx or None, [grad for every param in order])."""
+def rrdb_backward_f32(ctx, params, dout, need_dx=False, ada=None):
+    """Returns (dx or None, [grad for every param in order]).  ada: the _AdaptiveBackward of an adaptive generator, whose
+    first ada.n_rdb dense blocks belong to its adaptive blocks (see _AdaptiveBackward)."""
     L = ctx['L']
     nf = L.nf
     N, in_nc, H, W = ctx['shape']
@@ -201,7 +202,10 @@ def rrdb_backward_f32(ctx, params, dout, need_dx=False):
     for r in reversed(range(n_rdb)):
         b = bufs[r]
         last = (r % 3 == 2)
-        if last:
+        in_ada = ada is not None and r < ada.n_rdb
+        if in_ada:
+            g_y, a5, b1 = ada.enter(r, g_y, grads)
+        elif last:
             a5, b1 = 0.04, 0.2
             g_rrdb = g_y                                     # d out / d x_rrdb = 1 (beta2)
         else:
@@ -225,7 +229,7 @@ def rrdb_backward_f32(ctx, params, dout, need_dx=False):
             g_rrdb = None
         else:
             ops.axpby(View(GB, nf, 0), 1.0, None, 0.0, g_new)
-        g_y = g_new
+        g_y = ada.leave(r, g_new, grads) if in_ada else g_new
     # fea: trunk input gradient + the ShortcutBlock skip
     g_fea = _empty((N, H, W, nf), dev)
     ops.axpby(g_y, 1.0, g_lr, 1.0, g_fea)
@@ -958,9 +962,12 @@ def adaptive_rrdb_forward_bf16(x, amap, params, nb, nb_ada, concat, upscale=4, c
     return _trunk_tail_bf16(bufs, fea, L, params, cache, wk, bk, hk, bf)[0]
 
 
-def adaptive_rrdb_forward_f32(x, amap, params, nb, nb_ada, concat, upscale=4):
+def adaptive_rrdb_forward_f32(x, amap, params, nb, nb_ada, concat, upscale=4, save=False):
     """fp32 twin of adaptive_rrdb_forward_bf16 (the parity path): the 65-channel convs run on a materialised
-    [u | s * map] concat, the plain variant's map product is one elementwise kernel."""
+    [u | s * map] concat, the plain variant's map product is one elementwise kernel.
+    save: also keep what adaptive_rrdb_backward_f32 reads and return (out, ctx): every dense block in its own buffer (the x
+    slot of an adaptive concat block then holds A's output y_k, the dense block's input), each materialised [t | s * map]
+    input of A.0 and R.0, the outputs of A.0, R.0 and R.2, and for plain blocks the pre-map t3 = RDB3(...)."""
     a = _check_map(x, amap, nb, nb_ada)
     L = RRDBLayout(nb + nb_ada, params[0].shape[0], upscale)
     nf = L.nf
@@ -968,36 +975,49 @@ def adaptive_rrdb_forward_f32(x, amap, params, nb, nb_ada, concat, upscale=4):
     Bs = lambda i: params[2 * i + 1]
     pk = lambda i: ops.pack_filter_f32(params[2 * i])
     ext = _ada_ext(L, concat)
+    new = lambda c=nf: _empty((N, H, W, c), x)
 
     def conv64(src, i, dst):
         ops.conv2d_f32(src, pk(i), Bs(i), dst, 3, 1, 1, act=ACT_LRELU, slope=0.2)
 
-    cat = _empty((N, H, W, nf + 1), x) if concat else None
+    cat = new(nf + 1) if concat and not save else None
 
-    def conv_cat(src, s, i, dst):   # conv(cat(src, s * map)) + LeakyReLU  (block.py:524-527)
-        ops.axpby(src, 1.0, None, 0.0, View(cat, nf, 0))
-        ops.map_axpby(None, a, s, None, 0.0, View(cat, 1, nf))
-        conv64(cat, i, dst)
+    def conv_cat(src, s, i, dst):   # conv(cat(src, s * map)) + LeakyReLU  (block.py:524-527); returns the concat
+        c = new(nf + 1) if save else cat
+        ops.axpby(src, 1.0, None, 0.0, View(c, nf, 0))
+        ops.map_axpby(None, a, s, None, 0.0, View(c, 1, nf))
+        conv64(c, i, dst)
+        return c
 
-    xin = _empty((N, H, W, in_nc), x)
+    xin = new(in_nc)
     ops.nchw_to_nhwc(x.contiguous().float(), xin)
-    fea = _empty((N, H, W, nf), x)
+    fea = new()
     ops.conv2d_f32(xin, pk(L.i_fea), Bs(L.i_fea), fea, 3, 1, 1)
     n_rdb = L.n_rdb
-    rot = [_empty((N, H, W, nf + 4 * GC), x) for _ in range(3)]
-    bufs = [rot[i % 3] for i in range(n_rdb + 1)]
-    tmp, res = _empty((N, H, W, nf), x), _empty((N, H, W, nf), x)
+    if save:
+        bufs = [new(nf + 4 * GC) for _ in range(n_rdb)] + [new()]
+        tmp = res = None
+    else:
+        rot = [new(nf + 4 * GC) for _ in range(3)]
+        bufs = [rot[i % 3] for i in range(n_rdb + 1)]
+        tmp, res = new(), new()
+    sv = dict(a=a, concat=concat, nb_ada=nb_ada, cat=[None] * n_rdb, tA=[None] * n_rdb, catR=[], tmpR=[], res=[], t3=[])
     ops.axpby(fea, 1.0, None, 0.0, View(bufs[0], nf, 0))
     for r in range(n_rdb):
         b, blk = bufs[r], r // 3
         u, dst = View(b, nf, 0), View(bufs[r + 1], nf, 0)
         tail = _rrdb_tail(bufs, r, nf)
+        if save and blk < nb_ada and r % 3 == 0:
+            tmp, res = new(), new()
+            sv['tmpR'].append(tmp)
+            sv['res'].append(res)
         if blk < nb_ada and concat:
             if r % 3 == 0:
-                conv_cat(u, 1.0, ext(blk, 2), tmp)
+                sv['catR'].append(conv_cat(u, 1.0, ext(blk, 2), tmp))
                 conv64(tmp, ext(blk, 3), res)
-            conv_cat(u, 0.2, ext(blk, 0), tmp)
-            conv64(tmp, ext(blk, 1), u)
+            tA = sv['tA'][r] = new() if save else tmp
+            sv['cat'][r] = conv_cat(u, 0.2, ext(blk, 0), tA)
+            conv64(tA, ext(blk, 1), u)
             if r % 3 == 2:
                 tail = dict(alpha=0.04, res1=u, beta1=0.2, res2=res, beta2=1.0)
         elif blk < nb_ada:
@@ -1005,12 +1025,142 @@ def adaptive_rrdb_forward_f32(x, amap, params, nb, nb_ada, concat, upscale=4):
                 conv64(u, ext(blk, 0), tmp)
                 conv64(tmp, ext(blk, 1), res)
             if r % 3 == 2:      # RRDB3chain(u) * a + 0.1 * R(u)
-                _rdb_f32(b, tmp, r, L, pk, Bs, dict(alpha=0.2, res1=u, beta1=1.0))
-                ops.map_axpby(tmp, a, 1.0, res, 0.1, dst)
+                t3 = new() if save else tmp
+                _rdb_f32(b, t3, r, L, pk, Bs, dict(alpha=0.2, res1=u, beta1=1.0))
+                ops.map_axpby(t3, a, 1.0, res, 0.1, dst)
+                sv['t3'].append(t3)
                 continue
         _rdb_f32(b, dst, r, L, pk, Bs, tail)
-    out, _, _ = _trunk_tail_f32(View(bufs[n_rdb], nf, 0), fea, L, params, pk, Bs)
-    return out
+    out, ups, h0 = _trunk_tail_f32(View(bufs[n_rdb], nf, 0), fea, L, params, pk, Bs)
+    if not save:
+        return out
+    return out, dict(L=L, xin=xin, fea=fea, bufs=bufs, ups=ups, h0=h0, shape=(N, in_nc, H, W), ada=sv)
+
+
+class _AdaptiveBackward:
+    """The adaptive blocks of an adaptive generator inside rrdb_backward_f32 / rrdb_backward_bf16, whose dense-block loop
+    calls enter(r, g, grads) before dense block r (r < n_rdb) and leave(r, g, grads) after it.
+      enter: the gradient of the block's output becomes that of its last dense block.  concat (out = 0.2 t3 + R([u | a])):
+             conv5's epilogue scale 0.04, the skip 0.2, and the output gradient reaches R's output unscaled.  plain
+             (out = a * t3 + 0.1 R(u)): g_t3 = a * g and the map gradient <g, t3> per pixel (map_scale_bwd), R gets 0.1 g.
+             Neither variant has the RRDB's identity skip.
+      leave: concat: the gradient of the dense block's input y_k = A(t_{k-1}) goes back through A.2, A.0 to t_{k-1} (A's filter
+             and bias gradients accumulate over its three uses), and at the first dense block R's chain adds its share of
+             the block input's gradient; plain: R's chain at the first dense block.
+    A map conv's gradient reaches the map through its map input channel, scale s (A: 0.2, R: 1).  fp32: the materialised
+    65-channel input, a 65-channel dgrad whose channel 64 times s joins the map gradient.  bf16: the 64-channel part on the
+    wgmma dgrad / wgrad kernels, the map channel on map_channel_dgrad / map_channel_wgrad."""
+
+    def __init__(self, ctx, params, need_map, bf16, cache=None):
+        sv = ctx['ada']
+        self.sv, self.params, self.bufs, self.a = sv, params, ctx['bufs'], sv['a']
+        self.concat, self.n_rdb = sv['concat'], 3 * sv['nb_ada']
+        self.nf = ctx['L'].nf
+        self.ext = _ada_ext(ctx['L'], self.concat)
+        self.bf16, self.cache = bf16, cache
+        N, _, H, W = ctx['shape']
+        self.shape, self.dev = (N, H, W), ctx['fea']
+        self.dtype = torch.bfloat16 if bf16 else torch.float32
+        self.gmap = torch.zeros((N, 1, H, W), dtype=torch.float32, device=ctx['fea'].device) if need_map else None
+        self.g_res = None
+        self.tmpW = {}
+
+    def _new(self, c=None):
+        return _empty(self.shape + (c or self.nf,), self.dev, self.dtype)
+
+    def enter(self, r, g, grads):
+        if r % 3 != 2:
+            return g, 0.2, 1.0
+        if self.concat:
+            self.g_res = g
+            return g, 0.04, 0.2
+        g_t3, self.g_res = self._new(), self._new()
+        ops.map_scale_bwd(g, self.sv['t3'][r // 3], self.a, g_t3, self.gmap, accumulate=True)
+        ops.axpby(g, 0.1, None, 0.0, self.g_res)
+        return g_t3, 0.2, 1.0
+
+    def leave(self, r, g, grads):
+        blk, k = r // 3, r % 3
+        sv, u = self.sv, View(self.bufs[r], self.nf, 0)
+        if self.concat:
+            inp = sv['cat'][r] if not self.bf16 else sv['tin'][r]
+            g = self._chain(grads, g, u, sv['tA'][r], inp, self.ext(blk, 0), self.ext(blk, 1), 0.2, k != 2, None)
+            if k == 0:
+                inp = sv['catR'][blk] if not self.bf16 else sv['tin'][r]
+                g = self._chain(grads, self.g_res, sv['res'][blk], sv['tmpR'][blk], inp, self.ext(blk, 2), self.ext(blk, 3),
+                                1.0, False, g)
+        elif k == 0:
+            g = self._chain(grads, self.g_res, sv['res'][blk], sv['tmpR'][blk], u, self.ext(blk, 0), self.ext(blk, 1), None,
+                            False, g)
+        return g
+
+    def _chain(self, grads, g_y, y, h, inp, i1, i2, s, acc, add):
+        """y = lrelu(conv i2 (h)), h = lrelu(conv i1 (inp)), conv i1 with the map channel s * a (s None: none); g_y = the
+        gradient of y (overwritten).  Filter / bias gradients into grads (acc: accumulated), the map channel's share into
+        the map gradient; returns the gradient of inp's first nf channels, plus `add`."""
+        nf, W = self.nf, self.params
+        ops.act_bwd(g_y, y, 0.2)
+        self._wgrad(grads, h, g_y, i2, acc)
+        g_h = self._new()
+        self._dgrad(g_y, i2, g_h)
+        ops.act_bwd(g_h, h, 0.2)
+        if s is None:
+            self._wgrad(grads, inp, g_h, i1, acc)
+            g_in = self._new()
+            self._dgrad(g_h, i1, g_in, add)
+            return g_in
+        if not self.bf16:           # inp is the materialised [t | s * a]
+            ops.conv2d_wgrad_f32(inp, g_h, grads[2 * i1], grads[2 * i1 + 1], 3, 1, 1, accumulate=acc)
+            g65 = self._new(nf + 1)
+            ops.conv2d_f32(g_h, ops.pack_filter_f32(W[2 * i1], for_dgrad=True), None, g65, 3, 1, 1, mode=DGRAD)
+            if self.gmap is not None:
+                gm = self.gmap.view(self.shape + (1,))
+                ops.axpby(View(g65, 1, nf), s, gm, 1.0, gm)
+            if add is None:
+                return View(g65, nf, 0)
+            g_in = self._new()
+            ops.axpby(View(g65, nf, 0), 1.0, add, 1.0, g_in)
+            return g_in
+        w = W[2 * i1]
+        tmp = self.tmpW.get(i1)
+        if tmp is None:
+            tmp = self.tmpW[i1] = torch.empty((w.shape[0], nf, 3, 3), dtype=torch.float32, device=w.device)
+        ops.conv3x3_wgrad_tc(inp, g_h, tmp, accumulate=acc)
+        grads[2 * i1][:, :nf].copy_(tmp)
+        ops.map_channel_wgrad(g_h, self.a, s, grads[2 * i1], nf, accumulate=acc)
+        ops.bias_grad(g_h, grads[2 * i1 + 1], accumulate=acc)
+        g_in = self._new()
+        wd = self.cache.get(('wd64', i1), w, lambda: ops.pack_filter_tc(w.detach()[:, :nf].float().contiguous(), TC_DGRAD))
+        ops.conv_tc(g_h, wd, None, g_in, kind=TC_DGRAD, nt=_pick_nt(nf, nf), pre=add)
+        if self.gmap is not None:
+            taps = self.cache.get(('wmt', i1), w, lambda: ops.map_channel_taps(w, nf))
+            ops.map_channel_dgrad(g_h, taps, s, self.gmap, accumulate=True)
+        return g_in
+
+    def _wgrad(self, grads, x, g, i, acc):
+        if self.bf16:
+            ops.conv3x3_wgrad_tc(x, g, grads[2 * i], accumulate=acc)
+            ops.bias_grad(g, grads[2 * i + 1], accumulate=acc)
+        else:
+            ops.conv2d_wgrad_f32(x, g, grads[2 * i], grads[2 * i + 1], 3, 1, 1, accumulate=acc)
+
+    def _dgrad(self, g, i, out, add=None):
+        w = self.params[2 * i]
+        if self.bf16:
+            wd = self.cache.get(('wd', i), w, lambda: ops.pack_filter_tc(w.float(), TC_DGRAD))
+            ops.conv_tc(g, wd, None, out, kind=TC_DGRAD, nt=_pick_nt(self.nf, self.nf), pre=add)
+        elif add is None:
+            ops.conv2d_f32(g, ops.pack_filter_f32(w, for_dgrad=True), None, out, 3, 1, 1, mode=DGRAD)
+        else:
+            ops.conv2d_f32(g, ops.pack_filter_f32(w, for_dgrad=True), None, out, 3, 1, 1, mode=DGRAD, res1=add, beta1=1.0)
+
+
+def adaptive_rrdb_backward_f32(ctx, params, dout, need_dx=False, need_map=True):
+    """Backward of adaptive_rrdb_forward_f32(..., save=True): (dx or None, map gradient [N, 1, H, W] fp32 or None, [grad for
+    every param in order])."""
+    ada = _AdaptiveBackward(ctx, params, need_map, False)
+    dx, grads = rrdb_backward_f32(ctx, params, dout, need_dx, ada=ada)
+    return dx, ada.gmap, grads
 
 
 # ---- bf16 wgmma training (mixed precision: bf16 activations/gradients, fp32 accumulation, fp32 filter grads) ----
@@ -1071,10 +1221,11 @@ def _grad_arena(params, device, flat, who):
     return grads, flat, b_off
 
 
-def rrdb_backward_bf16(ctx, params, dout, cache=None, flat=None):
+def rrdb_backward_bf16(ctx, params, dout, cache=None, flat=None, ada=None):
     """Backward of the mixed-precision mode: input gradients (dgrad) on the wgmma kernel (3x3 conv with flipped,
     transposed filters; gradient contributions of a dense block accumulate in place in one bf16 buffer), filter
-    gradients on the wgmma wgrad kernel (MN-major operands straight from the NHWC tiles, fp32 register accumulation).  Returns fp32 grads."""
+    gradients on the wgmma wgrad kernel (MN-major operands straight from the NHWC tiles, fp32 register accumulation).  Returns fp32 grads.
+    ada: the _AdaptiveBackward of an adaptive generator (see rrdb_backward_f32)."""
     L = ctx['L']
     nf = L.nf
     N, in_nc, H, W = ctx['shape']
@@ -1161,7 +1312,10 @@ def rrdb_backward_bf16(ctx, params, dout, cache=None, flat=None):
         GB, g_x5 = GBs[idx % nset], gx5s[idx % nset]
         if side_done[idx % nset] is not None:
             main.wait_event(side_done[idx % nset])
-        if r % 3 == 2:
+        in_ada = ada is not None and r < ada.n_rdb
+        if in_ada:
+            g_y, a5, b1 = ada.enter(r, g_y, grads)
+        elif r % 3 == 2:
             a5, b1 = 0.04, 0.2
             g_rrdb = g_y
         else:
@@ -1224,13 +1378,98 @@ def rrdb_backward_bf16(ctx, params, dout, cache=None, flat=None):
                 side_done[idx % nset].record(side)
         else:
             reductions()
-        g_y = g_new
+        g_y = ada.leave(r, g_new, grads) if in_ada else g_new
     if overlap:
         main.wait_stream(side)
     g_fea = _empty((N, H, W, nf), dev, bf)
     ops.axpby(g_y, 1.0, g_lr, 1.0, g_fea)
     wgrad(xin, g_fea, L.i_fea, cin_real=in_nc)
     return None, grads, flat
+
+
+def adaptive_rrdb_forward_bf16_train(x, amap, params, nb, nb_ada, concat, upscale=4, cache=None):
+    """Forward of the mixed-precision training mode of the adaptive generators: the launches of adaptive_rrdb_forward_bf16
+    with the dense blocks on schedule SCHED1, every dense block in its own buffer, and what the inference forward overwrites
+    kept for the backward.  concat: the input t_{k-1} of each use of A stays in its own buffer (the previous dense block
+    writes it there, the first one is fea) and A's output y_k goes to the dense block's x slot; the outputs of A.0, R.0 and
+    R.2 are kept.  plain: RDB3's conv5 writes the pre-map t3 (kept), and out = a * t3 + 0.1 R(u) is one map_axpby launch
+    instead of RDB3's MAP_SCALE epilogue, which never materialises t3.  Returns (out, ctx)."""
+    a = _check_map(x, amap, nb, nb_ada)
+    L = RRDBLayout(nb + nb_ada, params[0].shape[0], upscale)
+    nf = L.nf
+    if nf != 64:
+        raise ops._lib.DasrError('adaptive RRDB generator: the wgmma path needs nf = 64 (got %d)' % nf)
+    cache = cache if cache is not None else _PackCache()
+    N, in_nc, H, W = x.shape
+    bf = torch.bfloat16
+    wk, bk = _tc_packers(params, cache, '', bf)
+    ext = _ada_ext(L, concat)
+    new = lambda c=nf: _empty((N, H, W, c), x, bf)
+
+    def conv64(src, i, dst):
+        ops.conv_tc(src, wk(i), bk(i), dst, nt=_pick_nt(nf, nf), act=ACT_LRELU, slope=0.2, pair=True)
+
+    def conv_map(src, i, dst, s):
+        w = params[2 * i]
+        wm = cache.get(('wm', i), w, lambda: ops.pack_filter_tc(w.detach()[:, :nf].float().contiguous(), TC_FPROP, bf))
+        taps = cache.get(('wmt', i), w, lambda: ops.map_channel_taps(w, nf))
+        ops.conv_tc(src, wm, bk(i), dst, act=ACT_LRELU, slope=0.2, amap=a, map_mode=ops.MAP_CHANNEL, map_scale=s, map_w=taps)
+
+    xin = torch.zeros((N, H, W, 32), dtype=bf, device=x.device)
+    ops.nchw_to_nhwc(x.contiguous().float(), View(xin, in_nc, 0))
+    fea = new()
+    ops.conv_tc(xin, wk(L.i_fea, cin_to=32), bk(L.i_fea), fea)
+    n_rdb, n_ada = L.n_rdb, 3 * nb_ada
+    bufs = [new(nf + 4 * GC + nf) for _ in range(n_rdb)] + [new()]
+    sv = dict(a=a, concat=concat, nb_ada=nb_ada, tin=[None] * n_rdb, tA=[None] * n_rdb, tmpR=[], res=[], t3=[])
+    if concat:
+        sv['tin'][:n_ada] = [fea] + [new() for _ in range(1, n_ada)]
+    else:
+        ops.axpby(fea, 1.0, None, 0.0, View(bufs[0], nf, 0))
+    for r in range(n_rdb):
+        b, blk = bufs[r], r // 3
+        u = View(b, nf, 0)
+        dst = sv['tin'][r + 1] if concat and r + 1 < n_ada else View(bufs[r + 1], nf, 0)
+        tail = _rrdb_tail(bufs, r, nf)
+        if blk < nb_ada:
+            if r % 3 == 0:
+                tmp, res = new(), new()
+                sv['tmpR'].append(tmp)
+                sv['res'].append(res)
+            if concat:
+                t = sv['tin'][r]
+                if r % 3 == 0:
+                    conv_map(t, ext(blk, 2), tmp, 1.0)
+                    conv64(tmp, ext(blk, 3), res)
+                tA = sv['tA'][r] = new()
+                conv_map(t, ext(blk, 0), tA, 0.2)
+                conv64(tA, ext(blk, 1), u)
+                if r % 3 == 2:
+                    tail = dict(alpha=0.04, res1=u, beta1=0.2, res2=res, beta2=1.0)
+            else:
+                if r % 3 == 0:
+                    conv64(u, ext(blk, 0), tmp)
+                    conv64(tmp, ext(blk, 1), res)
+                if r % 3 == 2:
+                    t3 = new()
+                    sv['t3'].append(t3)
+                    _rdb_bf16(b, t3, r, dict(alpha=0.2, res1=u, beta1=1.0), params, L, cache, False, wk, bk, SCHED1)
+                    ops.map_axpby(t3, a, 1.0, res, 0.1, dst)
+                    continue
+        _rdb_bf16(b, dst, r, tail, params, L, cache, False, wk, bk, SCHED1)
+    out, ups, h0 = _trunk_tail_bf16(bufs, fea, L, params, cache, wk, bk, '', bf, pair=False, save=True)
+    return out, dict(L=L, xin=xin, fea=fea, bufs=bufs, ups=ups, h0=h0, shape=(N, in_nc, H, W), ada=sv)
+
+
+def adaptive_rrdb_backward_bf16(ctx, params, dout, cache=None, need_map=True):
+    """Backward of adaptive_rrdb_forward_bf16_train: rrdb_backward_bf16 (dense blocks, trunk, side-stream filter and bias
+    reductions of the dense blocks) with the adaptive blocks' map convs (_AdaptiveBackward) on the main stream.  Returns
+    (map gradient [N, 1, H, W] fp32 or None, fp32 gradients in parameters() order, the flat tensor they are views of).  No
+    input-image gradient."""
+    cache = cache if cache is not None else _PackCache()
+    ada = _AdaptiveBackward(ctx, params, need_map, True, cache)
+    _, grads, flat = rrdb_backward_bf16(ctx, params, dout, cache, ada=ada)
+    return ada.gmap, grads, flat
 
 
 class _TrainGraphs:
@@ -1460,6 +1699,50 @@ class RRDBNetFunction(torch.autograd.Function):
         dx, grads = rrdb_backward_f32(ctx.saved, [p.detach() for p in ctx.params], dout, ctx.need_dx)
         ctx.saved = None
         return (dx, None, None) + tuple(grads)
+
+
+def _map_grad(gmap, amap):
+    return None if gmap is None else gmap.view(amap.shape).to(amap.dtype)
+
+
+class AdaptiveRRDBFunction(torch.autograd.Function):
+    """fp32 training node of the adaptive generators: (x, amap, nb, nb_ada, concat, upscale, *params in _engine_params()
+    order) -> out; gradients of x (when it requires grad), of the map (when it requires grad) and of every parameter."""
+
+    @staticmethod
+    def forward(ctx, x, amap, nb, nb_ada, concat, upscale, *params):
+        out, ctx.saved = adaptive_rrdb_forward_f32(x, amap, [p.detach() for p in params], nb, nb_ada, concat, upscale, save=True)
+        ctx.params, ctx.amap = params, amap
+        ctx.need_dx, ctx.need_map = x.requires_grad, amap.requires_grad
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        dx, gmap, grads = adaptive_rrdb_backward_f32(ctx.saved, [p.detach() for p in ctx.params], dout, ctx.need_dx,
+                                                     ctx.need_map)
+        ctx.saved = None
+        return (dx, _map_grad(gmap, ctx.amap), None, None, None, None) + tuple(grads)
+
+
+class AdaptiveRRDBFunctionBF16(torch.autograd.Function):
+    """Mixed-precision training node of the adaptive generators (wgmma fprop + dgrad + wgrad, fp32 filter and map
+    gradients), eager.  Same inputs as AdaptiveRRDBFunction after `cache` (a _PackCache); no input-image gradient."""
+
+    @staticmethod
+    def forward(ctx, x, amap, nb, nb_ada, concat, upscale, cache, *params):
+        if x.requires_grad:
+            raise ops._lib.DasrError('bf16 training mode does not return the input-image gradient; use precision fp32')
+        out, ctx.saved = adaptive_rrdb_forward_bf16_train(x, amap, [p.detach() for p in params], nb, nb_ada, concat, upscale,
+                                                          cache)
+        ctx.params, ctx.amap, ctx.cache, ctx.need_map = params, amap, cache, amap.requires_grad
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        gmap, grads, _ = adaptive_rrdb_backward_bf16(ctx.saved, [p.detach() for p in ctx.params], dout, ctx.cache, ctx.need_map)
+        ctx.saved = None
+        return (None, _map_grad(gmap, ctx.amap), None, None, None, None, None) + tuple(
+            gr.to(p.dtype) for gr, p in zip(grads, ctx.params))
 
 
 # ==================================================================================================

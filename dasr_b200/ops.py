@@ -561,16 +561,78 @@ def axpby(x, a, y, b, dst):
 
 
 def map_axpby(x, amap, a, y, b, dst):
-    """dst = amap * (a * x) + b * y on fp32 NHWC channel slices (x None: dst = a * amap); amap: fp32, one value per pixel."""
+    """dst = amap * (a * x) + b * y on fp32 or bf16 NHWC channel slices (x None: dst = a * amap); amap: fp32, one value per
+    pixel.  bf16: fp32 arithmetic, one rounding of the result (dasr_map_axpby_bf16)."""
     dst = as_view(dst)
     x = as_view(x) if x is not None else None
     y = as_view(y) if y is not None else None
-    npix = dst.t.numel() // dst.cs
+    npix = _check_slices('map_axpby', dst, tuple((n, v) for n, v in (('x', x), ('y', y)) if v is not None), _F32_BF16)
     if amap.numel() != npix or amap.dtype != torch.float32:
         raise _lib.DasrError('map_axpby: the map must hold one fp32 value per pixel')
-    check(_lib.load().dasr_map_axpby(x.ptr if x else None, _p(amap), y.ptr if y else None, dst.ptr, npix, dst.c,
-                                     x.cs if x else 0, x.coff if x else 0, y.cs if y else 0, y.coff if y else 0,
-                                     dst.cs, dst.coff, a, b, _stream()), 'map_axpby')
+    fn = _lib.load().dasr_map_axpby_bf16 if dst.t.dtype == torch.bfloat16 else _lib.load().dasr_map_axpby
+    check(fn(x.ptr if x else None, _p(amap), y.ptr if y else None, dst.ptr, npix, dst.c, x.cs if x else 0, x.coff if x else 0,
+             y.cs if y else 0, y.coff if y else 0, dst.cs, dst.coff, a, b, _stream()), 'map_axpby')
+
+
+def _check_map_grad(what, ga, npix):
+    if ga is not None and (ga.dtype != torch.float32 or ga.numel() != npix or not ga.is_contiguous()):
+        raise _lib.DasrError('%s: the map gradient must be a contiguous fp32 tensor of %d values (one per pixel)' % (what, npix))
+
+
+def map_channel_dgrad(g, w_map, s, ga, accumulate=False):
+    """Gradient of the map input channel (s * map) of a MAP_CHANNEL conv (dasr_map_channel_dgrad_bf16): g = View of the bf16
+    NHWC output gradient, w_map = the conv's [9][g.c] fp32 map taps (map_channel_taps); ga (fp32, one value per pixel)
+    (+)= s * sum over taps and channels of w_map * g at the pixels the tap reaches."""
+    g = as_view(g)
+    N, H, W, _ = g.t.shape
+    if g.t.dtype != torch.bfloat16 or g.t.dim() != 4:
+        raise _lib.DasrError('map_channel_dgrad: g must be a bf16 NHWC tensor (got %s %s)' % (g.t.dtype, tuple(g.t.shape)))
+    if w_map.dtype != torch.float32 or tuple(w_map.shape) != (9, g.c) or not w_map.is_contiguous():
+        raise _lib.DasrError('map_channel_dgrad: w_map must be contiguous fp32 [9, %d] (got %s %s)' % (g.c, w_map.dtype, tuple(w_map.shape)))
+    _check_map_grad('map_channel_dgrad', ga, N * H * W)
+    check(_lib.load().dasr_map_channel_dgrad_bf16(g.ptr, g.cs, g.coff, _p(w_map), _p(ga), N, H, W, g.c, float(s), int(accumulate),
+                                                  _stream()), 'map_channel_dgrad')
+
+
+def map_channel_wgrad(g, amap, s, dw, ch, accumulate=False):
+    """Filter gradient of the map input channel of a MAP_CHANNEL conv (dasr_map_channel_wgrad_bf16): dw[co][ch][dy][dx] (+)=
+    s * sum over pixels p of g[p, co] * amap[p + (dy - 1, dx - 1)]; g = View of the bf16 NHWC output gradient, amap fp32 one
+    value per pixel, dw fp32 contiguous OIHW [g.c][cin][3][3] (only input channel ch is written)."""
+    g = as_view(g)
+    N, H, W, _ = g.t.shape
+    if g.t.dtype != torch.bfloat16 or g.t.dim() != 4:
+        raise _lib.DasrError('map_channel_wgrad: g must be a bf16 NHWC tensor (got %s %s)' % (g.t.dtype, tuple(g.t.shape)))
+    if amap.dtype != torch.float32 or amap.numel() != N * H * W or not amap.is_contiguous():
+        raise _lib.DasrError('map_channel_wgrad: the map must be contiguous fp32 with one value per pixel')
+    if dw.dtype != torch.float32 or not dw.is_contiguous() or dw.dim() != 4 or tuple(dw.shape[2:]) != (3, 3) \
+            or dw.shape[0] != g.c or not 0 <= ch < dw.shape[1]:
+        raise _lib.DasrError('map_channel_wgrad: dw must be contiguous fp32 [%d, cin > %d, 3, 3] (got %s %s)' % (
+            g.c, ch, dw.dtype, tuple(dw.shape)))
+    lib = _lib.load()
+    ws = _workspace(lib.dasr_map_channel_wgrad_workspace(N, H, W, g.c), g.t.device)
+    check(lib.dasr_map_channel_wgrad_bf16(g.ptr, g.cs, g.coff, _p(amap), _p(dw), dw.shape[1], ch, N, H, W, g.c, float(s),
+                                          int(accumulate), _p(ws), ws.numel(), _stream()), 'map_channel_wgrad', 2)
+
+
+def map_scale_bwd(g, t, amap, gt, ga, accumulate=False):
+    """Backward of out = amap * t + ... (MAP_SCALE) on fp32 or bf16 NHWC channel slices (dasr_map_scale_bwd): gt = amap * g
+    (gt None: not written) and ga (fp32, one value per pixel; None: not written) (+)= sum over the channels of g * t."""
+    g = as_view(g)
+    others = tuple((n, as_view(v)) for n, v in (('t', t), ('gt', gt)) if v is not None)
+    npix = _check_slices('map_scale_bwd', g, others, _F32_BF16)
+    if amap.dtype != torch.float32 or amap.numel() != npix or not amap.is_contiguous():
+        raise _lib.DasrError('map_scale_bwd: the map must be contiguous fp32 with one value per pixel')
+    if gt is None and ga is None:
+        raise _lib.DasrError('map_scale_bwd: nothing to compute (gt and ga are None)')
+    if ga is not None and t is None:
+        raise _lib.DasrError('map_scale_bwd: the map gradient needs t')
+    _check_map_grad('map_scale_bwd', ga, npix)
+    t = as_view(t) if t is not None else None
+    gt = as_view(gt) if gt is not None else None
+    check(_lib.load().dasr_map_scale_bwd(g.ptr, g.cs, g.coff, t.ptr if t else None, t.cs if t else 0, t.coff if t else 0,
+                                         _p(amap), gt.ptr if gt else None, gt.cs if gt else 0, gt.coff if gt else 0, _p(ga),
+                                         npix, g.c, int(g.t.dtype == torch.bfloat16), int(accumulate), _stream()),
+          'map_scale_bwd')
 
 
 def _check_pool(what, x, k, s, dtypes, pooled=(), full=()):

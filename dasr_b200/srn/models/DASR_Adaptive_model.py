@@ -6,7 +6,8 @@ reference, net_patchD is never switched to eval(): its BatchNorm layers normalis
 and update their running statistics on every test() call.
 
 Training is not built: the shipped train config has no `FS` block, so the reference cannot construct it either
-(DASR_Adaptive_model.py:61), and the backward through the weight-map epilogue does not exist.
+(DASR_Adaptive_model.py:61).  The generators themselves train (architecture._AdaptiveRRDBNet with gradients enabled); the
+model's training step is what is missing.
 """
 import logging
 from collections import OrderedDict
@@ -27,7 +28,8 @@ class DASR_Adaptive_Model(BaseModel):
         if self.is_train:
             raise NotImplementedError(
                 'DASR_Adaptive_Model training is not built: the shipped train_DASR_Adaptive.json has no `FS` block (the '
-                'reference fails on opt["FS"]["fs"] as well), and the backward of the adaptive generators is not built')
+                'reference fails on opt["FS"]["fs"] as well), and its training step is not built (the adaptive generators '
+                'themselves train)')
         self.chop = opt['chop']
         self.scale = opt['scale']
         self.val_lpips = opt['val_lpips']

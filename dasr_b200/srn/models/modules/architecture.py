@@ -160,7 +160,9 @@ class _GraphedForwardMap(_GraphedForward):
 class _AdaptiveRRDBNet(nn.Module):
     """RRDBNet_Residual_conv / RRDBNet_Residual_conv_concat (architecture.py:208-297): fea_conv -> nb_ada adaptive blocks
     (weighted by the per-pixel map of the patch discriminator) -> nb RRDBs -> LR_conv + fea -> upconvs -> HR convs.
-    Same constructor, state_dict keys and forward(x, adaptive_weights) as the reference; inference only."""
+    Same constructor, state_dict keys and forward(x, adaptive_weights) as the reference.  Forwards that need gradients (of
+    the parameters, the map or x) train on CUDA tensors, eagerly, in train_precision: None -> DASR_B200_TRAIN_PRECISION or
+    'fp32' ('fp32' | 'bf16', as RRDBNet; bf16 returns no input-image gradient)."""
     concat = None
 
     def __init__(self, in_nc, out_nc, nf, nb, gc=32, upscale=4, norm_type=None, act_type='leakyrelu', mode='CNA',
@@ -192,6 +194,7 @@ class _AdaptiveRRDBNet(nn.Module):
         self.up_conv = B.sequential(*upsampler, HR_conv0, HR_conv1)
         self.nb, self.nb_ada, self.nf, self.upscale = nb, nb_ada, nf, upscale
         self.precision = None          # None -> DASR_B200_PRECISION or 'bf16' ('bf16' | 'fp16' | 'fp32')
+        self.train_precision = None    # training:  None -> DASR_B200_TRAIN_PRECISION or 'fp32' ('fp32' | 'bf16')
         self._pack_cache = engine._PackCache()
         self._graphs = {}
         self._graph_seen = None
@@ -216,7 +219,14 @@ class _AdaptiveRRDBNet(nn.Module):
     def forward(self, x, adaptive_weights):
         params = self._engine_params()
         if torch.is_grad_enabled() and (x.requires_grad or adaptive_weights.requires_grad or any(p.requires_grad for p in params)):
-            raise NotImplementedError('training of the adaptive generators is not built (run the forward under torch.no_grad())')
+            if not (x.is_cuda and adaptive_weights.is_cuda):
+                raise NotImplementedError('training of the adaptive generators is not built for CPU tensors (the dasr_b200 '
+                                          'path runs on CUDA only)')
+            args = (x, adaptive_weights, self.nb, self.nb_ada, self.concat, self.upscale)
+            tp = self.train_precision or os.environ.get('DASR_B200_TRAIN_PRECISION', 'fp32')
+            if tp == 'bf16':      # mixed precision: wgmma fprop / dgrad / wgrad, fp32 filter and map gradients
+                return engine.AdaptiveRRDBFunctionBF16.apply(*args, self._pack_cache, *params)
+            return engine.AdaptiveRRDBFunction.apply(*args, *params)
         prec = self.precision or _precision('bf16')
         if prec == 'fp32':
             return engine.adaptive_rrdb_forward_f32(x, adaptive_weights, params, self.nb, self.nb_ada, self.concat, self.upscale)
