@@ -24,7 +24,10 @@
 // keeps only its half of the filters resident, and the leader's TMA multicasts every A halo tile into both CTAs, so an
 // activation tile crosses L2 -> SMEM once for the pair.  That is what lets a 192-wide filter set (221 KB) run as one tile.
 // A dasr_conv_tc2 launch whose whole filter set fits one SM and whose grid has many tiles per SM runs one CTA per tile
-// instead (tc2_single).
+// instead (tc2_single).  A pair launch with a 32-channel Cout tile per CTA and an even number of 64-channel A loads splits
+// the pair by input channels instead (tc2_ksplit, KSPLIT): each CTA keeps the filters of its half of the input channels for
+// all 64 output channels, loads its own half of every A tile, runs m64n64k16 over it, and sends the partial sums of the 32
+// channels it does not finish to its peer's shared memory (st.async); each CTA then finishes its 32 channels.
 #include <type_traits>
 #include "tc_common.cuh"
 
@@ -65,7 +68,8 @@ struct TcKernelArgs {
   int epi_bytes;     // bytes of ONE staged epilogue tile: 128 pixels x nt channels bf16
   int has_pre, has_res1, has_res2;
   int nbuf;          // staged-epilogue tile frames (1..4): pre / residual blocks are requested nbuf tiles ahead
-  int pair;          // 1: launched as (1, 2, 1) clusters, A tiles multicast by the leader (rank 0)
+  int pair;          // 1: launched as (1, 2, 1) clusters, A tiles multicast by the leader (rank 0) unless KSPLIT
+  int xch_bytes;     // KSPLIT: the two exchange buffers and their barriers (XCH_BAR_BYTES)
   const float* map;  // weight map [N][H][W] fp32 (image stride p.map_stride), MAP != 0 only
   const float* map_w;// MAP 1: the map channel's filter taps [9][cout] fp32
 };
@@ -98,6 +102,17 @@ __device__ __forceinline__ void stsm4(uint32_t addr, const uint32_t* r) {
                "r"(r[3]));
 }
 __device__ __forceinline__ void compiler_fence() { asm volatile("" ::: "memory"); }
+// shared-memory address `addr` of this CTA -> the same offset in cluster CTA `rank`
+__device__ __forceinline__ uint32_t mapa_u32(uint32_t addr, uint32_t rank) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
+  return r;
+}
+// 16 bytes into another CTA's shared memory (cluster address), counted as transaction bytes on that CTA's barrier `bar`
+__device__ __forceinline__ void st_async_v4(uint32_t addr, float x, float y, float z, float w, uint32_t bar) {
+  asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.v4.f32 [%0], {%1, %2, %3, %4}, [%5];"
+               ::"r"(addr), "f"(x), "f"(y), "f"(z), "f"(w), "r"(bar) : "memory");
+}
 
 // Staged tile layout: nb64 blocks of 64 channels (128 B rows, SWIZZLE_128B), then a 32-channel block (64 B rows,
 // SWIZZLE_64B) if nt & 32, then a 16-channel block (32 B rows, SWIZZLE_32B) if nt & 16.  Byte offset of (pixel m, channel c).
@@ -276,12 +291,15 @@ enum { TEV_P_EMPTY = 10, TEV_P_ISSUED = 11, TEV_E_SFULL = 12, TEV_E_STORED = 13,
 // parity b = 2i + j store through parity b's strided output map, into channels [out_coff, out_coff + cout / 4) of the
 // 2H x 2W tensor.  Only the bias index (the bias stays in the conv's channel order) and the epilogue TMA warp's choice of
 // map and column differ from a plain conv.
-template <int EPI_MODE, bool HAS_PRE, int NRES, int MAP = 0, int NT = 0, int NTAPS = 9, bool PS = false>
+// KSPLIT (pair, ping-pong, 64-channel loads issued half-major): the pair splits the input channels, not the Cout tile.
+// NT is still the Cout tile a CTA finishes; its MMAs are 2 NT wide (the pair's whole Cout tile) over half of the input
+// channels, and the other NT channels' partial sums go to the peer, which adds them to its own: S(K half 0) + S(K half 1).
+template <int EPI_MODE, bool HAS_PRE, int NRES, int MAP = 0, int NT = 0, int NTAPS = 9, bool PS = false, bool KSPLIT = false>
 __global__ void __launch_bounds__(TCK_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ CUtensorMap tmap_w,
                const __grid_constant__ EpiMaps em, const TcKernelArgs a) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // carve: [W resident][A stages][staged tiles: out/pre][res1][res2][barriers, tap offsets, bias]
+  // carve: [W resident][A stages][staged tiles: out/pre][res1][res2][K-split exchange][barriers, tap offsets, bias]
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sW = smem;
   uint8_t* sA = smem + a.w_bytes;
@@ -289,7 +307,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
   uint8_t* sS = sA + (size_t)a.stages * a.a_stage_bytes;          // [nbuf] output staging (and pre-activation addend, in place)
   uint8_t* sR1 = sS + nbuf * a.epi_bytes;                         // [nbuf]
   uint8_t* sR2 = sR1 + (NRES >= 1 ? nbuf * a.epi_bytes : 0);     // [nbuf]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sR2 + (NRES >= 2 ? nbuf * a.epi_bytes : 0));
+  // K-split: [2] fp32 partial sums from the peer, one buffer per consumer warpgroup, fragment-ordered (16 B of thread t of
+  // the warpgroup at 16 (128 q + t)); then per warpgroup a barrier "the peer's sums landed" and one "the peer has read mine"
+  uint8_t* sX = sR2 + (NRES >= 2 ? nbuf * a.epi_bytes : 0);
+  constexpr int XCH_BYTES = 128 * NT * 4;
+  uint64_t* xfull_bar = reinterpret_cast<uint64_t*>(sX + 2 * XCH_BYTES);   // [2]
+  uint64_t* xfree_bar = xfull_bar + 2;                                    // [2]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sX + a.xch_bytes);
   uint64_t* full_bar = bars;                     // [stages]  A chunk landed
   uint64_t* empty_bar = bars + MAX_STAGES;       // [stages]  A chunk consumed (leader of a pair: by both CTAs)
   uint64_t* w_bar = bars + 2 * MAX_STAGES;       // [1]       resident filters landed
@@ -314,20 +338,28 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
   const uint32_t rank = pair ? cluster_ctarank() : 0u;
   const uint32_t a_row = a.chunk64 ? 2u * ROW_B : (uint32_t)ROW_B;    // bytes per pixel row of an A tile
   static_assert(NT == 0 || (EPI_MODE == 0 && MAP == 0 && NT % 16 == 0 && NT <= 96), "ping-pong: staged epilogue, N <= 96");
+  static_assert(!KSPLIT || (NT == 32 && NTAPS == 9 && !PS), "K-split: 32 channels finished per CTA, plain 3x3 taps");
   constexpr int TILE_WARPS = NT ? 4 : CONS_WARPS;      // consumer warps that read one A stage / write one staged tile
+  const bool mc = pair && !KSPLIT;                     // A tiles multicast by the leader, stages released by both CTAs
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_in);
     tma_prefetch_desc(&tmap_w);
     for (int s = 0; s < a.stages; s++) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], TILE_WARPS * ((pair && rank == 0) ? 2 : 1));   // one arrive per consumer warp (of both CTAs)
+      mbar_init(&empty_bar[s], TILE_WARPS * ((mc && rank == 0) ? 2 : 1));   // one arrive per consumer warp (of both CTAs)
     }
     mbar_init(w_bar, 1);
     for (int b = 0; b < EPI_BARS; b++) {
       mbar_init(&pre_bar[b], 1);
       mbar_init(&sfull_bar[b], TILE_WARPS);
       mbar_init(&sfree_bar[b], 1);
+    }
+    if constexpr (KSPLIT) {
+      for (int g = 0; g < 2; g++) {
+        mbar_init(&xfull_bar[g], 1);             // this CTA's expect_tx + the peer's bytes
+        mbar_init(&xfree_bar[g], 4);             // one remote arrive per warp of the peer's warpgroup g
+      }
     }
     fence_barrier_init();
     for (int t = 0; t < 9; t++) {
@@ -359,12 +391,23 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
     if (lane == 0) {
       // resident filters: rows [(var*ntaps + tap)*nchunks + c]*cout + ntile*nt .. +nt of the packed filter
       mbar_expect_tx(w_bar, (uint32_t)a.w_bytes);
-      for (int tap = 0; tap < ntaps; tap++)
-        for (int c = 0; c < a.nchunks; c++) {
-          int slot = tap * a.nchunks + c;
-          int row = ((var * ntaps + tap) * a.nchunks + c) * p.cout + ntile * nt;
-          tma_load_2d(sW + (size_t)slot * nt * ROW_B, &tmap_w, w_bar, 0, row);
-        }
+      if constexpr (KSPLIT) {
+        // chunks [rank, rank + 1) * nchunks / 2, the pair's 2 nt rows (both CTAs' Cout tiles): [tap][chunk][2 nt rows x 64 B]
+        const int nck = a.nchunks / 2;
+        for (int tap = 0; tap < ntaps; tap++)
+          for (int c = 0; c < nck; c++)
+            for (int h = 0; h < 2; h++) {
+              const int row = (tap * a.nchunks + (int)rank * nck + c) * p.cout + (ntile - (int)rank + h) * nt;
+              tma_load_2d(sW + (size_t)((tap * nck + c) * 2 + h) * nt * ROW_B, &tmap_w, w_bar, 0, row);
+            }
+      } else {
+        for (int tap = 0; tap < ntaps; tap++)
+          for (int c = 0; c < a.nchunks; c++) {
+            int slot = tap * a.nchunks + c;
+            int row = ((var * ntaps + tap) * a.nchunks + c) * p.cout + ntile * nt;
+            tma_load_2d(sW + (size_t)slot * nt * ROW_B, &tmap_w, w_bar, 0, row);
+          }
+      }
       pdl_wait();                        // activations come from the previous launch (filters / bias above do not)
       int stage = 0;
       uint32_t phase = 0;
@@ -378,10 +421,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
           if (c == 0) TC_STAMP(it, TEV_P_EMPTY);
           uint8_t* dst = sA + (size_t)stage * a.a_stage_bytes;
           if (p.a_mode == 0) {
-            // 64 channels per load when the slice or the chunk list allows it: half the TMA requests per byte
-            const int ch = p.nchunk_list ? p.chunk_off[a.chunk64 ? 2 * c : c] : p.in_coff + c * (a.chunk64 ? 2 : 1) * CHUNK;
+            // 64 channels per load when the slice or the chunk list allows it: half the TMA requests per byte.  K-split:
+            // nloads of the tile's 2 nloads loads, this CTA's half of the input channels
+            const int lc = KSPLIT ? (int)rank * a.nloads + c : c;
+            const int ch = p.nchunk_list ? p.chunk_off[a.chunk64 ? 2 * lc : lc] : p.in_coff + lc * (a.chunk64 ? 2 : 1) * CHUNK;
             mbar_expect_tx(&full_bar[stage], (uint32_t)((a.chunk64 ? 2 : 1) * A_HALO_BYTES));
-            if (!pair) tma_load_4d(dst, &tmap_in, &full_bar[stage], ch, x0 - 1, y0 - 1, n);
+            if (!mc) tma_load_4d(dst, &tmap_in, &full_bar[stage], ch, x0 - 1, y0 - 1, n);
             else if (rank == 0) tma_load_4d_mc(dst, &tmap_in, &full_bar[stage], ch, x0 - 1, y0 - 1, n, (uint16_t)3);
           } else {
             mbar_expect_tx(&full_bar[stage], (uint32_t)(ntaps * A_TAP_BYTES));
@@ -516,7 +561,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
     const uint64_t b_hi = desc_hi(16, 8 * ROW_B, DESC_SW64);
     const int ksteps = a.chunk64 ? 4 : 2;                                      // K = 16 steps per A load
     const uint32_t sA_u = smem_u32(sA), sW_u = smem_u32(sW);
-    const uint32_t b_slot = (uint32_t)(nt * ROW_B);
+    const uint32_t b_slot = (uint32_t)((KSPLIT ? 2 : 1) * nt * ROW_B);     // one resident filter chunk: MMA width x 64 B
     // first A row of this warpgroup's 64 pixels: 8 image rows down the halo tile, or 64 rows of a per-tap tile
     const uint32_t wg_off = (EPI_MODE == 3) ? 64u * wg * a_row : (p.a_mode == 0 ? 8u * wg * HALO_W * a_row : 64u * wg * (uint32_t)ROW_B);
     const int co_base = ntile * nt;
@@ -535,7 +580,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
       __syncwarp();
       if (lane == 0) {
         mbar_arrive(&empty_bar[s]);
-        if (pair && rank == 1) mbar_arrive_cluster(&empty_bar[s], 0);
+        if (mc && rank == 1) mbar_arrive_cluster(&empty_bar[s], 0);
       }
     };
     mbar_wait(w_bar, 0);
@@ -632,13 +677,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
       const uint32_t G = gridDim.x, ntiles = (uint32_t)a.ntiles;   // 32-bit tile arithmetic (checked on the host)
       const uint32_t nl = (uint32_t)a.nloads, ns = (uint32_t)a.stages;
       const uint32_t blk_off = 8u * HALO_W * a_row;
-      const uint32_t b_tap = (uint32_t)a.nchunks * b_slot;
+      const uint32_t b_tap = (uint32_t)(KSPLIT ? a.nchunks / 2 : a.nchunks) * b_slot;
+      constexpr int NM = KSPLIT ? 2 * NT : NT;                     // MMA width
       // KS (K = 16 steps per A load: 4 with 64-channel loads) and the operand type are launch constants: one copy of the
       // loop per combination, so no branch sits between the wgmmas that share the accumulators
       auto run = [&](auto ks_c, auto f16_c, auto halves_c) {
         constexpr int KS = decltype(ks_c)::value, F16 = decltype(f16_c)::value;
         constexpr bool HALVES = decltype(halves_c)::value;
-        float acc[NT];
+        float acc[NM];
         for (; blockIdx.x + it * G < ntiles; it += 2) {     // local tile it is tile blockIdx.x + it * G
           if (it > 0) asm volatile("bar.sync %0, 256;" ::"r"(2 + ((it - 1) & 1)) : "memory");
           const uint32_t g0 = it * nl;
@@ -649,7 +695,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
           for (int c = 0; c < a.nloads; c++) {
             mbar_wait(&full_bar[stage], phase);
             wgmma_fence();
-            issue_load_pp<NT, NTAPS, KS, F16, HALVES>(acc, sA_u + (uint32_t)stage * a.a_stage_bytes, blk_off, a_hi, sTap,
+            issue_load_pp<NM, NTAPS, KS, F16, HALVES>(acc, sA_u + (uint32_t)stage * a.a_stage_bytes, blk_off, a_hi, sTap,
                                                       sW_u + (uint32_t)(KS / 2) * (uint32_t)c * b_slot, b_tap, b_slot, b_hi, c == 0);
             wgmma_commit();
             if (prev >= 0) { wgmma_wait<1>(); release(prev); }
@@ -659,9 +705,42 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
           if (rec) TC_STAMP(it, 5 * wg + 1);
           if (blockIdx.x + (it + 1) * G < ntiles) asm volatile("bar.arrive %0, 256;" ::"r"(2 + (it & 1)) : "memory");   // tile it landed
           wgmma_wait<0>();
-          fence_regs<NT>(acc);
+          fence_regs<NM>(acc);
           release(prev);
           if (rec) TC_STAMP(it, 5 * wg + 2);
+          if constexpr (KSPLIT) {
+            // Both CTAs of the pair walk the same tiles with the same warpgroup, so thread t of warpgroup wg holds the same
+            // accumulator fragment in both: its NT partial sums of the peer's channels go to the same thread of the peer,
+            // and the NT of its own channels become S(own K half) + S(peer's K half) in acc[0, NT), the layout of an NT-wide
+            // accumulator.  k = this warpgroup's tile count: the peer's buffer is free once it has read tile k - 1.
+            const uint32_t k = it >> 1, peer = rank ^ 1u, t = threadIdx.x & 127;
+            const uint32_t xoff = smem_u32(sX) + (uint32_t)wg * XCH_BYTES + 16u * t;
+            auto exchange = [&](auto r_c) {
+              constexpr int R = decltype(r_c)::value, HS = NT / 2, NQ = NT / 4;   // acc[b NT + h HS + i]: m64 block b, Cout half h
+              if (k > 0) mbar_wait(&xfree_bar[wg], (k & 1) ^ 1);
+              const uint32_t dst = mapa_u32(xoff, peer), bar = mapa_u32(smem_u32(&xfull_bar[wg]), peer);
+#pragma unroll
+              for (int q = 0; q < NQ; q++) {
+                const float* v = acc + (q / (NQ / 2)) * NT + (1 - R) * HS + 4 * (q % (NQ / 2));
+                st_async_v4(dst + 2048u * q, v[0], v[1], v[2], v[3], bar);
+              }
+              if (wi == 0 && lane == 0) mbar_expect_tx(&xfull_bar[wg], (uint32_t)XCH_BYTES);
+              mbar_wait(&xfull_bar[wg], k & 1);
+#pragma unroll
+              for (int q = 0; q < NQ; q++) {
+                const int b = q / (NQ / 2), i = 4 * (q % (NQ / 2));
+                const float4 x = lds128f(xoff + 2048u * q);
+                float* o = acc + b * HS + i;
+                const float* s = acc + b * NT + R * HS + i;
+                o[0] = s[0] + x.x; o[1] = s[1] + x.y; o[2] = s[2] + x.z; o[3] = s[3] + x.w;
+              }
+              compiler_fence();
+              __syncwarp();
+              if (lane == 0) mbar_arrive_cluster(&xfree_bar[wg], peer);
+            };
+            if (rank == 0) exchange(std::integral_constant<int, 0>());
+            else exchange(std::integral_constant<int, 1>());
+          }
 
           const int sb = (int)(it % (uint32_t)nbuf);
           const uint32_t sphase = (it / (uint32_t)nbuf) & 1;
@@ -1066,6 +1145,45 @@ __global__ void __launch_bounds__(64, 1) tma_rate_kernel(const __grid_constant__
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// wgmma rate probe (selftest only): on every SM, two warpgroups issue the ping-pong consumers' MMA stream of a 64-channel
+// A load (issue_load_pp: 2 halves x 9 taps x 2 K steps, each on two m64 row blocks, m64nNk16 with both operands in shared
+// memory, the conv kernel's descriptors) `iters` times on a resident tile, one commit group in flight behind the issuing
+// one.  Reports SM cycles per m64nNk16 instruction, both warpgroups together.
+// ---------------------------------------------------------------------------------------------
+constexpr int WR_MMAS_PER_LOAD = 2 * 9 * 2 * 2;
+template <int N>
+__global__ void __launch_bounds__(256, 1) wgmma_rate_kernel(int iters, long long* out, float* sink) {
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  constexpr int A_BYTES = A_STAGE_ROWS * 2 * ROW_B, B_BYTES = 9 * 2 * N * ROW_B;
+  uint32_t* w = reinterpret_cast<uint32_t*>(smem);
+  for (int i = threadIdx.x; i < (A_BYTES + B_BYTES) / 4; i += blockDim.x)   // small finite bf16 pairs
+    w[i] = 0x3C003C00u | ((uint32_t)i * 2654435761u & 0x007F007Fu);
+  fence_proxy_async();
+  __syncthreads();
+  const uint32_t a_u = smem_u32(smem), b_u = a_u + A_BYTES;
+  uint32_t tap[9];
+#pragma unroll
+  for (int t = 0; t < 9; t++) tap[t] = (uint32_t)((t / 3) * HALO_W + t % 3) * 2u * ROW_B;
+  const uint64_t a_hi = desc_hi(16, HALO_W * 2 * ROW_B, DESC_SW128), b_hi = desc_hi(16, 8 * ROW_B, DESC_SW64);
+  const uint32_t b_slot = (uint32_t)(N * ROW_B), blk_off = 8u * HALO_W * 2 * ROW_B;
+  float acc[N];
+  const long long t0 = clock64();
+  for (int i = 0; i < iters; i++) {
+    wgmma_fence();
+    issue_load_pp<N, 9, 4, 0, true>(acc, a_u, blk_off, a_hi, tap, b_u, 2 * b_slot, b_slot, b_hi, i == 0);
+    wgmma_commit();
+    wgmma_wait<1>();
+  }
+  wgmma_wait<0>();
+  fence_regs<N>(acc);
+  __syncthreads();
+  const long long t1 = clock64();
+  if (threadIdx.x == 0 && blockIdx.x == 0) out[0] = t1 - t0;
+  if (acc[0] == 1234.5f) sink[threadIdx.x] = acc[N - 1];   // keeps the accumulators live
+}
+
 }  // namespace dasr
 
 using namespace dasr;
@@ -1195,13 +1313,13 @@ static const int TC_BAR_BYTES = (2 * MAX_STAGES + 8 + 3 * EPI_BARS) * 8 + 256 * 
 // Shared-memory plan: staged-epilogue buffers as many (<= 4) as still leave 4 A stages — loads of pre / residual tiles
 // are issued nbuf tiles ahead, which hides their latency — then as many A stages as fit (<= MAX_STAGES).  One buffer
 // (stores of a tile drain before the next tile's epilogue) only when two would leave fewer than 2 A stages.
-// Returns the number of A stages (< 2: does not fit).
-static int tc_plan(int w_bytes, int a_stage, int epi_bytes, int nres_loaded, int epi_mode, int* nbuf_out) {
+// xch_bytes: the K-split's exchange buffers (tc2_xch_bytes).  Returns the number of A stages (< 2: does not fit).
+static int tc_plan(int w_bytes, int a_stage, int epi_bytes, int nres_loaded, int epi_mode, int* nbuf_out, int xch_bytes = 0) {
   int nbuf = (epi_mode == 0) ? 4 : (epi_mode == 3 ? 1 : 2);
   int avail = 0;
   for (;; nbuf--) {
     const int epi_total = nbuf * epi_bytes * (1 + nres_loaded);
-    avail = SMEM_LIMIT - 1024 /*alignment slack*/ - w_bytes - epi_total - TC_BAR_BYTES;
+    avail = SMEM_LIMIT - 1024 /*alignment slack*/ - w_bytes - epi_total - xch_bytes - TC_BAR_BYTES;
     if (nbuf <= 1 || avail >= 4 * a_stage || (nbuf == 2 && avail >= 2 * a_stage)) break;
   }
   *nbuf_out = nbuf;
@@ -1221,12 +1339,17 @@ static bool chunk_list_pairs64(const DasrConvTcParams* p) {
   return true;
 }
 
+// K-split exchange buffers: 128 pixels x nt fp32 partial sums per consumer warpgroup, and four barriers
+constexpr int XCH_BAR_BYTES = 4 * 8;
+static int tc2_xch_bytes(int nt) { return 2 * 128 * nt * 4 + XCH_BAR_BYTES; }
+
 // pair = 1: (1, 2, 1) clusters, p->nt is the Cout tile of ONE CTA (half of the pair's tile).
 // order32: every output element sums its products in the order of 32-channel A loads (dasr_conv_tc2's launches, on the
 // pair or on one CTA), so a contiguous slice never takes the tap-major 64-channel loads.
+// ksplit (pair, tc2_ksplit): the pair splits the input channels; each CTA finishes the Cout tile p->nt.
 static int conv_tc_launch(const void* in, const void* w, const float* bias, const void* pre, const void* res1, const void* res2,
                           const void* mask_src, void* out, const DasrConvTcParams* p, void* stream, int pair, bool order32,
-                          const float* map = nullptr, const float* map_w = nullptr) {
+                          const float* map = nullptr, const float* map_w = nullptr, bool ksplit = false) {
   PFN_encodeTiled enc = get_encode();
   if (!enc) {
     set_error("conv_tc: cuTensorMapEncodeTiled not available");
@@ -1318,12 +1441,21 @@ static int conv_tc_launch(const void* in, const void* w, const float* bias, cons
       nbuf = nbuf64;
     }
   }
-  a.nloads = a.chunk64 ? a.nchunks / 2 : a.nchunks;
+  // K-split: the same resident filter bytes (half the chunks, twice the rows), 64-channel loads issued half-major, half of
+  // a tile's loads per CTA, and the exchange buffers (tc2_ksplit has checked that this plan fits)
+  a.xch_bytes = 0;
+  if (ksplit) {
+    a.chunk64 = 2;
+    a.xch_bytes = tc2_xch_bytes(p->nt);
+    stages = tc_plan(a.w_bytes, (int)a_stage_bytes_for(p, 1), a.epi_bytes, a.has_res1 + a.has_res2, 0, &nbuf, a.xch_bytes);
+    DASR_REQUIRE(pp == 1 && psi < 0 && nbuf >= 2 && stages >= 2, "conv_tc2: K-split plan (nt=%d cin=%d)", p->nt, p->cin);
+  }
+  a.nloads = a.chunk64 ? a.nchunks / (ksplit ? 4 : 2) : a.nchunks;
   a.a_stage_bytes = (int)a_stage_bytes_for(p, a.chunk64);
   a.nbuf = nbuf;
   a.stages = stages;
   const int epi_total = nbuf * a.epi_bytes * (1 + a.has_res1 + a.has_res2);
-  const size_t smem = 1024 + (size_t)a.w_bytes + (size_t)stages * a.a_stage_bytes + epi_total + TC_BAR_BYTES;
+  const size_t smem = 1024 + (size_t)a.w_bytes + (size_t)stages * a.a_stage_bytes + epi_total + a.xch_bytes + TC_BAR_BYTES;
 
   CUtensorMap tm_in, tm_w;
   EpiMaps em;
@@ -1381,11 +1513,17 @@ static int conv_tc_launch(const void* in, const void* w, const float* bias, cons
     }
   }
 
-  const KernelFn fn = psi >= 0 ? ps_kernels[psi] : pp >= 0 ? pp_kernels[pp][ki] : kernels[ki];
+  // K-split instantiations: the ping-pong row of NT = 32 with the trailing KSPLIT argument
+  static const KernelFn ks_kernels[6] = {
+      conv_tc_kernel<0, false, 0, 0, 32, 9, false, true>, conv_tc_kernel<0, false, 1, 0, 32, 9, false, true>,
+      conv_tc_kernel<0, false, 2, 0, 32, 9, false, true>, conv_tc_kernel<0, true, 0, 0, 32, 9, false, true>,
+      conv_tc_kernel<0, true, 1, 0, 32, 9, false, true>,  conv_tc_kernel<0, true, 2, 0, 32, 9, false, true>};
+  const KernelFn fn = ksplit ? ks_kernels[ki] : psi >= 0 ? ps_kernels[psi] : pp >= 0 ? pp_kernels[pp][ki] : kernels[ki];
   static bool attr_set[12] = {false, false, false, false, false, false, false, false, false, false, false, false};
   static bool attr_set_pp[5][6] = {};
   static bool attr_set_ps[2] = {};
-  bool& attr = psi >= 0 ? attr_set_ps[psi] : pp >= 0 ? attr_set_pp[pp][ki] : attr_set[ki];
+  static bool attr_set_ks[6] = {};
+  bool& attr = ksplit ? attr_set_ks[ki] : psi >= 0 ? attr_set_ps[psi] : pp >= 0 ? attr_set_pp[pp][ki] : attr_set[ki];
   if (!attr) {
     cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
     if (e != cudaSuccess) {
@@ -1558,6 +1696,25 @@ static bool tc2_single(const DasrConvTcParams* p, int nres, const float* map) {
   return work >= (long)TC2_SINGLE_WAVES * num_sms();
 }
 
+// dasr_conv_tc2 on the pair split by input channels (KSPLIT) instead of by Cout: when the pair's Cout tile is 64 (32 per
+// CTA, whose m64n32k16 MMAs read 1.5 x the shared-memory operand bytes per product of m64n64k16), the launch carries no
+// dgrad mask and no weight map, the input is an even number of 64-channel loads (a contiguous slice of 128k channels, or a
+// chunk list of 64-channel runs whose length is a multiple of 4), and the filters of half the input channels for both CTAs'
+// Cout tiles, the exchange buffers, two staging frames and the 64-channel A stages of two tiles fit one SM.  Dense-block
+// launch 5 (128 -> 64) is the launch this is for.
+static bool tc2_ksplit(const DasrConvTcParams* p, int nres, const float* map) {
+#ifdef DASR_TC_TRACE
+  if (g_trace_coop) return false;
+#endif
+  if (p->nt != 64 || p->mask_c1 > p->mask_c0 || map) return false;
+  const int nchunks = p->cin / CHUNK;
+  if (p->nchunk_list ? !(chunk_list_pairs64(p) && p->nchunk_list % 4 == 0) : nchunks % 4 != 0) return false;
+  int nbuf;
+  const int stages = tc_plan(9 * nchunks * (p->nt / 2) * ROW_B, (int)a_stage_bytes_for(p, 1), (p->nt / 2) * 128 * 2, nres, 0,
+                             &nbuf, tc2_xch_bytes(p->nt / 2));
+  return nbuf >= 2 && stages >= 2 * (nchunks / 4);
+}
+
 int dasr_conv_tc2_supported(const DasrConvTcParams* p) {
   // plain 3x3 fprop/dgrad geometry, staged bf16 epilogue; pre / residual tensors are announced through their channel
   // strides (pre_cs, res1_cs, res2_cs > 0), as dasr_conv_tc2 callers fill them
@@ -1601,7 +1758,8 @@ static int conv_tc2_run(const void* in, const void* w, const float* bias, const 
   if (tc2_single(p, (res1 ? 1 : 0) + (res2 ? 1 : 0), map))   // grid (SMs / (cout / nt), cout / nt), no cluster
     return conv_tc_launch(in, w, bias, pre, res1, res2, nullptr, out, &q, stream, 0, true, map, map_w);
   q.nt = p->nt / 2;                     // per CTA; grid.y = cout / (nt / 2), consecutive CTAs form the clusters
-  return conv_tc_launch(in, w, bias, pre, res1, res2, nullptr, out, &q, stream, 1, true, map, map_w);
+  return conv_tc_launch(in, w, bias, pre, res1, res2, nullptr, out, &q, stream, 1, true, map, map_w,
+                        tc2_ksplit(p, (res1 ? 1 : 0) + (res2 ? 1 : 0), map));
 }
 
 int dasr_conv_tc2(const void* in, const void* w, const float* bias, const void* pre, const void* res1, const void* res2,
@@ -1659,6 +1817,27 @@ int dasr_probe_tma_rate(int row_elems, int rows_per_box, int cs, int store, doub
   cudaFree(buf);
   if (e != cudaSuccess) { set_error("probe tma: %s", cudaGetErrorString(e)); return DASR_E_LAUNCH; }
   *cycles_per_box = (double)h / iters;
+  return DASR_OK;
+}
+
+// selftest-only probe: SM cycles per m64nNk16 wgmma (N = 32, 64 or 96) of the ping-pong consumers' MMA stream, all SMs busy
+int dasr_probe_wgmma_rate(int n, double* cycles_per_mma) {
+  void (*fn)(int, long long*, float*) = n == 32 ? wgmma_rate_kernel<32> : n == 64 ? wgmma_rate_kernel<64> : n == 96 ? wgmma_rate_kernel<96> : nullptr;
+  if (!fn) { set_error("probe wgmma: N must be 32, 64 or 96"); return DASR_E_BADARG; }
+  const int smem = 1024 + A_STAGE_ROWS * 2 * ROW_B + 9 * 2 * n * ROW_B, iters = 2000;
+  long long* d;
+  float* sink;
+  if (cudaMalloc(&d, 8) != cudaSuccess || cudaMalloc(&sink, 256 * 4) != cudaSuccess) return DASR_E_LAUNCH;
+  cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  for (int rep = 0; rep < 2; rep++)            // the first launch loads the module
+    fn<<<num_sms(), 256, smem>>>(iters, d, sink);
+  long long h = 0;
+  cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) e = cudaMemcpy(&h, d, 8, cudaMemcpyDeviceToHost);
+  cudaFree(d);
+  cudaFree(sink);
+  if (e != cudaSuccess) { set_error("probe wgmma: %s", cudaGetErrorString(e)); return DASR_E_LAUNCH; }
+  *cycles_per_mma = (double)h / ((double)iters * 2 * WR_MMAS_PER_LOAD);
   return DASR_OK;
 }
 

@@ -1,5 +1,5 @@
 // Standalone GPU self-test / micro-benchmark of the C-ABI library (no Python, no torch).
-// Usage: selftest [check] [bench]      (default: both)  |  selftest fused | tmarate | prof  |  selftest_trace trace
+// Usage: selftest [check] [bench]      (default: both)  |  selftest fused | tmarate | wgmmarate | prof  |  selftest_trace trace
 // `check` compares every conv kernel with a CPU double-precision loop nest on small shapes;
 // `bench` times the RRDB-shaped tensor-core convs at BASELINE config 2 size (16 x 256 x 256);
 // `trace` (the -DDASR_TC_TRACE build only) prints the per-tile phases of the five dense-block launches.
@@ -25,6 +25,7 @@
   } while (0)
 
 extern "C" int dasr_probe_tma_rate(int row_elems, int rows_per_box, int cs, int store, double* cycles_per_box);
+extern "C" int dasr_probe_wgmma_rate(int n, double* cycles_per_mma);
 static unsigned long long rng_state = 0x1234567ULL;
 static inline unsigned rnd() {
   rng_state = rng_state * 6364136223846793005ULL + 1442695040888963407ULL;
@@ -667,6 +668,21 @@ int main(int argc, char** argv) {
                      store ? "store" : "load ", re * 2, rows, pitch * 2, c, c / rows, re * 2.0 * rows / c, rc);
             }
       return 0;
+    }
+    if (!strcmp(argv[i], "wgmmarate")) {
+      // the ping-pong consumers' MMA stream (m64nNk16, both operands in shared memory) on every SM: what one product costs
+      // at the Cout widths a CTA runs (n32: dense-block launch 5 split by Cout on the pair, n64: split by input channels,
+      // n96: launch 1)
+      double c64 = 0;
+      int rc = dasr_probe_wgmma_rate(64, &c64);
+      for (int n : {32, 64, 96}) {
+        double c = 0;
+        rc |= dasr_probe_wgmma_rate(n, &c);
+        const double fpc = 2.0 * 64 * n * 16 / c;
+        printf("wgmma m64n%dk16 SS: %7.2f cycles/k16 step per SM  %7.1f FLOP/clk/SM  cycles per FLOP vs n64: %5.3f rc=%d\n", n,
+               c, fpc, (c / n) / (c64 / 64), rc);
+      }
+      return rc ? 1 : 0;
     }
     if (!strcmp(argv[i], "trace")) {
 #ifdef DASR_TC_TRACE
