@@ -26,8 +26,9 @@
 // A dasr_conv_tc2 launch whose whole filter set fits one SM and whose grid has many tiles per SM runs one CTA per tile
 // instead (tc2_single).  A pair launch with a 32-channel Cout tile per CTA and an even number of 64-channel A loads splits
 // the pair by input channels instead (tc2_ksplit, KSPLIT): each CTA keeps the filters of its half of the input channels for
-// all 64 output channels, loads its own half of every A tile, runs m64n64k16 over it, and sends the partial sums of the 32
-// channels it does not finish to its peer's shared memory (st.async); each CTA then finishes its 32 channels.
+// all 64 output channels, loads its own half of every A tile, runs m64n64k16 over it, and sends the partial sums of the m64
+// row block it does not finish to its peer's shared memory (st.async); CTA r then finishes row block r (image rows
+// 8r..8r+7 of the tile) for all 64 channels.
 #include <type_traits>
 #include "tc_common.cuh"
 
@@ -65,7 +66,7 @@ struct TcKernelArgs {
   int stages;
   int w_bytes;       // resident filter bytes of one CTA
   int a_stage_bytes; // bytes of one A stage
-  int epi_bytes;     // bytes of ONE staged epilogue tile: 128 pixels x nt channels bf16
+  int epi_bytes;     // bytes of ONE staged epilogue tile: 128 pixels x nt channels bf16 (K-split: 64 pixels x 2 nt)
   int has_pre, has_res1, has_res2;
   int nbuf;          // staged-epilogue tile frames (1..4): pre / residual blocks are requested nbuf tiles ahead
   int pair;          // 1: launched as (1, 2, 1) clusters, A tiles multicast by the leader (rank 0) unless KSPLIT
@@ -261,25 +262,28 @@ __device__ __forceinline__ uint32_t epi_pair(float v0, float v1, float b0, float
 }
 
 // Tile-phase trace (only in the selftest_trace build, compiled with -DDASR_TC_TRACE; the library never records):
-// clock64 stamps of the first TRACE_CTAS CTAs (grid row 0, i.e. the leader of a pair) for their first TRACE_TILES local tiles.
+// clock64 stamps of the first TRACE_CTAS CTAs of grid rows 0 and 1 (the leaders and the followers of the first pairs) for
+// their first TRACE_TILES local tiles; row y's CTAs are trace CTAs y * TRACE_CTAS + x.
 #ifdef DASR_TC_TRACE
-constexpr int TRACE_CTAS = 8, TRACE_TILES = 48, TRACE_EV = 20;
+constexpr int TRACE_CTAS = 8, TRACE_ROWS = 2, TRACE_TILES = 48, TRACE_EV = 24;
 __device__ long long* g_tc_trace;
 #define TC_STAMP(lt, ev)                                                                                           \
   do {                                                                                                             \
     const uint32_t lt_ = (uint32_t)(lt);                                                                           \
-    if (g_tc_trace && blockIdx.x < TRACE_CTAS && blockIdx.y == 0 && lt_ < TRACE_TILES)                             \
-      g_tc_trace[((size_t)blockIdx.x * TRACE_TILES + lt_) * TRACE_EV + (ev)] = clock64();                          \
+    if (g_tc_trace && blockIdx.x < TRACE_CTAS && blockIdx.y < TRACE_ROWS && lt_ < TRACE_TILES)                     \
+      g_tc_trace[((size_t)(blockIdx.y * TRACE_CTAS + blockIdx.x) * TRACE_TILES + lt_) * TRACE_EV + (ev)] = clock64(); \
   } while (0)
 #else
 #define TC_STAMP(lt, ev) do { } while (0)
 #endif
-// event slots of one tile: consumer warpgroup g (warp 4g, lane 0) at 5g + {0: first A wait begins, 1: last A wait ends,
-// 2: MMAs retired, 3: pre / sfree wait ends, 4: epilogue done}; producer: 15 empty wait of the first load begins,
-// 10: it ends, 11: last A load issued; epilogue TMA warp: 12 sfull wait ends, 13 stores issued, 14 stores have read the tile;
-// ping-pong consumer warpgroup g: 16 + 2g staged block 0 written, 17 + 2g the slots of block 1 ready.
+// event slots of one tile: consumer warpgroup g (warp 4g, lane 0) at 5g + {0: first A wait begins, 1: last A wait ends
+// (the MMAs of the last load are issued from here), 2: MMAs retired, 3: pre / sfree wait ends, 4: epilogue done};
+// producer: 15 empty wait of the first load begins, 10: it ends, 11: last A load issued; epilogue TMA warp: 12 sfull wait
+// ends, 13 stores issued, 14 stores have read the tile; ping-pong consumer warpgroup g: 16 + 2g staged block 0 written,
+// 17 + 2g the slots of block 1 ready; K-split consumer warpgroup g: 20 + 2g xfree wait ends (the peer has read the
+// previous partial sums), 21 + 2g xfull wait ends (the peer's partial sums have landed).
 enum { TEV_P_EMPTY = 10, TEV_P_ISSUED = 11, TEV_E_SFULL = 12, TEV_E_STORED = 13, TEV_E_READ = 14, TEV_P_EMPTY0 = 15,
-       TEV_C_BLK0 = 16, TEV_C_BLK1_READY = 17 };
+       TEV_C_BLK0 = 16, TEV_C_BLK1_READY = 17, TEV_X_FREE = 20, TEV_X_FULL = 21 };
 
 // EPI_MODE / HAS_PRE / NRES are compile-time so that each instantiation carries only its own epilogue code.
 // MAP (staged epilogue only): 0 = no weight map; DASR_MAP_CHANNEL = one more input channel map_scale * map convolved with
@@ -292,8 +296,10 @@ enum { TEV_P_EMPTY = 10, TEV_P_ISSUED = 11, TEV_E_SFULL = 12, TEV_E_STORED = 13,
 // 2H x 2W tensor.  Only the bias index (the bias stays in the conv's channel order) and the epilogue TMA warp's choice of
 // map and column differ from a plain conv.
 // KSPLIT (pair, ping-pong, 64-channel loads issued half-major): the pair splits the input channels, not the Cout tile.
-// NT is still the Cout tile a CTA finishes; its MMAs are 2 NT wide (the pair's whole Cout tile) over half of the input
-// channels, and the other NT channels' partial sums go to the peer, which adds them to its own: S(K half 0) + S(K half 1).
+// NT is still the Cout tile of one CTA (half the pair's); its MMAs are 2 NT wide (the pair's whole Cout tile) over half of
+// the input channels.  CTA r finishes m64 row block r for all 2 NT channels: the partial sums of the other block go to the
+// peer, which adds them to its own, S(K half 0) + S(K half 1), and the staged epilogue runs on one 64-pixel x 64-channel
+// block (8-row TMA boxes of 128-byte rows).
 template <int EPI_MODE, bool HAS_PRE, int NRES, int MAP = 0, int NT = 0, int NTAPS = 9, bool PS = false, bool KSPLIT = false>
 __global__ void __launch_bounds__(TCK_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ CUtensorMap tmap_w,
@@ -330,12 +336,15 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
   const int ntile = blockIdx.y - var * a.n_ntiles;
   const int nt = p.nt;
   const int ntaps = p.ntaps;
-  const int nb64 = nt >> 6;
-  const bool tail32 = (nt & 32) != 0, tail16 = (nt & 16) != 0;
+  // staged blocks of a tile; K-split: one 64-channel block of 64 pixels (the CTA's m64 row block, see KSPLIT above)
+  const int nb64 = KSPLIT ? 1 : nt >> 6;
+  const bool tail32 = !KSPLIT && (nt & 32) != 0, tail16 = !KSPLIT && (nt & 16) != 0;
   const int nblocks = nb64 + (tail32 ? 1 : 0) + (tail16 ? 1 : 0);
   const bool has_loads = (EPI_MODE == 0) && (HAS_PRE || NRES > 0);
   const bool pair = a.pair != 0;
   const uint32_t rank = pair ? cluster_ctarank() : 0u;
+  // first output channel (before out_coff) of the channels this CTA finishes: its Cout tile, or the pair's (K-split)
+  auto cb_tile = [&] { return (KSPLIT ? ntile - (int)rank : ntile) * nt; };
   const uint32_t a_row = a.chunk64 ? 2u * ROW_B : (uint32_t)ROW_B;    // bytes per pixel row of an A tile
   static_assert(NT == 0 || (EPI_MODE == 0 && MAP == 0 && NT % 16 == 0 && NT <= 96), "ping-pong: staged epilogue, N <= 96");
   static_assert(!KSPLIT || (NT == 32 && NTAPS == 9 && !PS), "K-split: 32 channels finished per CTA, plain 3x3 taps");
@@ -367,8 +376,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
       sTap[t] = (p.a_mode == 0) ? (uint32_t)(p.tap_dy[var][tt] * HALO_W + p.tap_dx[var][tt]) * a_row : (uint32_t)(tt * A_TAP_BYTES);
     }
   }
-  for (int i = threadIdx.x; i < nt; i += TCK_THREADS) {
-    int bi = ntile * nt + i;
+  for (int i = threadIdx.x; i < (KSPLIT ? 2 * nt : nt); i += TCK_THREADS) {
+    int bi = cb_tile() + i;
     if constexpr (PS) bi = (bi % (p.cout >> 2)) * 4 + bi / (p.cout >> 2);   // packed row b * cout / 4 + c: conv channel 4c + b
     sBias[i] = a.bias ? a.bias[bi] : 0.f;
   }
@@ -448,7 +457,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
     // warpgroup has written it and its slots return (next pre / residual loads, or sfree) as soon as that store has read
     // them; the other frames have one barrier per tile.
     if constexpr (EPI_MODE == 0) {
-      int par = var, cb_out = ntile * nt;
+      int par = var, cb_out = cb_tile();
+      const int ry = KSPLIT ? 8 * (int)rank : 0;              // K-split: the image rows of this CTA's m64 row block
       if constexpr (PS) {                                   // n_ntiles / 4 Cout tiles per parity, parity-major
         const int tpp = a.n_ntiles >> 2;
         par = ntile / tpp;
@@ -464,17 +474,17 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
         int x0, y0, n;
         tile_xyz(tile, x0, y0, n);
         if (lane == 0) {
-          const int cb = ntile * nt;
+          const int cb = cb_tile();
           for (int i = i0; i < i1; i++) {
             int col, off, k;
             staged_block(i, nb64, tail32, col, off, k);
             uint64_t* bar = &pre_bar[bar_of(f, i)];
-            if (NT > 0) mbar_expect_tx(bar, (uint32_t)(nload * (EPI_BLK64_BYTES >> k)));
+            if (NT > 0) mbar_expect_tx(bar, (uint32_t)(nload * (KSPLIT ? a.epi_bytes : EPI_BLK64_BYTES >> k)));
             else if (i == 0) mbar_expect_tx(bar, (uint32_t)(nload * a.epi_bytes));
             off += f * a.epi_bytes;
-            if constexpr (HAS_PRE) tma_load_4d(sS + off, &em.m[3 + k], bar, p.pre_coff + cb + col, x0, y0, n);
-            if constexpr (NRES >= 1) tma_load_4d(sR1 + off, &em.m[6 + k], bar, p.res1_coff + cb + col, x0, y0, n);
-            if constexpr (NRES >= 2) tma_load_4d(sR2 + off, &em.m[9 + k], bar, p.res2_coff + cb + col, x0, y0, n);
+            if constexpr (HAS_PRE) tma_load_4d(sS + off, &em.m[3 + k], bar, p.pre_coff + cb + col, x0, y0 + ry, n);
+            if constexpr (NRES >= 1) tma_load_4d(sR1 + off, &em.m[6 + k], bar, p.res1_coff + cb + col, x0, y0 + ry, n);
+            if constexpr (NRES >= 2) tma_load_4d(sR2 + off, &em.m[9 + k], bar, p.res2_coff + cb + col, x0, y0 + ry, n);
           }
         }
         __syncwarp();
@@ -512,7 +522,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
             for (int i = i0; i < i1; i++) {
               int col, off, k;
               staged_block(i, nb64, tail32, col, off, k);
-              tma_store_4d(&em.m[k + omap], sS + f * a.epi_bytes + off, co_base + col, x0, y0, n);
+              tma_store_4d(&em.m[k + omap], sS + f * a.epi_bytes + off, co_base + col, x0, y0 + ry, n);
             }
             bulk_commit();
             if (i1 == nblocks) TC_STAMP(it, TEV_E_STORED);
@@ -564,7 +574,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
     const uint32_t b_slot = (uint32_t)((KSPLIT ? 2 : 1) * nt * ROW_B);     // one resident filter chunk: MMA width x 64 B
     // first A row of this warpgroup's 64 pixels: 8 image rows down the halo tile, or 64 rows of a per-tap tile
     const uint32_t wg_off = (EPI_MODE == 3) ? 64u * wg * a_row : (p.a_mode == 0 ? 8u * wg * HALO_W * a_row : 64u * wg * (uint32_t)ROW_B);
-    const int co_base = ntile * nt;
+    const int co_base = cb_tile();
     const int OW = p.W * p.out_mul, OH = p.H * p.out_mul;
     const int act = p.act;
     const float slope = p.slope, alpha = p.alpha;
@@ -670,9 +680,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
       // tile, as in the cooperative path.  Warpgroup (it & 1) starts waiting for the A loads of tile it only after the
       // other warpgroup has seen every load of tile it - 1 land (named barrier 2 + ((it - 1) & 1)): every earlier phase
       // of each A stage has then completed, so a parity wait can never be satisfied by a phase two rounds old.
-      constexpr int NB64 = NT / 64;
-      constexpr bool T32 = (NT & 32) != 0;
-      constexpr int NBLK = NB64 + (T32 ? 1 : 0) + ((NT & 16) ? 1 : 0);
+      constexpr int NB64 = KSPLIT ? 1 : NT / 64;
+      constexpr bool T32 = !KSPLIT && (NT & 32) != 0;
+      constexpr int NBLK = NB64 + (T32 ? 1 : 0) + (!KSPLIT && (NT & 16) ? 1 : 0);
       static_assert(NBLK <= FRAME_BLKS, "ping-pong: one barrier per staged block");
       const uint32_t G = gridDim.x, ntiles = (uint32_t)a.ntiles;   // 32-bit tile arithmetic (checked on the host)
       const uint32_t nl = (uint32_t)a.nloads, ns = (uint32_t)a.stages;
@@ -710,28 +720,30 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
           if (rec) TC_STAMP(it, 5 * wg + 2);
           if constexpr (KSPLIT) {
             // Both CTAs of the pair walk the same tiles with the same warpgroup, so thread t of warpgroup wg holds the same
-            // accumulator fragment in both: its NT partial sums of the peer's channels go to the same thread of the peer,
-            // and the NT of its own channels become S(own K half) + S(peer's K half) in acc[0, NT), the layout of an NT-wide
-            // accumulator.  k = this warpgroup's tile count: the peer's buffer is free once it has read tile k - 1.
+            // accumulator fragment in both: NT fp32 of m64 row block b in acc[b NT, (b + 1) NT).  CTA r finishes block r:
+            // the thread sends its partial sums of block 1 - r to the same thread of the peer, and block r becomes
+            // S(own K half) + S(peer's K half) in acc[0, NT), the fragment of one m64n64 accumulator.  k = this warpgroup's
+            // tile count: the peer's buffer is free once it has read tile k - 1.
             const uint32_t k = it >> 1, peer = rank ^ 1u, t = threadIdx.x & 127;
             const uint32_t xoff = smem_u32(sX) + (uint32_t)wg * XCH_BYTES + 16u * t;
             auto exchange = [&](auto r_c) {
-              constexpr int R = decltype(r_c)::value, HS = NT / 2, NQ = NT / 4;   // acc[b NT + h HS + i]: m64 block b, Cout half h
+              constexpr int R = decltype(r_c)::value, NQ = NT / 4;
               if (k > 0) mbar_wait(&xfree_bar[wg], (k & 1) ^ 1);
+              if (rec) TC_STAMP(it, TEV_X_FREE + 2 * wg);
               const uint32_t dst = mapa_u32(xoff, peer), bar = mapa_u32(smem_u32(&xfull_bar[wg]), peer);
 #pragma unroll
               for (int q = 0; q < NQ; q++) {
-                const float* v = acc + (q / (NQ / 2)) * NT + (1 - R) * HS + 4 * (q % (NQ / 2));
+                const float* v = acc + (1 - R) * NT + 4 * q;
                 st_async_v4(dst + 2048u * q, v[0], v[1], v[2], v[3], bar);
               }
               if (wi == 0 && lane == 0) mbar_expect_tx(&xfull_bar[wg], (uint32_t)XCH_BYTES);
               mbar_wait(&xfull_bar[wg], k & 1);
+              if (rec) TC_STAMP(it, TEV_X_FULL + 2 * wg);
 #pragma unroll
               for (int q = 0; q < NQ; q++) {
-                const int b = q / (NQ / 2), i = 4 * (q % (NQ / 2));
                 const float4 x = lds128f(xoff + 2048u * q);
-                float* o = acc + b * HS + i;
-                const float* s = acc + b * NT + R * HS + i;
+                float* o = acc + 4 * q;
+                const float* s = acc + R * NT + 4 * q;
                 o[0] = s[0] + x.x; o[1] = s[1] + x.y; o[2] = s[2] + x.z; o[3] = s[3] + x.w;
               }
               compiler_fence();
@@ -757,41 +769,49 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
             if (rec && i == 0) TC_STAMP(it, 5 * wg + 3);
             if (rec && i == 1) TC_STAMP(it, TEV_C_BLK1_READY + 2 * wg);
             compiler_fence();
-            // Column groups j of the block in batches of JB: every bias / pre / residual load of a batch, then its math, then
-            // its stores.  Sub-tile (blk = k >> 1, h = k & 1, j) is matrix k of one ldmatrix / stmatrix, so each lane addresses
-            // row lm of the warpgroup's tile.  pre is read and overwritten in place in sS, but each element only by the lane
-            // that holds it, and its store depends on the value loaded, so no other ordering is needed.
+            // One ldmatrix / stmatrix step covers GS column groups from j: matrix k is sub-tile (blk = k >> 1, h = k & 1,
+            // group j) of the warpgroup's two m64 blocks, or on the K-split (one m64 block) sub-tile (h = k & 1, group
+            // j + (k >> 1)); each lane addresses row lm of the staged block, in column group j + jo.  Steps run in batches of
+            // JB: every bias / pre / residual load of a batch, then its math, then its stores.  pre is read and overwritten in
+            // place in sS, but each element only by the lane that holds it, and its store depends on the value loaded, so no
+            // other ordering is needed.
             auto body = [&](auto mask_c) {
               constexpr bool MASK = decltype(mask_c)::value;
-              constexpr int NLD = (HAS_PRE ? 1 : 0) + NRES, JBLK = (c1 - c0) / 8;
-              constexpr int JREGS = 4 * NLD + 2;                              // registers loaded per column group
-              constexpr int JB = JBLK * JREGS <= 32 ? JBLK : (JBLK * JREGS <= 64 ? JBLK / 2 : 2);   // <= 32 per batch
-              const int lm = 64 * (lane >> 4) + 16 * wi + 8 * ((lane >> 3) & 1) + (lane & 7);
+              constexpr int GS = KSPLIT ? 2 : 1;
+              constexpr int NLD = (HAS_PRE ? 1 : 0) + NRES, JSTEPS = (c1 - c0) / 8 / GS;
+              constexpr int JREGS = 4 * NLD + 2 * GS;                         // registers loaded per step
+              constexpr int JB = JSTEPS * JREGS <= 32 ? JSTEPS : (JSTEPS * JREGS <= 64 ? JSTEPS / 2 : 2);   // <= 32 per batch
+              const int lm = (KSPLIT ? 0 : 64 * (lane >> 4)) + 16 * wi + 8 * ((lane >> 3) & 1) + (lane & 7);
+              const int jo = KSPLIT ? lane >> 4 : 0;
               const EpiConst ek = epi_const(p, has_bias, mask_mode, co_base + cq);
 #pragma unroll
-              for (int jb = c0 / 8; jb < c1 / 8; jb += JB) {
+              for (int jb = c0 / 8; jb < c1 / 8; jb += JB * GS) {
                 uint32_t qp[JB][4] = {}, q1[JB][4] = {}, q2[JB][4] = {}, r[JB][4];
-                float2 b[JB];
+                float2 b[JB][GS];
 #pragma unroll
                 for (int jj = 0; jj < JB; jj++) {
-                  const uint32_t o = staged_off(lm, 8 * (jb + jj), NB64, T32);
-                  b[jj] = lds64f(sBias_u + 4u * (uint32_t)(8 * (jb + jj) + cq));
+                  const int j = jb + jj * GS;
+                  const uint32_t o = staged_off(lm, 8 * (j + jo), NB64, T32);
+#pragma unroll
+                  for (int g = 0; g < GS; g++) b[jj][g] = lds64f(sBias_u + 4u * (uint32_t)(8 * (j + g) + cq));
                   if constexpr (HAS_PRE) ldsm4(bS + o, qp[jj]);
                   if constexpr (NRES >= 1) ldsm4(bR1 + o, q1[jj]);
                   if constexpr (NRES >= 2) ldsm4(bR2 + o, q2[jj]);
                 }
 #pragma unroll
                 for (int jj = 0; jj < JB; jj++) {
-                  const int j = jb + jj;
+                  const int j = jb + jj * GS;
 #pragma unroll
                   for (int k = 0; k < 4; k++) {
-                    const float* v = acc + (k >> 1) * (NT / 2) + 4 * j + 2 * (k & 1);
-                    r[jj][k] = epi_pair<HAS_PRE, NRES, MASK, false>(v[0], v[1], b[jj].x, b[jj].y, qp[jj][k], q1[jj][k], q2[jj][k], 1.f,
-                                                                    ek.act(j), ek.mask(j), ek, F16);
+                    const int jk = KSPLIT ? j + (k >> 1) : j;                   // the sub-tile's column group
+                    const float* v = acc + (KSPLIT ? 0 : (k >> 1) * (NT / 2)) + 4 * jk + 2 * (k & 1);
+                    const float2 bb = b[jj][KSPLIT ? k >> 1 : 0];
+                    r[jj][k] = epi_pair<HAS_PRE, NRES, MASK, false>(v[0], v[1], bb.x, bb.y, qp[jj][k], q1[jj][k], q2[jj][k], 1.f,
+                                                                    ek.act(jk), ek.mask(jk), ek, F16);
                   }
                 }
 #pragma unroll
-                for (int jj = 0; jj < JB; jj++) stsm4(bS + staged_off(lm, 8 * (jb + jj), NB64, T32), r[jj]);
+                for (int jj = 0; jj < JB; jj++) stsm4(bS + staged_off(lm, 8 * (jb + jj * GS + jo), NB64, T32), r[jj]);
               }
             };
             if (NRES >= 1 && mask_mode) body(std::true_type());
@@ -1277,11 +1297,12 @@ int dasr_pack_filter_tc_batch(const DasrPackJob* jobs_dev, int njobs, int blocks
 // mul = 1: the [N, H, W, cs] tensor at `base`.  mul = 2: the sub-pixel view out[n, 2y + py, 2x + px, c] of a [N, 2H, 2W, cs]
 // tensor (the caller offsets `base` to pixel (py, px)): same W x H index space as the input tiles, doubled pixel strides —
 // the four parity variants of the fused nearest-x2 conv store their tiles through TMA like any other layer.
+// rows: image rows per box (a whole tile, or the 8 of one m64 row block on the K-split).
 static int encode_act_map(PFN_encodeTiled enc, CUtensorMap* tm, const void* base, int cs, int W, int H, int N,
-                          int width, const char* what, int mul = 1) {
+                          int width, const char* what, int mul = 1, int rows = TILE_H) {
   cuuint64_t gdim[4] = {(cuuint64_t)cs, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
   cuuint64_t gstr[3] = {(cuuint64_t)mul * cs * 2, (cuuint64_t)mul * (mul * W) * cs * 2, (cuuint64_t)(mul * H) * (mul * W) * cs * 2};
-  cuuint32_t box[4] = {(cuuint32_t)width, TILE_W, TILE_H, 1};
+  cuuint32_t box[4] = {(cuuint32_t)width, TILE_W, (cuuint32_t)rows, 1};
   cuuint32_t estr[4] = {1, 1, 1, 1};
   const CUtensorMapSwizzle sw = width == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : (width == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
   CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), gdim, gstr, box, estr,
@@ -1342,6 +1363,21 @@ static bool chunk_list_pairs64(const DasrConvTcParams* p) {
 // K-split exchange buffers: 128 pixels x nt fp32 partial sums per consumer warpgroup, and four barriers
 constexpr int XCH_BAR_BYTES = 4 * 8;
 static int tc2_xch_bytes(int nt) { return 2 * 128 * nt * 4 + XCH_BAR_BYTES; }
+// K-split A stage: the 180 rows of one 64-channel halo tile (no taps-in-N reads past them), rounded up to the 1 KB of a
+// SWIZZLE_128B pattern
+constexpr int KSPLIT_A_STAGE_BYTES = (HALO_W * HALO_H * 2 * ROW_B + 1023) / 1024 * 1024;
+
+// Shared-memory plan of a K-split launch (nt: the Cout tile of one CTA, half the pair's): the filters of half the input
+// channels for the pair's Cout tile, the exchange buffers, two staging frames, then as many A stages as fit.  Measured on
+// launch 5 (DESIGN §6), a third A stage gains more than a third or fourth frame.  Returns the number of A stages (< 2:
+// does not fit).
+static int tc2_ksplit_plan(const DasrConvTcParams* p, int nt, int nres, int* nbuf) {
+  *nbuf = 2;
+  const int avail = SMEM_LIMIT - 1024 /*alignment slack*/ - 9 * (p->cin / CHUNK) * nt * ROW_B - *nbuf * nt * 128 * 2 * (1 + nres) -
+                    tc2_xch_bytes(nt) - TC_BAR_BYTES;
+  const int stages = avail > 0 ? avail / KSPLIT_A_STAGE_BYTES : 0;
+  return stages > MAX_STAGES ? MAX_STAGES : stages;
+}
 
 // pair = 1: (1, 2, 1) clusters, p->nt is the Cout tile of ONE CTA (half of the pair's tile).
 // order32: every output element sums its products in the order of 32-channel A loads (dasr_conv_tc2's launches, on the
@@ -1447,11 +1483,11 @@ static int conv_tc_launch(const void* in, const void* w, const float* bias, cons
   if (ksplit) {
     a.chunk64 = 2;
     a.xch_bytes = tc2_xch_bytes(p->nt);
-    stages = tc_plan(a.w_bytes, (int)a_stage_bytes_for(p, 1), a.epi_bytes, a.has_res1 + a.has_res2, 0, &nbuf, a.xch_bytes);
+    stages = tc2_ksplit_plan(p, p->nt, a.has_res1 + a.has_res2, &nbuf);
     DASR_REQUIRE(pp == 1 && psi < 0 && nbuf >= 2 && stages >= 2, "conv_tc2: K-split plan (nt=%d cin=%d)", p->nt, p->cin);
   }
   a.nloads = a.chunk64 ? a.nchunks / (ksplit ? 4 : 2) : a.nchunks;
-  a.a_stage_bytes = (int)a_stage_bytes_for(p, a.chunk64);
+  a.a_stage_bytes = ksplit ? KSPLIT_A_STAGE_BYTES : (int)a_stage_bytes_for(p, a.chunk64);
   a.nbuf = nbuf;
   a.stages = stages;
   const int epi_total = nbuf * a.epi_bytes * (1 + a.has_res1 + a.has_res2);
@@ -1507,7 +1543,9 @@ static int conv_tc_launch(const void* in, const void* w, const float* bias, cons
     } else {
       for (int t = 0; t < 4; t++) {
         if (!used[t]) continue;
-        int rc = encode_staged_maps(enc, &em.m[3 * t], bases[t], css[t], p->nt, p->W, p->H, p->N, names[t]);
+        // K-split: each CTA moves one m64 row block of the pair's 64 channels, 8 x 8 pixels x 128 B boxes
+        int rc = ksplit ? encode_act_map(enc, &em.m[3 * t], bases[t], css[t], p->W, p->H, p->N, 64, names[t], 1, TILE_H / 2)
+                        : encode_staged_maps(enc, &em.m[3 * t], bases[t], css[t], p->nt, p->W, p->H, p->N, names[t]);
         if (rc) return rc;
       }
     }
@@ -1710,8 +1748,7 @@ static bool tc2_ksplit(const DasrConvTcParams* p, int nres, const float* map) {
   const int nchunks = p->cin / CHUNK;
   if (p->nchunk_list ? !(chunk_list_pairs64(p) && p->nchunk_list % 4 == 0) : nchunks % 4 != 0) return false;
   int nbuf;
-  const int stages = tc_plan(9 * nchunks * (p->nt / 2) * ROW_B, (int)a_stage_bytes_for(p, 1), (p->nt / 2) * 128 * 2, nres, 0,
-                             &nbuf, tc2_xch_bytes(p->nt / 2));
+  const int stages = tc2_ksplit_plan(p, p->nt / 2, nres, &nbuf);
   return nbuf >= 2 && stages >= 2 * (nchunks / 4);
 }
 
@@ -1782,7 +1819,7 @@ int dasr_conv_tc2_map(const void* in, const void* w, const float* bias, const vo
 // traced selftest build only: where the tile-phase stamps go (nullptr: none) and which consumer schedule to launch
 int dasr_tc_trace_attach(long long* buf, int coop, int* ctas, int* tiles, int* events) {
   g_trace_coop = coop;
-  *ctas = TRACE_CTAS;
+  *ctas = TRACE_ROWS * TRACE_CTAS;
   *tiles = TRACE_TILES;
   *events = TRACE_EV;
   return cudaMemcpyToSymbol(g_tc_trace, &buf, sizeof(buf)) == cudaSuccess ? DASR_OK : DASR_E_LAUNCH;

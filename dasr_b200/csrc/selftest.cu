@@ -558,10 +558,11 @@ static void trace_rdb(int coop) {
   const Launch ls[5] = {{64, 192, 64, {}, -1, 1, 0},       {32, 32, 96, {64}, 96, 0, 0},
                         {64, 64, 128, {64, 96}, 128, 1, 0}, {32, 32, 160, {128}, 160, 0, 0},
                         {128, 64, 0, {64, 96, 128, 160}, 192, 1, 1}};
-  printf("trace (%s consumers): median per tile, us; first %d CTAs (leader of each pair), tiles 2..%d\n",
-         coop ? "cooperative" : "ping-pong", ctas, tiles - 1);
-  printf("launch  K   N  us/launch us/tile | A-wait  MMA  epi-in-wait epilogue busy  period | prod: empty-wait issue-gap | "
-         "epi-TMA: sfull-lag store-issue read | ping-pong blocks: blk0-math blk1-wait blk1-math\n");
+  printf("trace (%s consumers): median per tile, us; first %d CTAs of each pair rank (r0 leaders, r1 followers), tiles "
+         "2..%d\n", coop ? "cooperative" : "ping-pong", ctas / 2, tiles - 1);
+  printf("launch     K   N  us/launch us/tile | A-wait  MMA  epi-in-wait epilogue busy  period | prod: empty-wait issue-gap | "
+         "epi-TMA: sfull-lag store-issue read | ping-pong blocks: blk0-math blk1-wait blk1-math | K-split: xfree xfull pre "
+         "| MMA-overlap\n");
   for (int li = 0; li < 5; li++) {
     const Launch& L = ls[li];
     std::vector<float> w((size_t)L.cout * L.cin * 9);
@@ -612,37 +613,54 @@ static void trace_rdb(int coop) {
     dasr_tc_trace_attach(nullptr, coop, &ctas, &tiles, &nev);
     std::vector<long long> tr((size_t)ctas * tiles * nev);
     CK(cudaMemcpy(tr.data(), dtr, tr.size() * 8, cudaMemcpyDeviceToHost));
-    std::vector<double> ph[14];
-    for (int c = 0; c < ctas; c++) {
-      auto ev = [&](int t, int e) { return tr[((size_t)c * tiles + t) * nev + e]; };
-      auto cons = [&](int t, int e) { return ev(t, 4) ? ev(t, e) : ev(t, 5 + e); };   // whichever warpgroup ran tile t
-      for (int t = 2; t < tiles; t++) {
-        if (!cons(t, 4) || !cons(t - 1, 4) || !ev(t, 11)) continue;
-        const double v[11] = {(double)(cons(t, 1) - cons(t, 0)), (double)(cons(t, 2) - cons(t, 1)),
-                              (double)(cons(t, 3) - cons(t, 2)), (double)(cons(t, 4) - cons(t, 3)),
-                              (double)(cons(t, 4) - cons(t, 0)), (double)(cons(t, 4) - cons(t - 1, 4)),
-                              (double)(ev(t, 10) - ev(t, 15)),   (double)(ev(t, 11) - ev(t - 1, 11)),
-                              (double)(ev(t, 12) - cons(t, 4)),  (double)(ev(t, 13) - ev(t, 12)),
-                              (double)(ev(t, 14) - ev(t, 13))};
-        for (int k = 0; k < 11; k++) ph[k].push_back(v[k] / cyc_per_us);
-        // ping-pong staged blocks (events 16 + 2g: block 0 written, 17 + 2g: block 1's slots ready; g = the warpgroup)
-        const int g = ev(t, 4) ? 0 : 1;
-        const long long b0 = ev(t, 16 + 2 * g), b1 = ev(t, 17 + 2 * g);
-        if (b0) ph[11].push_back((b0 - cons(t, 3)) / cyc_per_us);
-        if (b0 && b1) {
-          ph[12].push_back((b1 - b0) / cyc_per_us);
-          ph[13].push_back((cons(t, 4) - b1) / cyc_per_us);
-        }
-      }
-    }
     int sms = 0;
     CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0));
     const double tiles_per_cta = (double)N * (H / 16) * (W / 8) / (sms / 2);
-    printf("  %d   %3d %3d  %8.1f %6.2f  | %6.2f %5.2f %6.2f %9.2f %6.2f %6.2f | %6.2f %9.2f          | %6.2f %9.2f %6.2f |"
-           " %9.2f %9.2f %9.2f\n",
-           li + 1, L.cin, L.cout, ms * 1e3, ms * 1e3 / tiles_per_cta, median(ph[0]), median(ph[1]), median(ph[2]),
-           median(ph[3]), median(ph[4]), median(ph[5]), median(ph[6]), median(ph[7]), median(ph[8]), median(ph[9]),
-           median(ph[10]), median(ph[11]), median(ph[12]), median(ph[13]));
+    // one row per rank of the pair: trace CTAs [r * ctas / 2, (r + 1) * ctas / 2) are grid row r (no row 1: one CTA per tile)
+    for (int rank = 0; rank < 2; rank++) {
+      std::vector<double> ph[18];
+      for (int c = rank * ctas / 2; c < (rank + 1) * ctas / 2; c++) {
+        auto ev = [&](int t, int e) { return tr[((size_t)c * tiles + t) * nev + e]; };
+        auto wg_of = [&](int t) { return ev(t, 4) ? 0 : 1; };                         // whichever warpgroup ran tile t
+        auto cons = [&](int t, int e) { return ev(t, 5 * wg_of(t) + e); };
+        for (int t = 2; t < tiles; t++) {
+          if (!cons(t, 4) || !cons(t - 1, 4) || !ev(t, 11)) continue;
+          const double v[11] = {(double)(cons(t, 1) - cons(t, 0)), (double)(cons(t, 2) - cons(t, 1)),
+                                (double)(cons(t, 3) - cons(t, 2)), (double)(cons(t, 4) - cons(t, 3)),
+                                (double)(cons(t, 4) - cons(t, 0)), (double)(cons(t, 4) - cons(t - 1, 4)),
+                                (double)(ev(t, 10) - ev(t, 15)),   (double)(ev(t, 11) - ev(t - 1, 11)),
+                                (double)(ev(t, 12) - cons(t, 4)),  (double)(ev(t, 13) - ev(t, 12)),
+                                (double)(ev(t, 14) - ev(t, 13))};
+          for (int k = 0; k < 11; k++) ph[k].push_back(v[k] / cyc_per_us);
+          // ping-pong staged blocks (events 16 + 2g: block 0 written, 17 + 2g: block 1's slots ready; g = the warpgroup)
+          const int g = wg_of(t);
+          const long long b0 = ev(t, 16 + 2 * g), b1 = ev(t, 17 + 2 * g);
+          if (b0) ph[11].push_back((b0 - cons(t, 3)) / cyc_per_us);
+          if (b0 && b1) {
+            ph[12].push_back((b1 - b0) / cyc_per_us);
+            ph[13].push_back((cons(t, 4) - b1) / cyc_per_us);
+          }
+          // K-split: the wait for the peer to free the exchange buffer, for the peer's partial sums (including this
+          // warpgroup's own st.async issue), then for the pre / residual tiles
+          const long long xf = ev(t, 20 + 2 * g), xl = ev(t, 21 + 2 * g);
+          if (xf && xl) {
+            ph[14].push_back((xf - cons(t, 2)) / cyc_per_us);
+            ph[15].push_back((xl - xf) / cyc_per_us);
+            ph[16].push_back((cons(t, 3) - xl) / cyc_per_us);
+          }
+          // MMA phases (last A wait ends .. MMAs retired) of tiles t - 1 and t, which the two warpgroups run: their overlap
+          const long long s0 = cons(t - 1, 1), e0 = cons(t - 1, 2), s1 = cons(t, 1), e1 = cons(t, 2);
+          ph[17].push_back(std::max(0LL, std::min(e0, e1) - std::max(s0, s1)) / cyc_per_us);
+        }
+      }
+      if (ph[0].empty()) continue;
+      printf("  %d r%d %3d %3d  %8.1f %6.2f  | %6.2f %5.2f %6.2f %9.2f %6.2f %6.2f | %6.2f %9.2f          | %6.2f %9.2f %6.2f |"
+             " %9.2f %9.2f %9.2f | %6.2f %6.2f %6.2f %6.2f\n",
+             li + 1, rank, L.cin, L.cout, ms * 1e3, ms * 1e3 / tiles_per_cta, median(ph[0]), median(ph[1]), median(ph[2]),
+             median(ph[3]), median(ph[4]), median(ph[5]), median(ph[6]), median(ph[7]), median(ph[8]), median(ph[9]),
+             median(ph[10]), median(ph[11]), median(ph[12]), median(ph[13]), median(ph[14]), median(ph[15]), median(ph[16]),
+             median(ph[17]));
+    }
     cudaFree(dw); cudaFree(dwp); cudaFree(bias);
   }
   cudaFree(dtr); cudaFree(b); cudaFree(dst); cudaFree(rin);
